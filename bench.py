@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py — features+matches/sec of the B200 point/line front-end (BASELINE.json metric).
+"""bench.py — features+matches/sec of the H100 point/line front-end (BASELINE.json metric).
 
 A "step" is one pass of the hot path over one batch of synthetic frames on every GPU:
 ORB extraction (+ line extraction when built) of the rank's frames, vocabulary-node assignment and
@@ -11,12 +11,15 @@ SearchByBoW matching of every consecutive frame pair, and one NCCL all-gather of
 
 `value`  : whole-job (features+matches)/s with the frames already resident in HBM (CUDA events, max over ranks)
 `e2e`    : same metric through the host-buffer API: pinned-host frames H2D, results D2H, every step
-`roofline`: dominant kernel's algorithmic bytes / CUDA-event duration vs MEASURED_PEAKS.json hbm_gbs
+`roofline`: dominant kernel's algorithmic bytes / CUDA-event duration vs the H100 SXM's 3.35 TB/s of HBM3 (or MEASURED_PEAKS.json hbm_gbs)
 `cpu_baseline`: the same step on the host cores with the CPU oracle (port of the reference CPU path)
 --impl reference : times the CPU oracle (the reference's OpenCV build is not compilable here, DESIGN.md) on
                    the same config/metric, all host threads.
+--dump-outputs DIR: after the timed steps, what the last timed step computed (keypoints, descriptors, lines, match tables of a
+                   fixed, seeded sample of its frames) as DIR/<name>.npy, so that two builds can be compared output for output.
 """
 import argparse
+import gc
 import json
 import os
 import subprocess
@@ -25,7 +28,7 @@ import threading
 import time
 
 # The loops below keep ~30 CUDA streams busy (ten frame / line handles with two streams each, matchers, the gather's stream).  With the
-# default of 8 hardware connections streams share queues and falsely serialise (measured: end-to-end step 28.3 ms at 8, 25.8-26.1 ms at 32).
+# default of 8 hardware connections streams share queues and falsely serialise.
 # Must be set before the CUDA context exists.
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 
@@ -45,6 +48,7 @@ WORKLOADS = {
     "single1280": dict(width=1280, height=960, nfeatures=4000, frames_per_gpu=16, nlines=500),
 }
 NWORDS, NNRATIO = 100, 0.7
+RING_DEFAULT = 6
 
 
 def host_cores():
@@ -85,7 +89,7 @@ def make_config(args, cfg, world, lines=True, ring=None, nsets=None, B=None):
 
 
 def gen_frames(cfg, rank, nsets, B=None):
-    """nsets distinct input batches (so that the inputs cycle through more than the 126 MB L2)."""
+    """nsets distinct input batches (so that the inputs cycle through more than the 50 MB L2)."""
     import synth
     B = B or cfg["frames_per_gpu"] + 1
     sets = []
@@ -254,6 +258,48 @@ class ClockSampler:
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": sorted(reasons)}
 
 
+DUMP_FRAMES = 32          # frames of the last step written by --dump-outputs (a fixed, seeded sample: the whole batch would be ~200 MB)
+
+
+def dump_outputs(out_dir, pkg, ext, lseg, d_match, d_nmatch, d_lmatch, d_nlmatch, B, Bf, download):
+    """What a caller of the device-resident path receives after the last timed step, as <out_dir>/<name>.npy: per-frame counts of
+    every frame, and keypoints, descriptors, keylines, LBD descriptors, line equations and the point / line match tables of a fixed
+    sample of frames.  Entries past a frame's count are not results (the buffers keep older contents there): they are written as 0,
+    and -1 in the match tables.  Row p of a match table belongs to the pair (p, p + 1) and is indexed by frame p + 1's features."""
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    frames = np.sort(np.random.default_rng(0).choice(Bf, size=min(Bf, DUMP_FRAMES), replace=False))
+    out = {}
+    kps, desc, n, cap = ext.device_results()
+    n = download(n, (B,), "<i4")
+    keep = np.arange(cap)[None, :] < n[frames, None]
+    k = download(kps, (B, cap * pkg.KEYPOINT_DTYPE.itemsize), "|u1").view(pkg.KEYPOINT_DTYPE)[frames]
+    for f in pkg.KEYPOINT_DTYPE.names:
+        out[f"keypoint_{f}"] = np.where(keep, k[f], 0).astype(np.float32)
+    out["descriptors"] = np.where(keep[..., None], download(desc, (B, cap, 32), "|u1")[frames], 0).astype(np.float32)
+    out["n_keypoints"] = n.astype(np.float32)
+    m = d_match.cpu().numpy()
+    out["point_matches"] = np.where(np.arange(m.shape[1])[None, :] < n[frames + 1, None], m[frames], -1).astype(np.float32)   # row p: frame p+1's features
+    out["n_point_matches"] = d_nmatch.cpu().numpy().astype(np.float32)
+    if lseg is not None:
+        kl, ld, eq, nl, capl = lseg.device_results()
+        nl = download(nl, (B,), "<i4")
+        keep = np.arange(capl)[None, :] < nl[frames, None]
+        k = download(kl, (B, capl * pkg.KEYLINE_DTYPE.itemsize), "|u1").view(pkg.KEYLINE_DTYPE)[frames]
+        for f in pkg.KEYLINE_DTYPE.names:
+            out[f"keyline_{f}"] = np.where(keep, k[f], 0).astype(np.float32)
+        out["line_descriptors"] = np.where(keep[..., None], download(ld, (B, capl, 32), "|u1")[frames], 0).astype(np.float32)
+        out["line_equations"] = np.where(keep[..., None], download(eq, (B, capl, 3), "<f8")[frames], 0).astype(np.float64)
+        out["n_lines"] = nl.astype(np.float32)
+        lm = d_lmatch.cpu().numpy()
+        out["line_matches"] = np.where(np.arange(lm.shape[1])[None, :] < nl[frames + 1, None], lm[frames], -1).astype(np.float32)
+        out["n_line_matches"] = d_nlmatch.cpu().numpy().astype(np.float32)
+    out["sampled_frames"] = frames.astype(np.float32)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def main():
     if len(sys.argv) > 1 and sys.argv[1] == "--cv2-worker":
         return cv2_worker_main(sys.argv[2:])
@@ -267,7 +313,10 @@ def main():
                     help="weak: frames_per_gpu frames on every GPU; strong: BASELINE.json config 5 as written, the workload's frames in total, sharded")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-lines", action="store_true", help="ORB + point matching only")
-    ap.add_argument("--line-ring", type=int, default=10, help="line / frame handles (streams + workspaces) kept in flight (measured: 10 gives the shortest step, device-resident and end to end; 6, 8, 12, 14 are 1-2 ms slower)")
+    ap.add_argument("--line-ring", type=int, default=RING_DEFAULT, help="line / frame handles (streams + workspaces) kept in flight; "
+                    "each end-to-end frame handle of the batch640 workload holds 10.4 GB, so an 80 GB H100 fits at most 7; "
+                    "the default of 6 leaves memory headroom (7 measured slightly faster device-resident)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed as DIR/<name>.npy (float32 / float64)")
     ap.add_argument("--walkers-per-sm", type=float, default=0.0, help="per line handle: resident LSD region walkers per SM (0 = one per frame)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
@@ -324,7 +373,7 @@ def main():
     cap = ext.cap
     voc = synth.vocabulary(NWORDS)
     d_voc = torch.from_numpy(voc).to(dev)
-    nsets = max(2, int(np.ceil(160e6 / (B * W * H))))   # cycle > 126 MB of distinct inputs => inputs never L2-resident
+    nsets = max(2, int(np.ceil(160e6 / (B * W * H))))   # cycle > 160 MB of distinct inputs (L2: 50 MB) => inputs never L2-resident
     sets = gen_frames(cfg, rank, nsets, B)
     d_sets = [torch.from_numpy(s).to(dev) for s in sets]
     d_match = torch.empty((Bf, cap), dtype=torch.int32, device=dev)
@@ -333,9 +382,9 @@ def main():
     d_nlmatch = [torch.zeros((Bf,), dtype=torch.int32, device=dev) for _ in range(R)]
     d_gather = torch.empty((world * Bf, cap), dtype=torch.int32, device=dev) if world > 1 else None
     d_lgather = torch.empty((world * Bf, NL), dtype=torch.int32, device=dev) if world > 1 else None
-    class _DevArr:                                      # a torch view of a device array owned by the library (counts only)
-        def __init__(self, ptr, n):
-            self.__cuda_array_interface__ = {"shape": (n,), "typestr": "<i4", "data": (ptr, False), "version": 2}
+    class _DevArr:                                      # a torch view of a device array owned by the library
+        def __init__(self, ptr, n, typestr="<i4"):
+            self.__cuda_array_interface__ = {"shape": n if isinstance(n, tuple) else (n,), "typestr": typestr, "data": (ptr, False), "version": 2}
     _views = {}
     def dev_i32(ptr, n):                                # (the result arrays exist after the handle's first call: looked up per step, cached)
         if (ptr, n) not in _views:
@@ -441,6 +490,11 @@ def main():
     launches = launches_now() - launches0
     clocks = sampler.stop() if rank == 0 else None
     units_timed = int(u_pts.item()) + sum(int(u.item()) for u in u_lin)      # counted inside the timed region, on the device
+    if args.dump_outputs and rank == 0:                 # the last timed step's lines are in ring slot r
+        r = (args.warmup + args.steps - 1) % R if LINES else None
+        dump_outputs(args.dump_outputs, pkg, ext, lsr[r] if LINES else None, d_match, d_nmatch, d_lmatch[r] if LINES else None,
+                     d_nlmatch[r] if LINES else None, B, Bf,
+                     lambda ptr, shape, typestr: torch.as_tensor(_DevArr(int(ptr), shape, typestr), device=dev).cpu().numpy())
 
     # ---- N > 1: the gathered tables must be the single-GPU tables (every rank checks its rows and all ranks agree) ----
     gather_check = None
@@ -558,7 +612,7 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0)); which = "measured" if "hbm_gbs" in peaks else "fallback"
+        peak = float(peaks.get("hbm_gbs", 3350.0)); which = "measured" if "hbm_gbs" in peaks else "H100 SXM data sheet"
         P = sum(ext.level_size(l)[0] * ext.level_size(l)[1] for l in range(8))
         ncand = 0
         for l in range(8):
@@ -579,16 +633,8 @@ def main():
         }
         dom = max(acc, key=acc.get)
         achieved = alg.get(dom, 0) * B / (acc[dom] * 1e-3) / 1e9
-        # dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` captures of the same
-        # 513-frame batch (profiles/r01_ncu_k_lsd_regions_513_final.md, profiles/r01_ncu_orb_kernels_final.md); bytes
-        ncu_traffic = {}
-        try:                                            # written by tools/ncu_summary.py from the round's ncu capture of this workload
-            tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-            ncu_traffic = tj.get(f"{args.workload}:{B}", {})
-        except Exception:
-            pass
         roofline = {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                    "traffic": ncu_traffic.get(dom), "traffic_unit": "bytes per launch (ncu dram read+write, profiles/ncu_traffic.json)", "peak_source": which, "stage_ms": acc,
+                    "peak_source": which, "stage_ms": acc,
                     "algorithmic_bytes_per_launch": alg.get(dom, 0) * B,
                     "note": ("lsd_regions is the order-dependent LSD region stage: latency / issue bound, reported against HBM "
                              "with SURVEY 8(d)'s 17 S bytes per frame" if dom == "lsd_regions" else ""),
@@ -725,29 +771,31 @@ def main():
                 "ms_per_step": ms_total / args.steps, "higher_is_better": True, "scaling": args.scaling, "vs_baseline": None,
                 "dtype": "u8", "data": "synthetic",
                 "config": make_config(args, cfg, world, LINES),
-                "run": {"line_ring": R, "primed": "every ring handle called once before the warm-up steps", "cuda_device_max_connections": os.environ.get("CUDA_DEVICE_MAX_CONNECTIONS"), "e2e_frame_handles": FR, "l2": f"inputs cycle through {nsets} distinct batches ({nsets * B * W * H / 1e6:.0f} MB > 126 MB L2)",
+                "run": {"line_ring": R, "primed": "every ring handle called once before the warm-up steps", "cuda_device_max_connections": os.environ.get("CUDA_DEVICE_MAX_CONNECTIONS"), "e2e_frame_handles": FR, "l2": f"inputs cycle through {nsets} distinct batches ({nsets * B * W * H / 1e6:.0f} MB > 50 MB L2)",
                         "units_counted": "on the device inside the timed region"},
                 "e2e": {"value": eu_all / (e2e_ms * 1e-3), "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                         "ms_per_step": e2e_ms / args.steps},
                 "gpu_launches": int(launches), "clocks": clocks, "roofline": roofline, "cpu_baseline": cpu, "cpu_baseline_cv2": cpu_cv2,
                 "gather_check": gather_check, "table_check": table_check, "in_pipeline": in_pipeline}
         print(json.dumps(line)); sys.stdout.flush()
-    # orderly teardown: the matchers run on the frame handles' streams, so they go first
+    # orderly teardown: the matchers run on the frame handles' streams, so they go first.  The pinned result buffers were copied into on
+    # those streams, and torch records an event on every such stream when it frees them: they go before the streams do.
     torch.cuda.synchronize()
+    for bufs in (h_match, h_nmatch, h_lmatch, h_nlmatch):
+        bufs.clear()
     for m_ in mts + lms:
         m_.close()
     for f_ in frs:
         f_.close()
     if world > 1:
         dist.destroy_process_group()
-    # leave here: the tensors of this frame alias device memory of the handles closed above, and their destructors (run on return)
-    # were seen to fault inside torch at interpreter exit; everything has been printed, synchronised and closed in order
-    sys.stdout.flush(); sys.stderr.flush()
-    os._exit(0)
+    _views.clear()          # views of device memory of the handles closed above: released while torch and the context are up
+    return 0
 
 
 if __name__ == "__main__":
     import faulthandler; faulthandler.enable()
     rc = main()
-    sys.stdout.flush(); sys.stderr.flush()
-    os._exit(rc)          # handles are closed in order above; skip interpreter-exit destructors (arbitrary order across CUDA objects)
+    # main()'s nested functions form reference cycles over its device tensors: collect them now, not during interpreter shutdown
+    gc.collect()
+    sys.exit(rc)

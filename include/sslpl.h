@@ -1,5 +1,5 @@
 /*
- * include/sslpl.h — C ABI of the B200-native point/line front-end (libsslpl_b200.so).
+ * include/sslpl.h — C ABI of the H100-native point/line front-end (libsslpl_b200.so).
  *
  * This is the drop-in boundary for the three data-parallel hot paths of
  * yanyan-li/Structure-SLAM-PointLine's Tracking::TrackWithPL():

@@ -1,6 +1,6 @@
 """structure-slam-pointline_b200 — host-side Python mirror of the reference interface over libsslpl_b200.so.
 
-The product is the C-ABI shared library (include/sslpl.h) built from csrc/*.cu for sm_100a; the C++
+The product is the C-ABI shared library (include/sslpl.h) built from csrc/*.cu for sm_90a; the C++
 adapters with the reference's own class signatures live in host/.  This module is the thin ctypes layer
 the tests and bench.py use; its classes carry the reference's names and argument meaning:
 

@@ -1,4 +1,4 @@
-// common.cuh — shared helpers of libsslpl_b200 (sm_100a).  Product code: no oracle, no CPU fallback.
+// common.cuh — shared helpers of libsslpl_b200 (sm_90a).  Product code: no oracle, no CPU fallback.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

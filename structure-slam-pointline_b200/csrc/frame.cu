@@ -1,4 +1,4 @@
-// frame.cu — the frame-level entry point of libsslpl_b200 (sm_100a): what Frame::Frame(imGray, ...) does with the two
+// frame.cu — the frame-level entry point of libsslpl_b200 (sm_90a): what Frame::Frame(imGray, ...) does with the two
 // extractors (reference src/Frame.cc:69-131), plus the colour conversion in front of it (src/Tracking.cc:148-161) and the keypoint
 // undistortion behind it (Frame::UndistortKeyPoints / ComputeImageBounds, src/Frame.cc:483-543 — SURVEY.md 8(f) row 4):
 //   * ONE host->device copy of the frame (the reference's two extractors each read the same cv::Mat; the per-extractor host entry

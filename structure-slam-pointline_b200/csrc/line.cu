@@ -1,4 +1,4 @@
-// line.cu — B200 (sm_100a) line path: LSD (OpenCV 4.13 LineSegmentDetector, LSD_REFINE_ADV) + KeyLine packaging +
+// line.cu — H100 (sm_90a) line path: LSD (OpenCV 4.13 LineSegmentDetector, LSD_REFINE_ADV) + KeyLine packaging +
 // LBD 256-bit descriptors + line equations.  Replaces LineSegment::ExtractLineSegment
 // (reference src/ExtractLineSegment.cpp:18-69, which delegates to cv::line_descriptor / cv::LineSegmentDetector).
 //
@@ -579,8 +579,8 @@ template <int SOLO> __device__ __noinline__ int l_region_grow(int sx, int sy, do
 
 // -------------------------------------------------------------------------------------------------
 // region_grow, LEAN form (one warp per frame, round 2b).  Same sequential semantics as l_region_grow<1>, restructured around
-// the measured dependent-chain latencies of sm_100a (tools/lat_probe.cu: SHFL 37, MATCH 72, FDIV 57, double alignment test 82,
-// L1 hit 50, L2 hit 280, LDS 34 cycles), because the walker is one warp following one chain:
+// the dependent-chain latencies of the GPU (tools/lat_probe.cu measures SHFL, MATCH, FDIV, the double alignment test, L1 and L2
+// hits and LDS), because the walker is one warp following one chain:
 //   * the region list's tail lives in a shared-memory ring (the frontier is read with LDS, not through L1/L2; the full list
 //     still goes to global memory for region2rect / refine, fire and forget);
 //   * the alignment test runs on the float DEGREES that both operands come from (|theta - a| <= prec is decided in float
@@ -1268,7 +1268,7 @@ __device__ __noinline__ int l_claim(const WalkFrame& F) {
     return found >= ns ? -2 : k;
 }
 
-// 128 registers: a build held to 80 (three 8-warp CTAs per SM) spilled and was 15-20 % slower in every configuration measured
+// 128 registers: a build held to 80 (three 8-warp CTAs per SM) spills
 __global__ void __launch_bounds__(WALK_MAXW * 32) k_lsd_regions(const __grid_constant__ LineGeom g, LineWs ws, int nframes) {
     extern __shared__ unsigned s_bits[];                       // committed `used` bitmap of the frame
     const int lane = threadIdx.x & 31;
@@ -1390,8 +1390,8 @@ __global__ void __launch_bounds__(WALK_MAXW * 32) k_lsd_regions(const __grid_con
 }
 
 // THROUGHPUT form of the same stage for big batches: ONE WARP PER FRAME, no speculation (every instruction is useful work, 72
-// registers, ~28 frames resident per SM; 46 ms latency per frame, ~17 us per frame amortised with >= 3000 frames in flight).
-// sslpl picks it when a call brings at least two frames per SM; smaller calls use the multi-warp walker above (17 ms per frame).
+// registers, ~28 frames resident per SM; latency-bound per frame, amortised when thousands of frames are in flight).
+// sslpl picks it when a call brings at least two frames per SM; smaller calls use the multi-warp walker above.
 #ifndef SSLPL_SOLO_MINB
 #define SSLPL_SOLO_MINB 28
 #endif
@@ -1442,10 +1442,9 @@ __global__ void __launch_bounds__(32, SSLPL_SOLO_MINB) k_lsd_regions_solo(const 
   }
 }
 
-// The same loop over the frame's seeds with the LEAN region growing (l_region_grow_lean).  Alone it takes the same time as
-// k_lsd_regions_solo (49.5 vs 50.6 ms for 148 frames), with several launches overlapping it is slower (38.5 vs 29.2 ms per bench
-// step): it executes 5 % MORE warp instructions (the lazy-angle bookkeeping costs what the removed FP64 saved), and a lone warp's time
-// is instructions x ~8 cycles.  Kept for A/B runs (SSLPL_WALKER_LEAN=1) and as the base of the v3 and lane-parallel growth.
+// The same loop over the frame's seeds with the LEAN region growing (l_region_grow_lean).  It is not faster than
+// k_lsd_regions_solo: it executes slightly MORE warp instructions (the lazy-angle bookkeeping costs what the removed FP64 saved), and a
+// lone warp's time is its instruction count times the dependent-issue latency.  Kept for A/B runs (SSLPL_WALKER_LEAN=1) and as the base of the v3 and lane-parallel growth.
 __global__ void __launch_bounds__(32, 28) k_lsd_regions_lean(const __grid_constant__ LineGeom g, LineWs ws, int nframes) {
     const int lane = threadIdx.x;
   for (;;) {
@@ -1499,9 +1498,8 @@ __global__ void __launch_bounds__(32, 28) k_lsd_regions_lean(const __grid_consta
 
 // =================================================================================================
 // Multi-warp region walker, v3 (round 2b).  Same idea as k_lsd_regions — regions are grown AHEAD of the sequential order
-// by several warps and retired strictly IN that order — with the two costs that dominated it removed (measured on one
-// 640x480 frame: 58 % of the frame's cycles under the commit lock, 3600 cycles per commit, every invalid attempt regrown
-// under that lock while 15 warps wait):
+// by several warps and retired strictly IN that order — with the two costs that dominated it removed (much of a frame's
+// cycles under the commit lock, every invalid attempt regrown under that lock while 15 warps wait):
 //   * RETIRING AN ATTEMPT IS O(1).  "Used" is not a bitmap that a commit has to fill but a property of the ticket found in
 //     LPix.used: a ticket (rank, try) of a retired rank is USED iff that try is the one the rank committed with.  That
 //     is try 0 unless the rank's bit is set in a 64k-bit exception map in shared memory (then one byte per rank in global
@@ -1510,7 +1508,7 @@ __global__ void __launch_bounds__(32, 28) k_lsd_regions_lean(const __grid_consta
 //   * validity is tracked where it is decided: an attempt that takes a pixel from a live attempt of higher rank POISONS it;
 //     an attempt that meets a pixel held by a live attempt of LOWER rank assumes it used and records that attempt as a
 //     dependency (two at most), valid iff it commits with that very try without ever having released a pixel;
-//   * warp 0 is the CONTROL warp (claims seeds in order into a ring of 256 tiny slots (more ranks in flight only add wasted speculation: 14.4-15.0 ms per frame at 128-256, 17.9 at 1024, 30.7 at 4096), retires the head); the others are
+//   * warp 0 is the CONTROL warp (claims seeds in order into a ring of 256 tiny slots (more ranks in flight only add wasted speculation), retires the head); the others are
 //     workers that pick the lowest runnable slot.  No locks.  An invalid attempt goes back to the ring with try + 1; the
 //     head of the ring can neither meet a live lower rank nor be poisoned, so its attempt always commits.
 // Region growing is the lean form (float-degree test, lazy angle, list tail in shared memory) with tickets taken by CAS whose
@@ -2065,8 +2063,8 @@ __global__ void __launch_bounds__(V3_MAXW * 32) k_lsd_regions_v3(const __grid_co
 
 // =================================================================================================
 // LANE-PARALLEL region walker (round 2b, k_lsd_regions_lanes): ONE WARP PER FRAME, every LANE grows its own region.
-// The one-warp walkers spend ~230 warp instructions per growth step on 32 neighbour tests of ONE region, almost all of it
-// warp-uniform bookkeeping: a lone warp retires one instruction every ~8 cycles, so the stage is bound by instruction count.
+// The one-warp walkers spend hundreds of warp instructions per growth step on 32 neighbour tests of ONE region, almost all of it
+// warp-uniform bookkeeping: a lone warp retires one instruction every several cycles, so the stage is bound by instruction count.
 // Here region growing is the plain scalar loop of lsd.cpp run by each lane on a different seed (same protocol as the multi-warp
 // walker v3: ranks in seed order, tickets in LPix.used, poison / dependencies / released-pixel lists, strictly ordered retire —
 // v3_retire_pass and v3_claim_pass are used as they are), so that one warp instruction serves up to 32 regions.  A neighbour is
@@ -2830,7 +2828,7 @@ struct sslpl_line {
     LbdCoef coef;
     bool trace = false;
     int used_smem = 0;
-    int sm_count = 148;
+    int sm_count = 132;         // replaced by the device's count at creation
     int max_walkers = 0;        // 0 = one walker CTA per frame
     int walker_warps = 0;       // 0 = automatic (8 or 16 warps per frame)
     int walker_v3 = 0;          // multi-warp walker: 0 = the round-2a form (shipped), 1 = v3 (control warps + workers, O(1) retire), -1 = v3 by frame size
@@ -2968,10 +2966,10 @@ int run_pipeline(sslpl_line* h, int B) {
     SSLPL_CUDA(cudaMemsetAsync(h->ws.rejctl, 0, 4 * sizeof(int), st));
     SSLPL_CUDA(cudaMemsetAsync(h->ws.wstat, 0, 16 * sizeof(unsigned long long), st));
     {   // one CTA per frame; few frames -> more warps per frame (latency), many frames -> more CTAs per SM (throughput)
-        // automatic choice (measured, B200): big batches -> one warp per frame (throughput); one or a few frames -> a multi-warp CTA per
-        // frame, the round-2a walker with 16 warps.  v3 (SSLPL_WALKER_V3=1, 8 warps) is level with it on 640x480 frames (15.0-17.0 ms over
-        // runs against 17.2 ms) and behind on 1280x960 (115 ms against 69 ms: its deeper speculation loses more work than it overlaps), so
-        // it is not the default; SSLPL_WALKER_V3=-1 picks it by frame size (up to ~0.3 M detection-scale pixels)
+        // automatic choice: big batches -> one warp per frame (throughput); one or a few frames -> a multi-warp CTA per frame, the
+        // round-2a walker with 16 warps.  v3 (SSLPL_WALKER_V3=1, 8 warps) is at best level with it on 640x480 frames and behind on
+        // 1280x960 (its deeper speculation loses more work than it overlaps), so it is not the default; SSLPL_WALKER_V3=-1 picks it by
+        // frame size (up to ~0.3 M detection-scale pixels)
         const bool small = g.pix_stride <= 300000;
         const bool v3 = h->walker_v3 > 0 || (h->walker_v3 < 0 && small);
         const int ww = h->walker_warps < 0 ? 0 : h->walker_warps > 0 ? std::min(h->walker_warps, WALK_MAXW) : (B >= 2 * h->sm_count ? 0 : (v3 ? 8 : WALK_MAXW));

@@ -1,4 +1,4 @@
-// match.cu — B200 (sm_100a) Hamming matchers: brute-force 2-NN (cv::BFMatcher knnMatch k=2), vocabulary-node
+// match.cu — H100 (sm_90a) Hamming matchers: brute-force 2-NN (cv::BFMatcher knnMatch k=2), vocabulary-node
 // assignment, SearchByBoW (KF-Frame and KF-KF), SearchForTriangulation, rotation-histogram filter, and the
 // knn-based LSDmatcher entry points.  Replaces the distance work of src/ORBmatcher.cc and src/LSDmatcher.cpp.
 //
@@ -14,7 +14,7 @@
 namespace sslpl {
 
 constexpr int TH_LOW = 50;          // ORBmatcher.cc:38
-constexpr int MAX_DYN_SMEM = 200 * 1024;   // dynamic shared memory the two data-dependent kernels may ask for (sm_100: 227 KB per CTA, static included)
+constexpr int MAX_DYN_SMEM = 200 * 1024;   // dynamic shared memory the two data-dependent kernels may ask for (sm_90: 227 KB per CTA, static included)
 constexpr int HISTO_LENGTH = 30;    // ORBmatcher.cc:39
 
 // A set of frames in HBM (strides in elements of the respective type)
@@ -105,7 +105,7 @@ __global__ void __launch_bounds__(128) k_bow_assign(const uint8_t* desc, long lo
 // DBoW2 TemplatedVocabulary<FORB>::transform (Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1218-1259): descend the
 // k-ary tree by Hamming distance (strict '<': the first best child wins), one thread per descriptor.  The tree is
 // stored as CSR children lists (ascending node id, as loadFromTextFile builds them) + 32-byte node descriptors; the
-// upper levels stay resident in L1/L2 (ORBvoc: 1.1 M nodes x 32 B = 35 MB < 126 MB L2).
+// upper levels stay resident in L1/L2 (ORBvoc: 1.1 M nodes x 32 B = 35 MB < 50 MB L2).
 //   word  = word id of the leaf,  node = NodeId at level L - levelsup (0 if the leaf comes earlier),
 //   rank  = dense index of `node` among the possible values (0 = root / early leaf, 1 + rank inside the level), or -1 for a
 //           stopped word (weight <= 0), which the reference keeps out of the FeatureVector (:1162-1166).
@@ -1083,7 +1083,7 @@ int sslpl_matcher_create(const sslpl_matcher_params* p, sslpl_matcher** out) {
         for (int i = 0; i <= p->max_nodes; i++) iota[i] = i;
         e2 = cudaMemcpy(m->iota, iota.data(), sizeof(int) * iota.size(), cudaMemcpyHostToDevice);
     }
-    // the two kernels with data-dependent dynamic shared memory may use the whole 227 KB of an sm_100 CTA
+    // the two kernels with data-dependent dynamic shared memory may use the whole 227 KB of an sm_90 CTA
     if (e2 == cudaSuccess) e2 = cudaFuncSetAttribute(k_bow_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM);
     if (e2 == cudaSuccess) e2 = cudaFuncSetAttribute(k_build_csr, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM);
     if (e2 != cudaSuccess) { set_error("sslpl_matcher_create: %s", cudaGetErrorString(e2)); sslpl_matcher_destroy(m); return SSLPL_ERR_CUDA; }

@@ -1,4 +1,4 @@
-// orb.cu — B200 (sm_100a) ORB extractor: pyramid / FAST+NMS / octree distribution / IC orientation /
+// orb.cu — H100 (sm_90a) ORB extractor: pyramid / FAST+NMS / octree distribution / IC orientation /
 // 7x7 blur / rBRIEF-256, batched over frames.  Replaces ORBextractor (reference src/ORBextractor.cc).
 //
 // Everything stays in HBM between the frame upload and the keypoint/descriptor download:
@@ -152,7 +152,7 @@ __device__ __forceinline__ int fast_score_tile(const uint8_t* p, int pitch, int 
 }
 
 // ------------------------------------------------------------------------------------------------
-// TMA / mbarrier helpers (sm_100a): one elected thread arms the barrier with the byte count and issues a
+// TMA / mbarrier helpers (sm_90a): one elected thread arms the barrier with the byte count and issues a
 // cp.async.bulk.tensor.3d tile load (x, y, frame); out-of-bounds elements are zero-filled by the hardware.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -164,12 +164,25 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+// Watchdog: a copy still pending after 20 s of wall time is mis-programmed, and the CTA traps instead of hanging the GPU.  The
+// bound is a time, not a number of polls: an H100 polls fast, and on a GPU shared with other processes (time slices) or crowded
+// with resident LSD walkers a correct copy can outlast any fixed count of polls that is short enough to matter.
+__device__ __forceinline__ uint64_t global_ns() {
+    uint64_t t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     uint32_t ok = 0;
-    for (int spin = 0; !ok; spin++) {
+    uint64_t t0 = 0;
+    for (unsigned spin = 1; !ok; spin++) {
         asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}\n"
                      : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-        if (spin > (1 << 24)) __trap();          // never hang the box on a mis-programmed copy
+        if (!ok && (spin & 1023u) == 0) {
+            const uint64_t t = global_ns();
+            if (t0 == 0) t0 = t;
+            else if (t - t0 > 20000000000ull) __trap();
+        }
     }
 }
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* tm, int x, int y, int z, uint64_t* bar) {
@@ -178,8 +191,9 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* t
 }
 
 constexpr int TL_W = 64, TL_H = 32;            // output tile of the stencil kernels
-constexpr int TL_P = 96, TL_IH = TL_H + 6;     // staged box: 96 x 38 bytes, origin (x0 - 16, y0 - 3).  For 1-byte elements TMA
-                                               // requires the box to START on a 16-byte boundary in x (measured: tools/tma_probe.cu)
+constexpr int TL_P = 96, TL_IH = TL_H + 6;     // staged box: 96 x 38 bytes, origin (x0 - 16, y0 - 3).  Constraint: a TMA box of
+                                               // 1-byte elements must START on a 16-byte boundary in x (any other origin is an
+                                               // illegal instruction that kills the context), so every box origin is a multiple of 16
 constexpr int TL_X = 16;                       // smem column of the tile's first output pixel
 
 // Stage the 96x38 box of level `l`, frame `f` at (bx, by) into s_img (pitch TL_P).  TMA path: one bulk tensor copy,
@@ -225,8 +239,8 @@ __device__ __forceinline__ void stage_box(uint8_t* s_img, uint64_t* s_bar, const
 // from that its tile of level L+1.  Neighbouring CTAs recompute the one-pixel halo of level L (about 30 % more level-L arithmetic;
 // level L-1 is read once, level L is never read back).  Same fixed-point arithmetic and tables as k_resize, so the planes are
 // bit-identical.  The host falls back to k_resize for a level pair whose spans exceed the tiles below (never at scale 1.2) and for
-// the last level when their number is odd.  MEASURED (513 frames 640x480): 1.00 ms against 0.85 ms for the seven k_resize launches —
-// the plain kernel's byte loads already hit L1 / L2, while a 64x16 tile pays one TMA round trip and 30 % recomputed halo; it is kept
+// the last level when their number is odd.  The plain kernel's byte loads already hit L1 / L2, while a 64x16 tile pays one TMA round
+// trip and 30 % recomputed halo; it is kept
 // behind SSLPL_PYR2=1 (tests/test_orb_gpu.py::test_pyramid_two_levels_per_launch_path), k_resize stays the default.
 constexpr int PY_TW = 64, PY_TH = 16, PY_MP = 88, PY_MH = 24, PY_BW = 128, PY_BH = 32;
 
@@ -909,7 +923,7 @@ struct sslpl_orb {
     TMaps tm;                           // per-level tensor maps (level 0 re-encoded per call: the input view moves)
     PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
     bool tma_levels_ok = false, use_tma = true;
-    bool use_pyr2 = false;              // SSLPL_PYR2=1: two levels per launch (k_pyr2); measured 1.00 ms against 0.85 ms for the seven k_resize launches (513 frames)
+    bool use_pyr2 = false;              // SSLPL_PYR2=1: two levels per launch (k_pyr2), not faster than the seven k_resize launches
     bool pyr2_ok[MAXL] = {};            // level pair (L, L+1) fits the tiles of k_pyr2 (checked against the resize tables)
     const uint8_t* tm0_base = nullptr; int tm0_pitch = 0, tm0_frames = 0; long long tm0_fs = 0;
 };

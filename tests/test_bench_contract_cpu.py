@@ -1,5 +1,5 @@
 """The driver-facing contract of bench.py that can be checked without a GPU: the reference arm prints ONE JSON line with the
-agreed keys (and does nothing on ranks != 0), and the B200 arm fails loudly — no silent CPU fallback — when no GPU exists."""
+agreed keys (and does nothing on ranks != 0), and the GPU arm fails loudly — no silent CPU fallback — when no GPU exists."""
 import json
 import os
 import subprocess

@@ -1,6 +1,6 @@
-"""GPU: the drop-in claim, end to end.  tests/integration/_bin/ref_link_test is linked from the reference's OWN unmodified translation
+"""GPU: the drop-in claim, end to end.  oracle/_ref/ref_link_test (built by build(), oracle/ref_link_build.sh) is linked from the reference's OWN unmodified translation
 units (Frame.cc, KeyFrame.cc, MapPoint.cc, MapLine.cpp, Map.cc, KeyFrameDatabase.cc, ORBmatcher.cc, LSDmatcher.cpp, DBoW2), the
-adapters of structure-slam-pointline_b200/host/ and libsslpl_b200.so (tests/integration/build_ref_link.sh).  It runs Frame::Frame,
+adapters of structure-slam-pointline_b200/host/ (tests/integration/ref_link_test.cpp) and libsslpl_b200.so.  It runs Frame::Frame,
 ComputeBoW, KeyFrame, ORBmatcher::SearchByBoW / SearchByProjection and LSDmatcher::SearchByProjection the way Tracking does; what it
 produced through the GPU is compared here with the fixtures frozen from the reference and with oracle/_ref (the reference on the CPU)."""
 import os
@@ -13,14 +13,12 @@ from test_ref_golden_cpu import load
 from test_ref_parity_cpu import write_vocab_text
 
 pytestmark = pytest.mark.gpu
-BIN = os.path.join(ROOT, "tests", "integration", "_bin", "ref_link_test")
+BIN = os.path.join(ROOT, "oracle", "_ref", "ref_link_test")
 
 
 def test_reference_objects_plus_adapters_on_the_gpu(pkg, oracle, icl_gray, tmp_path):
-    if os.path.isdir("/root/reference/src"):
-        subprocess.run(["bash", os.path.join(ROOT, "tests", "integration", "build_ref_link.sh")], check=True, stdout=subprocess.DEVNULL)
     if not os.path.exists(BIN):
-        pytest.skip("tests/integration/_bin/ref_link_test not built (needs /root/reference)")
+        pytest.skip("oracle/_ref/ref_link_test not built (build() builds it where the reference's sources are present)")
     from oracle import ref as R
     if not R.available():
         pytest.skip("oracle/_ref not built")

@@ -28,7 +28,7 @@ def _run(n):
 def test_gathered_tables_equal_single_gpu():
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     a, b = _run(1), _run(2)
     assert a["table_check"]["rows"] == b["table_check"]["rows"] == 64 and a["table_check"]["matches"] > 1000
     assert a["table_check"] == {**b["table_check"], "frames": a["table_check"]["frames"]} or a["table_check"]["checksum"] == b["table_check"]["checksum"], (a["table_check"], b["table_check"])

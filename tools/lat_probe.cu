@@ -1,5 +1,5 @@
-// tools/lat_probe.cu — dependent-chain latencies on sm_100a (one warp): what the sequential LSD walker is made of.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -fmad=false -o /tmp/lat_probe tools/lat_probe.cu && /tmp/lat_probe
+// tools/lat_probe.cu — dependent-chain latencies on sm_90a (one warp): what the sequential LSD walker is made of.
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -fmad=false -o /tmp/lat_probe tools/lat_probe.cu && /tmp/lat_probe
 #include <cstdio>
 #include <cuda_runtime.h>
 #define N 4096

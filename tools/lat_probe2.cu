@@ -1,4 +1,4 @@
-// tools/lat_probe2.cu — does prefetch.global.L1 warm the L1 on sm_100a?  (time of a dependent load after different warm-ups)
+// tools/lat_probe2.cu — does prefetch.global.L1 warm the L1 on sm_90a?  (time of a dependent load after different warm-ups)
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void k(const unsigned* g, unsigned* out, long long* cyc, int mode, int stride) {

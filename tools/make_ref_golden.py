@@ -1,12 +1,13 @@
 #!/usr/bin/env python3
 """Freeze outputs of THE REFERENCE ITSELF (oracle/_ref/libref.so = the reference's sources compiled unmodified, see
-oracle/ref_build.sh) into small fixtures under tests/golden/ref_*.npz, so that boxes without /root/reference (the GPU box)
-can still hold the oracle and the CUDA path against the reference.  Run in the build container:
+oracle/ref_build.sh) into small fixtures under tests/golden/ref_*.npz, so that machines without the reference's sources
+can still hold the oracle and the CUDA path against the reference.  Run where oracle/ref_build.sh can build the reference:
 
     python tools/make_ref_golden.py
 
 Inputs are the committed ICL frame and the deterministic synthetic frames of tools/synth.py; every array the tests need
-to rebuild the call is stored next to the reference's output."""
+to rebuild the call is stored next to the reference's output.  tests/golden/ref_parity.npz holds the reference's answers to
+every call of tests/test_ref_parity_cpu.py (tests/ref_replay.py), recorded by running that module."""
 import os
 import sys
 import hashlib
@@ -78,7 +79,10 @@ def main():
     np.savez_compressed(os.path.join(G, "ref_frame.npz"), keylines=fr["keylines"], ldesc=fr["ldesc"], lineeq=fr["lineeq"],
                         grid_off=fr["grid_off"], grid_idx=fr["grid_idx"])
     row3()
-    for f in ("ref_orb.npz", "ref_match.npz", "ref_frame.npz", "ref_row3.npz"):
+    import subprocess
+    subprocess.run([sys.executable, "-m", "pytest", "-q", "-p", "no:cacheprovider", os.path.join(ROOT, "tests", "test_ref_parity_cpu.py")],
+                   check=True, cwd=ROOT, env=dict(os.environ, SSLPL_REF_RECORD="1"))
+    for f in ("ref_orb.npz", "ref_match.npz", "ref_frame.npz", "ref_row3.npz", "ref_parity.npz"):
         p = os.path.join(G, f)
         print(f, os.path.getsize(p), hashlib.sha1(open(p, "rb").read()).hexdigest()[:12])
 

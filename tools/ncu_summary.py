@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Summarise an .ncu-rep (ncu --set full capture) as markdown: python tools/ncu_summary.py file.ncu-rep > profiles/x.md"""
+"""Summarise an .ncu-rep (ncu --set full capture) as markdown: python tools/ncu_summary.py file.ncu-rep > summary.md"""
 import csv, subprocess, sys
 rep = sys.argv[1]
 raw = subprocess.run(["ncu", "-i", rep, "--page", "raw", "--csv"], capture_output=True, text=True).stdout

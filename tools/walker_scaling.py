@@ -6,7 +6,7 @@ import numpy as np, torch
 import __graft_entry__ as g, synth
 pkg = g.load_package()
 base = synth.batch(640, 480, 64)
-for B in [int(a) for a in sys.argv[1:]] or (148, 513, 1026, 2052, 4104):
+for B in [int(a) for a in sys.argv[1:]] or (132, 513, 1026, 2052, 4104):
     frames = np.concatenate([base] * (B // 64 + 1))[:B]
     d = torch.from_numpy(frames).cuda()
     ls = pkg.LineSegment(40, max_width=640, max_height=480, max_batch=B)
