@@ -2,7 +2,7 @@
 // LBD 256-bit descriptors + line equations.  Replaces LineSegment::ExtractLineSegment
 // (reference src/ExtractLineSegment.cpp:18-69, which delegates to cv::line_descriptor / cv::LineSegmentDetector).
 //
-// Per-pixel stages are ordinary data-parallel kernels (k_sep7, k_resize_exact, k_ll_angle, k_lsd_seeds, k_lsd_nfa_*, k_sobel).
+// Per-pixel stages are ordinary data-parallel kernels (k_lsd_prep: both blurs, resize, ll_angle and Sobel in one pass; k_lsd_seeds, k_lsd_nfa_*).
 // The region stage (k_lsd_regions) is order-dependent by definition (seeds in descending gradient bins, shared
 // `used` map, incrementally updated region angle): one warp walks one frame; the warp's lanes cooperate on neighbour
 // fetches and on the rectangle scans of rect_nfa, frames of a batch run on different SMs.  It is latency-bound,
@@ -27,17 +27,15 @@ constexpr double L_3_2_PI = (3 * L_PI) / 2;
 constexpr double L_2PI = 2 * L_PI;
 constexpr float NOTDEF_F = -1024.f;
 constexpr int NBINS = 1024;
-constexpr int LT_W = 64, LT_H = 32;          // tile of the separable filter
 
 struct LineGeom {
     int w, h, pitch;            // input frame (pitch of the staging / view)
-    int bpitch;                 // blurred planes (7-tap for LSD, 5-tap for LBD)
-    int sw, sh, spitch;         // LSD detection scale (0.8x)
-    int tiles_x, tiles_y;
+    int sw, sh;                 // LSD detection scale (0.8x)
+    int tiles_x, tiles_y;       // tiles of k_lsd_prep
     int xtab_off, ytab_off;     // INTER_LINEAR_EXACT tables (int2: index, w1)
     int seg_cap;                // raw segments per frame
     int kl_cap;                 // lsdNFeatures
-    long long in_stride, blur_stride, scaled_stride, pix_stride /* sw*sh */, full_stride /* w*h */;
+    long long in_stride, pix_stride /* sw*sh */, full_stride /* w*h */;
     double rho, prec, p, log_nt;
     int min_reg_size;
     int trace_cap;              // rows of the debug trace per frame (0 = off)
@@ -50,7 +48,6 @@ struct LineGeom {
 struct __align__(16) LPix { float ang, cx, cy; unsigned used; };   // `used` = ticket of the region-growing attempt holding the pixel (0 = none)
 
 struct LineWs {
-    uint8_t* blur7; uint8_t* blur5; uint8_t* scaled;
     float* angdeg; LPix* pix; float2* cs0; double* modgrad;
     unsigned long long* maxgrad; unsigned* seeds; int* nseeds;
     unsigned* reg;              // region pixel list (x | y << 16) of the turn holder (whole-frame capacity)
@@ -75,82 +72,6 @@ struct LineWs {
 
 struct LView { const uint8_t* base; int pitch; long long frame_stride; };
 
-// -------------------------------------------------------------------------------------------------
-// Separable fixed-point filter (OpenCV 4.13 GaussianBlur 8U path): out = (sum_j k_j sum_i k_i p + 32768) >> 16
-// taps are passed as 7 ints (5-tap kernels are zero-padded), BORDER_REFLECT_101.
-// -------------------------------------------------------------------------------------------------
-struct Taps7 { int k[7]; };
-
-// Packed arithmetic: the horizontal pass is two dp4a per output on byte windows cut out of three aligned words with funnel
-// shifts; its u16 results are stored as vertical PAIRS (row r | row r+1 << 16) so that the vertical pass is four dp2a per
-// output.  All taps are < 256 and every partial sum < 65536, so the packed forms are exact.
-// One launch filters the SAME staged input tile with two tap sets (LSD's 7-tap pre-blur and the 5-tap blur of the LBD stage): the tile
-// is read from global memory once (round 2b; two launches of the one-filter form before).  out1 == nullptr: one filter only.
-__global__ void __launch_bounds__(256) k_sep7(const __grid_constant__ LineGeom g, LView v, uint8_t* out0, uint8_t* out1, long long out_stride, Taps7 t0, Taps7 t1) {
-    constexpr int IW = LT_W + 6, IP = LT_W + 8, IH = LT_H + 6;           // IP % 4 == 0: rows of s_in are word aligned
-    __shared__ __align__(4) uint8_t s_in[IH * IP];
-    __shared__ __align__(16) unsigned s_pair[IH * LT_W];                 // [r][x] = row r | row r+1 << 16
-    unsigned short* s_half = reinterpret_cast<unsigned short*>(s_pair);
-    const int tile = blockIdx.x, f = blockIdx.y, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int ty = tile / g.tiles_x, tx = tile - ty * g.tiles_x, x0 = tx * LT_W, y0 = ty * LT_H;
-    const uint8_t* img = v.base + f * v.frame_stride;
-    for (int yy = wid; yy < IH; yy += 8) {                               // a warp per input row: no per-element division
-        const uint8_t* src = img + (long long)reflect101(y0 + yy - 3, g.h) * v.pitch;
-        for (int xx = lane; xx < IW; xx += 32) s_in[yy * IP + xx] = __ldg(src + reflect101(x0 + xx - 3, g.w));
-    }
-    __syncthreads();
-#pragma unroll 1
-    for (int pass = 0; pass < 2; pass++) {
-        uint8_t* out = pass ? out1 : out0;
-        if (!out) break;
-        const Taps7& t = pass ? t1 : t0;
-        const unsigned T0 = (unsigned)t.k[0] | ((unsigned)t.k[1] << 8) | ((unsigned)t.k[2] << 16) | ((unsigned)t.k[3] << 24);
-        const unsigned T1 = (unsigned)t.k[4] | ((unsigned)t.k[5] << 8) | ((unsigned)t.k[6] << 16);
-        for (int i = tid; i < IH * (LT_W / 4); i += 256) {
-            const int yy = i / (LT_W / 4), x4 = (i - yy * (LT_W / 4)) * 4;
-            const unsigned* w = reinterpret_cast<const unsigned*>(&s_in[yy * IP + x4]);
-            const unsigned w0 = w[0], w1 = w[1], w2 = w[2];                  // bytes x4 .. x4+11 (output k uses bytes k .. k+6)
-#pragma unroll
-            for (int k = 0; k < 4; k++) {
-                const unsigned A = k ? __funnelshift_r(w0, w1, 8 * k) : w0, B = k ? __funnelshift_r(w1, w2, 8 * k) : w1;
-                const unsigned r = __dp4a(A, T0, __dp4a(B, T1, 0u));
-                s_half[(yy * LT_W + x4 + k) * 2] = (unsigned short)r;                          // low half of pair row yy
-                if (yy > 0) s_half[((yy - 1) * LT_W + x4 + k) * 2 + 1] = (unsigned short)r;    // high half of pair row yy-1
-            }
-        }
-        __syncthreads();
-        uint8_t* o = out + f * out_stride;
-        const unsigned C01 = (unsigned)t.k[0] | ((unsigned)t.k[1] << 8), C23 = (unsigned)t.k[2] | ((unsigned)t.k[3] << 8);
-        const unsigned C45 = (unsigned)t.k[4] | ((unsigned)t.k[5] << 8), C6 = (unsigned)t.k[6];
-        for (int i = tid; i < LT_H * (LT_W / 4); i += 256) {
-            const int yy = i / (LT_W / 4), x4 = (i - yy * (LT_W / 4)) * 4;
-            if (y0 + yy >= g.h || x0 + x4 >= g.w) continue;
-            const uint4 p0 = *reinterpret_cast<const uint4*>(&s_pair[yy * LT_W + x4]), p2 = *reinterpret_cast<const uint4*>(&s_pair[(yy + 2) * LT_W + x4]);
-            const uint4 p4 = *reinterpret_cast<const uint4*>(&s_pair[(yy + 4) * LT_W + x4]), p6 = *reinterpret_cast<const uint4*>(&s_pair[(yy + 6) * LT_W + x4]);
-            const unsigned a0 = __dp2a_lo(p0.x, C01, __dp2a_lo(p2.x, C23, __dp2a_lo(p4.x, C45, __dp2a_lo(p6.x, C6, 32768u))));
-            const unsigned a1 = __dp2a_lo(p0.y, C01, __dp2a_lo(p2.y, C23, __dp2a_lo(p4.y, C45, __dp2a_lo(p6.y, C6, 32768u))));
-            const unsigned a2 = __dp2a_lo(p0.z, C01, __dp2a_lo(p2.z, C23, __dp2a_lo(p4.z, C45, __dp2a_lo(p6.z, C6, 32768u))));
-            const unsigned a3 = __dp2a_lo(p0.w, C01, __dp2a_lo(p2.w, C23, __dp2a_lo(p4.w, C45, __dp2a_lo(p6.w, C6, 32768u))));
-            *reinterpret_cast<uint32_t*>(o + (long long)(y0 + yy) * g.bpitch + x0 + x4) = (a0 >> 16) | ((a1 >> 16) << 8) | ((a2 >> 16) << 16) | ((a3 >> 16) << 24);
-        }
-        __syncthreads();                                                  // s_pair is rewritten by the second filter
-    }
-}
-
-// cv::resize(INTER_LINEAR_EXACT) 8U, 8.8 fixed point (SURVEY.md A.6 iii): tables hold (i0, w1)
-__global__ void __launch_bounds__(256) k_resize_exact(const __grid_constant__ LineGeom g, LineWs ws) {
-    const int x = blockIdx.x * 32 + threadIdx.x, y = blockIdx.y * 8 + threadIdx.y, f = blockIdx.z;
-    if (x >= g.sw || y >= g.sh) return;
-    const uint8_t* S = ws.blur7 + f * g.blur_stride;
-    const int2 tx = __ldg(&ws.tab[g.xtab_off + x]), ty = __ldg(&ws.tab[g.ytab_off + y]);
-    const int i0 = tx.x, i1 = min(i0 + 1, g.w - 1), w1 = tx.y, w0 = 256 - w1;
-    const uint8_t* S0 = S + (long long)ty.x * g.bpitch;
-    const uint8_t* S1 = S + (long long)min(ty.x + 1, g.h - 1) * g.bpitch;
-    const int r0 = w0 * __ldg(S0 + i0) + w1 * __ldg(S0 + i1), r1 = w0 * __ldg(S1 + i0) + w1 * __ldg(S1 + i1);
-    const int v1 = ty.y, v0 = 256 - v1;
-    ws.scaled[f * g.scaled_stride + (long long)y * g.spitch + x] = (uint8_t)((v0 * r0 + v1 * r1 + 32768) >> 16);
-}
-
 // sin / cos of x in [0, 2 pi] to ~1 ulp (double): Cody-Waite reduction by pi/2 and the fdlibm kernel polynomials.
 // Branch-free and table-free (libm's sincos drags its large-argument path and constant-bank tables through the
 // memory pipe); the callers round the results to float, which hides the last-ulp freedom.
@@ -171,20 +92,163 @@ __device__ __forceinline__ void l_sincos_2pi(double x, double* s_out, double* c_
     *c_out = (q == 0) ? c : (q == 1) ? -s : (q == 2) ? -c : s;
 }
 
-// ll_angle (lsd.cpp): 2x2 gradient, level-line angle, gradient norm, max over defined pixels
-// Four horizontally adjacent pixels per thread: 4 loads and 9 vector stores per 4 pixels instead of 16 + 16 (the
-// scalar version was limited by the memory-instruction queue, not by HBM or by the trigonometry).
-__global__ void __launch_bounds__(256) k_ll_angle(const __grid_constant__ LineGeom g, LineWs ws) {
-    const int x0 = (blockIdx.x * 32 + threadIdx.x) * 4, y = blockIdx.y * 8 + threadIdx.y, f = blockIdx.z;
+// -------------------------------------------------------------------------------------------------
+// The per-pixel pre-pass of LSD and LBD in one kernel, one CTA per tile.  From one staged box of the input frame it computes
+//   blur5  GaussianBlur(5x5, sigma 1) of BinaryDescriptor  -> Sobel 3x3 -> dx, dy (s16, input resolution)
+//   blur7  GaussianBlur(sigma 0.6/0.8) of lsd.cpp          -> resize 0.8x (INTER_LINEAR_EXACT) -> ll_angle -> pix, angdeg, cs0, modgrad, maxgrad
+// and keeps blur5, blur7 and the resized image in shared memory: none of the three is written to global memory.
+// 0.8 = 4/5, so a PT_W x PT_H tile of input pixels maps exactly onto PT_SW x PT_SH detection-scale pixels (the 4 resized pixels of
+// a group of 5 input columns or rows read only those 5).  Halos are recomputed by each CTA.
+// Both blurs are OpenCV 4.13's GaussianBlur 8U fixed point, out = (sum_j k_j sum_i k_i p + 32768) >> 16 with BORDER_REFLECT_101, and
+// have five non-zero taps (lsd.cpp's 7-tap kernel rounds its end taps to 0).  The horizontal pass is two dp4a per output on byte
+// windows of three aligned words, the vertical pass dp2a on (row r | row r+1 << 16) pairs: all taps are < 256 and every partial
+// sum of the horizontal pass < 65536, so the packed forms are exact.
+// -------------------------------------------------------------------------------------------------
+constexpr int PT_W = 160, PT_H = 40, PT_SW = 128, PT_SH = 32;    // input tile and its 0.8x image
+constexpr int PT_NT = 128;                                      // threads per CTA
+constexpr int PI_X = 4, PI_Y = 3;                               // staged box origin (X0 - 4, Y0 - 3): X0 % 32 == 0, so the origin is word aligned
+constexpr int PI_W = 172, PI_H = 47;                            // staged box: columns X0-4 .. X0+167, rows Y0-3 .. Y0+43
+constexpr int PB_W = 164, PB_H = 42;                            // blurred box (162 columns used): blur5 from (X0-1, Y0-1), blur7 from (X0, Y0)
+constexpr int PH_H = PB_H + 4;                                  // rows of the horizontal pass
+constexpr int PS_W = 132, PS_H = PT_SH + 1;                     // resized box from (SX0, SY0): the tile + one column and one row (129 columns used)
+constexpr unsigned BL7_T0 = 4u | 56u << 8 | 136u << 16 | 56u << 24, BL7_T4 = 4u;      // lsd.cpp: {0, 4, 56, 136, 56, 4, 0}
+constexpr unsigned BL5_T0 = 14u | 62u << 8 | 104u << 16 | 62u << 24, BL5_T4 = 14u;    // BinaryDescriptor: {14, 62, 104, 62, 14}
+
+// bytes s .. s+3 of the 12-byte string w0:w1:w2 (bytes past the string read as 0)
+__device__ __forceinline__ unsigned byte_window(unsigned w0, unsigned w1, unsigned w2, int s) {
+    return s < 4 ? __funnelshift_r(w0, w1, 8 * s) : s < 8 ? __funnelshift_r(w1, w2, 8 * (s - 4)) : w2 >> (8 * (s - 8));
+}
+
+// Horizontal pass over the staged box: s_h[r][c] = sum_t k_t in[r + ROFF][c + SH + t] (u16), for PH_H rows and PB_W columns.
+template <int SH, int ROFF>
+__device__ __forceinline__ void prep_hpass(const unsigned* s_in, unsigned short* s_h, unsigned T0, unsigned T4) {
+    for (int i = threadIdx.x; i < PH_H * (PB_W / 4); i += PT_NT) {
+        const int r = i / (PB_W / 4), c4 = i - r * (PB_W / 4);
+        const unsigned* w = s_in + (r + ROFF) * (PI_W / 4) + c4;
+        const unsigned w0 = w[0], w1 = w[1], w2 = w[2];
+        unsigned o[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) o[k] = __dp4a(byte_window(w0, w1, w2, SH + k), T0, __dp4a(byte_window(w0, w1, w2, SH + k + 4), T4, 0u));
+        *reinterpret_cast<uint2*>(s_h + r * PB_W + 4 * c4) = make_uint2(o[0] | o[1] << 16, o[2] | o[3] << 16);
+    }
+}
+
+// Vertical pass: s_b[r][c] = (sum_t k_t s_h[r + t][c] + 32768) >> 16, for PB_H rows and PB_W columns.
+__device__ __forceinline__ void prep_vpass(const unsigned short* s_h, uint8_t* s_b, unsigned T0, unsigned T4) {
+    const unsigned C01 = T0 & 0xffffu, C23 = T0 >> 16, C4L = T4, C4H = T4 << 8;
+    for (int i = threadIdx.x; i < PB_H * (PB_W / 4); i += PT_NT) {
+        const int r = i / (PB_W / 4), c4 = i - r * (PB_W / 4);
+        const uint2* p = reinterpret_cast<const uint2*>(s_h + r * PB_W) + c4;
+        const uint2 h0 = p[0], h1 = p[PB_W / 4], h2 = p[2 * (PB_W / 4)], h3 = p[3 * (PB_W / 4)], h4 = p[4 * (PB_W / 4)];
+        // __byte_perm(a, b, 0x5410) pairs the low halves of rows a, b (column 2m), 0x7632 the high halves (column 2m + 1)
+        const unsigned a0 = __dp2a_lo(__byte_perm(h0.x, h1.x, 0x5410), C01, __dp2a_lo(__byte_perm(h2.x, h3.x, 0x5410), C23, __dp2a_lo(h4.x, C4L, 32768u)));
+        const unsigned a1 = __dp2a_lo(__byte_perm(h0.x, h1.x, 0x7632), C01, __dp2a_lo(__byte_perm(h2.x, h3.x, 0x7632), C23, __dp2a_lo(h4.x, C4H, 32768u)));
+        const unsigned a2 = __dp2a_lo(__byte_perm(h0.y, h1.y, 0x5410), C01, __dp2a_lo(__byte_perm(h2.y, h3.y, 0x5410), C23, __dp2a_lo(h4.y, C4L, 32768u)));
+        const unsigned a3 = __dp2a_lo(__byte_perm(h0.y, h1.y, 0x7632), C01, __dp2a_lo(__byte_perm(h2.y, h3.y, 0x7632), C23, __dp2a_lo(h4.y, C4H, 32768u)));
+        reinterpret_cast<unsigned*>(s_b + r * PB_W)[c4] = (a0 >> 16) | ((a1 >> 16) << 8) | ((a2 >> 16) << 16) | ((a3 >> 16) << 24);
+    }
+}
+
+// ll_angle (lsd.cpp): 2x2 gradient, level-line angle, gradient norm, max over defined pixels.  Four horizontally adjacent pixels
+// per thread and item: 9 vector stores per 4 pixels (the scalar form was limited by the memory-instruction queue, not by HBM or by
+// the trigonometry).
+__global__ void __launch_bounds__(PT_NT) k_lsd_prep(const __grid_constant__ LineGeom g, LView v, LineWs ws) {
+    __shared__ __align__(16) unsigned s_in[PI_H * (PI_W / 4)];     // staged input, reflected at the frame's borders
+    __shared__ __align__(16) unsigned short s_h[PH_H * PB_W];      // horizontal pass; then the resized box (PS_H x PS_W bytes)
+    __shared__ __align__(16) uint8_t s_b[PB_H * PB_W];             // blur5, then blur7
+    unsigned* s_sc = reinterpret_cast<unsigned*>(s_h);
+    const int tile = blockIdx.x, f = blockIdx.y, tid = threadIdx.x;
+    const int trow = tile / g.tiles_x, tcol = tile - trow * g.tiles_x;
+    const int X0 = tcol * PT_W, Y0 = trow * PT_H, SX0 = tcol * PT_SW, SY0 = trow * PT_SH;
+    {   // stage: aligned words where the view allows and the word lies inside the row, reflected bytes elsewhere
+        const uint8_t* img = v.base + f * v.frame_stride;
+        const bool aligned = (((size_t)img | (size_t)v.pitch) & 3) == 0;
+#pragma unroll 4
+        for (int i = tid; i < PI_H * (PI_W / 4); i += PT_NT) {
+            const int r = i / (PI_W / 4), x = X0 - PI_X + 4 * (i - r * (PI_W / 4));
+            const uint8_t* src = img + (long long)reflect101(Y0 - PI_Y + r, g.h) * v.pitch;
+            unsigned wv;
+            if (aligned && x >= 0 && x + 3 < g.w) wv = __ldg(reinterpret_cast<const unsigned*>(src + x));
+            else wv = (unsigned)__ldg(src + reflect101(x, g.w)) | (unsigned)__ldg(src + reflect101(x + 1, g.w)) << 8 |
+                      (unsigned)__ldg(src + reflect101(x + 2, g.w)) << 16 | (unsigned)__ldg(src + reflect101(x + 3, g.w)) << 24;
+            s_in[i] = wv;
+        }
+    }
+    __syncthreads();
+    prep_hpass<1, 0>(s_in, s_h, BL5_T0, BL5_T4);     // blur5 column c = input column X0-1+c: window X0-3+c .. X0+1+c = staged c+1 ..
+    __syncthreads();
+    prep_vpass(s_h, s_b, BL5_T0, BL5_T4);
+    __syncthreads();
+    // Sobel 3x3 of blur5 with BORDER_REFLECT_101 -> dx, dy; four pixels per item
+    for (int i = tid; i < PT_H * (PT_W / 4); i += PT_NT) {
+        const int r = i / (PT_W / 4), q = i - r * (PT_W / 4);
+        const int y = Y0 + r, x0 = X0 + 4 * q;
+        if (y >= g.h || x0 >= g.w) continue;
+        const int rows[3] = {reflect101(y - 1, g.h) - Y0 + 1, r + 1, reflect101(y + 1, g.h) - Y0 + 1};
+        int vv[3][6];                                            // columns x0-1 .. x0+4 of the three rows (blur5 column c is s_b column c-X0+1)
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            const unsigned* p = reinterpret_cast<const unsigned*>(s_b + rows[k] * PB_W) + q;
+            const unsigned a = p[0], b = p[1];
+            vv[k][0] = x0 ? a & 0xff : (a >> 16) & 0xff;         // column -1 reflects to column 1
+            vv[k][1] = (a >> 8) & 0xff; vv[k][2] = (a >> 16) & 0xff; vv[k][3] = a >> 24; vv[k][4] = b & 0xff; vv[k][5] = (b >> 8) & 0xff;
+        }
+        short dxs[4], dys[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const int x = x0 + k;
+            int m0 = vv[0][k], m1 = vv[1][k], m2 = vv[2][k], c0 = vv[0][k + 1], c2 = vv[2][k + 1], p0 = vv[0][k + 2], p1 = vv[1][k + 2], p2 = vv[2][k + 2];
+            if (x == g.w - 1) { p0 = m0; p1 = m1; p2 = m2; }    // reflect101(w) = w - 2 = x - 1
+            dxs[k] = (short)((p0 - m0) + 2 * (p1 - m1) + (p2 - m2));
+            dys[k] = (short)((m2 - m0) + 2 * (c2 - c0) + (p2 - p0));
+        }
+        const long long o = f * g.full_stride + (long long)y * g.w + x0;
+        if ((g.w & 3) == 0 && (g.full_stride & 3) == 0) {
+            *reinterpret_cast<short4*>(ws.dx + o) = make_short4(dxs[0], dxs[1], dxs[2], dxs[3]);
+            *reinterpret_cast<short4*>(ws.dy + o) = make_short4(dys[0], dys[1], dys[2], dys[3]);
+        } else {
+#pragma unroll
+            for (int k = 0; k < 4; k++) if (x0 + k < g.w) { ws.dx[o + k] = dxs[k]; ws.dy[o + k] = dys[k]; }
+        }
+    }
+    prep_hpass<2, 1>(s_in, s_h, BL7_T0, BL7_T4);     // blur7 column c = input column X0+c: window X0-2+c .. X0+2+c = staged c+2 ..
+    __syncthreads();
+    prep_vpass(s_h, s_b, BL7_T0, BL7_T4);
+    __syncthreads();
+    // cv::resize(INTER_LINEAR_EXACT) 8U, 8.8 fixed point (SURVEY.md A.6 iii): the tables hold (i0, w1).  Resized columns past the tile's
+    // one-column halo or the image are never read: they are written as 0.
+    for (int i = tid; i < PS_H * (PS_W / 4); i += PT_NT) {
+        const int r = i / (PS_W / 4), c4 = (i - r * (PS_W / 4)) * 4, y = SY0 + r;
+        unsigned o = 0;
+        if (y < g.sh) {
+            const int2 ty = __ldg(&ws.tab[g.ytab_off + y]);
+            const uint8_t* S0 = s_b + (ty.x - Y0) * PB_W;
+            const uint8_t* S1 = s_b + (min(ty.x + 1, g.h - 1) - Y0) * PB_W;
+            const int v1 = ty.y, v0 = 256 - v1;
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                const int x = SX0 + c4 + k;
+                if (c4 + k > PT_SW || x >= g.sw) continue;
+                const int2 tx = __ldg(&ws.tab[g.xtab_off + x]);
+                const int i0 = tx.x - X0, i1 = min(tx.x + 1, g.w - 1) - X0, w1 = tx.y, w0 = 256 - w1;
+                const int r0 = w0 * S0[i0] + w1 * S0[i1], r1 = w0 * S1[i0] + w1 * S1[i1];
+                o |= (unsigned)((v0 * r0 + v1 * r1 + 32768) >> 16) << (8 * k);
+            }
+        }
+        s_sc[i] = o;
+    }
+    __syncthreads();
     unsigned long long bits = 0ull;                    // max gradient norm of the defined pixels (positive doubles order like integers)
-    if (x0 < g.sw && y < g.sh) {
+    for (int i = tid; i < PT_SH * (PT_SW / 4); i += PT_NT) {
+        const int r = i / (PT_SW / 4), q = i - r * (PT_SW / 4);
+        const int x0 = SX0 + 4 * q, y = SY0 + r;
+        if (x0 >= g.sw || y >= g.sh) continue;
         float ang[4]; float2 cs[4], cs0[4]; double norm[4];
-        const uint8_t* p = ws.scaled + f * g.scaled_stride + (long long)y * g.spitch + x0;
         unsigned r0 = 0, r1 = 0; int e0 = 0, e1 = 0;    // rows y, y+1: bytes x0..x0+3 and x0+4
         const bool row_ok = y < g.sh - 1;
         if (row_ok) {
-            r0 = *reinterpret_cast<const unsigned*>(p); r1 = *reinterpret_cast<const unsigned*>(p + g.spitch);   // spitch % 64 == 0, x0 % 4 == 0
-            if (x0 + 4 < g.sw) { e0 = p[4]; e1 = p[g.spitch + 4]; }
+            const unsigned* p = s_sc + r * (PS_W / 4) + q;
+            r0 = p[0]; r1 = p[PS_W / 4]; e0 = p[1] & 0xff; e1 = p[PS_W / 4 + 1] & 0xff;
         }
 #pragma unroll
         for (int k = 0; k < 4; k++) {
@@ -251,7 +315,7 @@ __global__ void __launch_bounds__(SEED_WARPS * 32) k_lsd_seeds(const __grid_cons
     __shared__ int s_warp[33];
     constexpr int NT = SEED_WARPS * 32, BPT = NBINS / NT;   // bins per thread in the prefix step
     const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    // a pixel is defined (angle != NOTDEF) exactly when its gradient norm exceeds rho (k_ll_angle): one array to read
+    // a pixel is defined (angle != NOTDEF) exactly when its gradient norm exceeds rho (k_lsd_prep): one array to read
     const double* mod = ws.modgrad + f * g.pix_stride;
     const double mg = __longlong_as_double((long long)ws.maxgrad[f]), rho = g.rho;
     const double bin_coef = (mg > 0) ? double(NBINS - 1) / mg : 0;
@@ -2675,42 +2739,6 @@ __global__ void __launch_bounds__(256) k_keylines(const __grid_constant__ LineGe
     if (tid == 0) ws.nl[f] = keep;
 }
 
-// Sobel 3x3 -> s16 (dx, dy) with BORDER_REFLECT_101 on the 5-tap blurred image.  Four pixels per thread: three
-// aligned 32-bit row loads (+ the two edge bytes) and two 8-byte stores instead of 8 byte loads and 2 short stores per pixel.
-__global__ void __launch_bounds__(256) k_sobel(const __grid_constant__ LineGeom g, LineWs ws) {
-    const int x0 = (blockIdx.x * 32 + threadIdx.x) * 4, y = blockIdx.y * 8 + threadIdx.y, f = blockIdx.z;
-    if (x0 >= g.w || y >= g.h) return;
-    const uint8_t* img = ws.blur5 + f * g.blur_stride;
-    const uint8_t* rows[3] = {img + (long long)reflect101(y - 1, g.h) * g.bpitch, img + (long long)y * g.bpitch, img + (long long)reflect101(y + 1, g.h) * g.bpitch};
-    const int xl = reflect101(x0 - 1, g.w);
-    int v[3][6];                                             // columns x0-1 .. x0+4 of the three rows
-#pragma unroll
-    for (int r = 0; r < 3; r++) {
-        const unsigned wv = *reinterpret_cast<const unsigned*>(rows[r] + x0);     // bpitch % 64 == 0, x0 % 4 == 0; x0+3 < bpitch
-        v[r][0] = rows[r][xl];
-        v[r][1] = wv & 0xff; v[r][2] = (wv >> 8) & 0xff; v[r][3] = (wv >> 16) & 0xff; v[r][4] = wv >> 24;
-        v[r][5] = rows[r][reflect101(min(x0 + 4, g.w), g.w)];
-    }
-    // pixels beyond the last column (only when w % 4 != 0) take the reflected neighbours the scalar definition uses
-    short dxs[4], dys[4];
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        const int x = x0 + k;
-        int m0 = v[0][k], m1 = v[1][k], m2 = v[2][k], c0 = v[0][k + 1], c2 = v[2][k + 1], p0 = v[0][k + 2], p1 = v[1][k + 2], p2 = v[2][k + 2];
-        if (x == g.w - 1) { p0 = m0; p1 = m1; p2 = m2; }    // reflect101(w) = w - 2 = x - 1
-        dxs[k] = (short)((p0 - m0) + 2 * (p1 - m1) + (p2 - m2));
-        dys[k] = (short)((m2 - m0) + 2 * (c2 - c0) + (p2 - p0));
-    }
-    const long long o = f * g.full_stride + (long long)y * g.w + x0;
-    if ((g.w & 3) == 0 && (g.full_stride & 3) == 0) {
-        *reinterpret_cast<short4*>(ws.dx + o) = make_short4(dxs[0], dxs[1], dxs[2], dxs[3]);
-        *reinterpret_cast<short4*>(ws.dy + o) = make_short4(dys[0], dys[1], dys[2], dys[3]);
-    } else {
-#pragma unroll
-        for (int k = 0; k < 4; k++) if (x0 + k < g.w) { ws.dx[o + k] = dxs[k]; ws.dy[o + k] = dys[k]; }
-    }
-}
-
 // LBD (BinaryDescriptor::computeLBD, binary_descriptor.cpp) — one CTA (64 threads) per line: thread h walks row h
 // of the 63-row line support region sequentially (float sums keep the reference's order), thread 0 folds the rows
 // into the 9 bands in row order, then builds the 72-float vector and the 32 pair-comparison bytes.
@@ -2854,13 +2882,11 @@ void lmark(sslpl_line* h, const char* name) {
 void make_geometry(const sslpl_line* h, int W, int H, LineGeom& g, std::vector<int2>* tab) {
     memset(&g, 0, sizeof(g));
     g.w = W; g.h = H; g.pitch = (int)align_up(W, 16);
-    g.bpitch = (int)align_up(W, 64);
-    g.sw = (int)lrint(W * 0.8); g.sh = (int)lrint(H * 0.8); g.spitch = (int)align_up(g.sw, 64);
-    g.tiles_x = (W + LT_W - 1) / LT_W; g.tiles_y = (H + LT_H - 1) / LT_H;
+    g.sw = (int)lrint(W * 0.8); g.sh = (int)lrint(H * 0.8);
+    // a tile covers PT_W x PT_H input and PT_SW x PT_SH detection-scale pixels (both counts agree for every size; max() for clarity)
+    g.tiles_x = std::max((W + PT_W - 1) / PT_W, (g.sw + PT_SW - 1) / PT_SW); g.tiles_y = std::max((H + PT_H - 1) / PT_H, (g.sh + PT_SH - 1) / PT_SH);
     g.xtab_off = 0; g.ytab_off = g.sw;
     g.in_stride = (long long)g.pitch * H;
-    g.blur_stride = (long long)align_up((size_t)g.bpitch * H, 256);
-    g.scaled_stride = (long long)align_up((size_t)g.spitch * g.sh, 256);
     g.pix_stride = (long long)g.sw * g.sh;
     g.full_stride = (long long)W * H;
     g.kl_cap = h->p.lsdNFeatures;
@@ -2893,8 +2919,6 @@ void make_geometry(const sslpl_line* h, int W, int H, LineGeom& g, std::vector<i
 void carve(sslpl_line* h, Arena& A, const LineGeom& g, int B) {
     LineWs& ws = h->ws;
     h->d_input = A.take<uint8_t>((size_t)B * g.in_stride + 256);
-    ws.blur7 = A.take<uint8_t>((size_t)B * g.blur_stride); ws.blur5 = A.take<uint8_t>((size_t)B * g.blur_stride);
-    ws.scaled = A.take<uint8_t>((size_t)B * g.scaled_stride);
     ws.angdeg = A.take<float>((size_t)B * g.pix_stride); ws.pix = A.take<LPix>((size_t)B * g.pix_stride);
     ws.modgrad = A.take<double>((size_t)B * g.pix_stride); ws.cs0 = A.take<float2>((size_t)B * g.pix_stride);
     ws.maxgrad = A.take<unsigned long long>(B);
@@ -2950,17 +2974,11 @@ int configure(sslpl_line* h, int W, int H) {
 int run_pipeline(sslpl_line* h, int B) {
     const LineGeom& g = h->g;
     cudaStream_t st = h->stream;
-    const Taps7 t7 = {{0, 4, 56, 136, 56, 4, 0}};       // GaussianBlur(sigma 0.6/0.8) of lsd.cpp, 4.13 fixed point
-    const Taps7 t5 = {{0, 14, 62, 104, 62, 14, 0}};     // GaussianBlur(5x5, sigma 1) of BinaryDescriptor
-    const dim3 tiles(g.tiles_x * g.tiles_y, B);
     h->ev_n = 0;
     lmark(h, "start");
-    k_sep7<<<tiles, 256, 0, st>>>(g, h->view, h->ws.blur7, h->ws.blur5, g.blur_stride, t7, t5);      // both blurs from one staged tile
-    k_resize_exact<<<dim3((g.sw + 31) / 32, (g.sh + 7) / 8, B), dim3(32, 8), 0, st>>>(g, h->ws);
-    lmark(h, "lsd_prep");
     SSLPL_CUDA(cudaMemsetAsync(h->ws.maxgrad, 0, sizeof(unsigned long long) * B, st));
-    k_ll_angle<<<dim3((g.sw + 127) / 128, (g.sh + 7) / 8, B), dim3(32, 8), 0, st>>>(g, h->ws);
-    lmark(h, "lsd_ll_angle");
+    k_lsd_prep<<<dim3(g.tiles_x * g.tiles_y, B), PT_NT, 0, st>>>(g, h->view, h->ws);      // blurs, resize, ll_angle, Sobel
+    lmark(h, "lsd_prep");
     k_lsd_seeds<<<B, SEED_WARPS * 32, 0, st>>>(g, h->ws);
     lmark(h, "lsd_seeds");
     SSLPL_CUDA(cudaMemsetAsync(h->ws.rejctl, 0, 4 * sizeof(int), st));
@@ -2995,10 +3013,9 @@ int run_pipeline(sslpl_line* h, int B) {
     k_lsd_nfa_improve<<<std::min(h->sm_count * 8, (B * 64 + 3) / 4), 128, 0, st>>>(g, h->ws);
     lmark(h, "lsd_nfa");
     k_keylines<<<B, 256, 0, st>>>(g, h->ws);
-    k_sobel<<<dim3((g.w + 127) / 128, (g.h + 7) / 8, B), dim3(32, 8), 0, st>>>(g, h->ws);
     k_lbd<<<dim3(g.kl_cap, B), 64, 0, st>>>(g, h->ws, h->coef);
     lmark(h, "keylines_lbd");
-    h->launches += 11;     // kernels only (the two small memsets are not counted)
+    h->launches += 8;      // kernels only (the three small memsets are not counted)
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }

@@ -167,6 +167,8 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 // Watchdog: a copy still pending after 20 s of wall time is mis-programmed, and the CTA traps instead of hanging the GPU.  The
 // bound is a time, not a number of polls: an H100 polls fast, and on a GPU shared with other processes (time slices) or crowded
 // with resident LSD walkers a correct copy can outlast any fixed count of polls that is short enough to matter.
+// %globaltimer follows the host's clock and can step (backwards too) while a CTA waits: the watchdog sums the small forward increments
+// between consecutive polls, so a step of the clock is never counted as waiting time (a backward step used to wrap t - t0 and trap).
 __device__ __forceinline__ uint64_t global_ns() {
     uint64_t t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -174,14 +176,16 @@ __device__ __forceinline__ uint64_t global_ns() {
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     uint32_t ok = 0;
-    uint64_t t0 = 0;
+    uint64_t last = 0, waited = 0;
     for (unsigned spin = 1; !ok; spin++) {
         asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}\n"
                      : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
         if (!ok && (spin & 1023u) == 0) {
             const uint64_t t = global_ns();
-            if (t0 == 0) t0 = t;
-            else if (t - t0 > 20000000000ull) __trap();
+            const long long dt = (long long)(t - last);
+            if (last != 0 && dt > 0 && dt < 1000000000ll) waited += (uint64_t)dt;
+            last = t;
+            if (waited > 20000000000ull) __trap();
         }
     }
 }
