@@ -331,6 +331,16 @@ int  sslpl_line_download_segments(sslpl_line* h, int frame, float* seg4, int cap
 /* debug: with SSLPL_LINE_TRACE=1 in the environment at create time, one row of 10 doubles per LSD region that reached
    region2rect: seed pixel, size before/after refine, log_nfa, x1,y1,x2,y2,width,p (detection scale) */
 int  sslpl_line_debug_trace(sslpl_line* h, int frame, double* out, int cap_rows, int* n);
+/* debug: the per-pixel pre-pass of frame f of the last call (waits for the handle's stream).  Input resolution w x hgt: Sobel dx, dy.
+   Detection scale sw x sh: level-line angle in degrees (-1024 = NOTDEF), pix_cs[2 per pixel] = (float)cos / sin of (float)(angle in
+   radians), cs0[2 per pixel] = float(cos / sin) of the angle in radians as double, gradient norm, *maxgrad = largest norm of a defined
+   pixel (0 when none), seeds = defined pixel indices (y * sw + x) by descending gradient bin, raster order inside a bin (room for sw * sh
+   entries), *nseeds.  Any output pointer may be NULL.  Region growing changes none of these, so they stay valid after a full call. */
+int  sslpl_line_download_prep(sslpl_line* h, int frame, int* w, int* hgt, int* sw, int* sh, int16_t* dx, int16_t* dy, float* angdeg,
+                              float* pix_cs, float* cs0, double* modgrad, double* maxgrad, uint32_t* seeds, int* nseeds);
+/* debug: the pre-pass's per-pixel ll_angle arithmetic on every 2x2 difference pair (DA = D - A, BC = B - C, each in [-255, 255]),
+   entry (DA + 255) * 511 + (BC + 255): 261121 angles, cs / cs0 pairs and norms, as in sslpl_line_download_prep.  NULL = skip. */
+int  sslpl_line_debug_ll_table(sslpl_line* h, float* angdeg, float* cs, float* cs0, double* modgrad);
 
 /* =====================================================================================
  * (4) Frame level — what Frame::Frame(imGray, ...) does with the two extractors (src/Frame.cc:69-131), the colour conversion in

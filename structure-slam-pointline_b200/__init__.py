@@ -813,6 +813,28 @@ class LineSegment:
         _check(lib().sslpl_line_download_segments(self._h, frame, _p(seg), cap, C.byref(n)))
         return seg[:min(n.value, cap)].copy()
 
+    def prep_planes(self, frame=0):
+        """Per-pixel pre-pass of `frame` of the last call: dict(dx, dy [h, w] int16; angdeg [sh, sw] float32 (-1024 = NOTDEF);
+        cs, cs0 [sh, sw, 2] float32; modgrad [sh, sw] float64; maxgrad float; seeds uint32 pixel indices y * sw + x)."""
+        w, h, sw, sh, ns = C.c_int(), C.c_int(), C.c_int(), C.c_int(), C.c_int()
+        _check(lib().sslpl_line_download_prep(self._h, frame, C.byref(w), C.byref(h), C.byref(sw), C.byref(sh), *([None] * 9)))
+        W, H, SW, SH = w.value, h.value, sw.value, sh.value
+        dx = np.empty((H, W), np.int16); dy = np.empty((H, W), np.int16); ang = np.empty((SH, SW), np.float32)
+        cs = np.empty((SH, SW, 2), np.float32); cs0 = np.empty((SH, SW, 2), np.float32); mod = np.empty((SH, SW), np.float64)
+        mg = C.c_double(); seeds = np.empty(max(SW * SH, 1), np.uint32)
+        _check(lib().sslpl_line_download_prep(self._h, frame, None, None, None, None, _p(dx), _p(dy), _p(ang), _p(cs), _p(cs0), _p(mod),
+                                              C.byref(mg), _p(seeds), C.byref(ns)))
+        return dict(dx=dx, dy=dy, angdeg=ang, cs=cs, cs0=cs0, modgrad=mod, maxgrad=mg.value, seeds=seeds[:ns.value].copy())
+
+    def ll_table(self):
+        """The pre-pass's ll_angle arithmetic on every 2x2 difference pair: arrays [511, 511] indexed [DA + 255, BC + 255]
+        (angdeg, modgrad) and [511, 511, 2] (cs, cs0)."""
+        n = 511
+        ang = np.empty((n, n), np.float32); cs = np.empty((n, n, 2), np.float32); cs0 = np.empty((n, n, 2), np.float32)
+        mod = np.empty((n, n), np.float64)
+        _check(lib().sslpl_line_debug_ll_table(self._h, _p(ang), _p(cs), _p(cs0), _p(mod)))
+        return dict(angdeg=ang, cs=cs, cs0=cs0, modgrad=mod)
+
     def set_max_walkers(self, n):
         _check(lib().sslpl_line_set_max_walkers(self._h, int(n)))
 

@@ -149,7 +149,32 @@ __device__ __forceinline__ void prep_vpass(const unsigned short* s_h, uint8_t* s
     }
 }
 
-// ll_angle (lsd.cpp): 2x2 gradient, level-line angle, gradient norm, max over defined pixels.  Four horizontally adjacent pixels
+// ll_angle (lsd.cpp) of one pixel from its 2x2 differences DA = D - A, BC = B - C: the gradient norm and, where it exceeds rho, the
+// level-line angle in degrees (NOTDEF_F elsewhere), (float)cos / sin of (float)(angle in radians) — the values region_grow sums — and
+// float(cos / sin) of the angle in radians taken as double — region_grow's seed values (both 0 where undefined).  k_lsd_prep and the
+// debug table k_ll_table both evaluate it, so the table checks the kernel's own arithmetic.
+struct LLPix { double norm; float ang; float2 cs, cs0; };
+__device__ __forceinline__ LLPix ll_pixel(int DA, int BC, double rho) {
+    LLPix o;
+    o.ang = NOTDEF_F; o.cs = make_float2(0.f, 0.f); o.cs0 = make_float2(0.f, 0.f);
+    const int gx = DA + BC, gy = DA - BC;
+    o.norm = sqrt((double)(gx * gx + gy * gy) / 4.0);
+    if (o.norm > rho) {
+        o.ang = fast_atan2_deg((float)gx, (float)-gy);
+        const double ad = (double)o.ang * L_DEG;
+        double sn, cn;
+        l_sincos_2pi((double)(float)ad, &sn, &cn);
+        o.cs = make_float2((float)cn, (float)sn);
+        // region_grow's seed values float(cos(ad)), float(sin(ad)) get their own reduction.  A second-order Taylor step from (cn, sn)
+        // is accurate to a few double ulps in absolute terms only: near a zero of cos or sin (90 and 180 degrees) that is a relative
+        // error of ~1e-7, which survives the narrowing to float.  (Redoing the reduction only there was slower: more registers.)
+        l_sincos_2pi(ad, &sn, &cn);
+        o.cs0 = make_float2((float)cn, (float)sn);
+    }
+    return o;
+}
+
+// ll_angle over the tile: 2x2 gradient, level-line angle, gradient norm, max over defined pixels.  Four horizontally adjacent pixels
 // per thread and item: 9 vector stores per 4 pixels (the scalar form was limited by the memory-instruction queue, not by HBM or by
 // the trigonometry).
 __global__ void __launch_bounds__(PT_NT) k_lsd_prep(const __grid_constant__ LineGeom g, LView v, LineWs ws) {
@@ -253,25 +278,14 @@ __global__ void __launch_bounds__(PT_NT) k_lsd_prep(const __grid_constant__ Line
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             ang[k] = NOTDEF_F; cs[k] = make_float2(0.f, 0.f); cs0[k] = make_float2(0.f, 0.f); norm[k] = 0;
-            if (row_ok && x0 + k < g.sw - 1) {
+            if (row_ok && x0 + k < g.sw - 1) {      // the last row and column stay NOTDEF with norm 0 (lsd.cpp)
                 const int A = (r0 >> (8 * k)) & 0xff, C = (r1 >> (8 * k)) & 0xff;
                 const int Bv = (k < 3) ? (int)((r0 >> (8 * k + 8)) & 0xff) : e0, D = (k < 3) ? (int)((r1 >> (8 * k + 8)) & 0xff) : e1;
-                const int DA = D - A, BC = Bv - C;
-                const int gx = DA + BC, gy = DA - BC;
-                norm[k] = sqrt((double)(gx * gx + gy * gy) / 4.0);
-                if (norm[k] > g.rho) {
-                    const unsigned long long nb = (unsigned long long)__double_as_longlong(norm[k]);
+                const LLPix p = ll_pixel(D - A, Bv - C, g.rho);
+                norm[k] = p.norm; ang[k] = p.ang; cs[k] = p.cs; cs0[k] = p.cs0;
+                if (p.norm > g.rho) {
+                    const unsigned long long nb = (unsigned long long)__double_as_longlong(p.norm);
                     bits = nb > bits ? nb : bits;
-                    ang[k] = fast_atan2_deg((float)gx, (float)-gy);
-                    const double ad = (double)ang[k] * L_DEG;
-                    const float a = (float)ad;
-                    double sn, cn;
-                    l_sincos_2pi((double)a, &sn, &cn);
-                    cs[k].x = (float)cn; cs[k].y = (float)sn;
-                    // region_grow's seed values float(cos(ad)), float(sin(ad)): ad = a + d with |d| < 2e-7, so a second-order
-                    // Taylor step from (cn, sn) is accurate to a few double ulps (the d^3 term is < 1e-20) — one sincos, not four calls
-                    const double d = ad - (double)a, hd2 = 0.5 * d * d;
-                    cs0[k].x = (float)(cn - sn * d - cn * hd2); cs0[k].y = (float)(sn + cn * d - sn * hd2);
                 }
             }
         }
@@ -297,6 +311,15 @@ __global__ void __launch_bounds__(PT_NT) k_lsd_prep(const __grid_constant__ Line
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) { const unsigned long long t = __shfl_xor_sync(0xffffffffu, bits, o); bits = t > bits ? t : bits; }
     if ((threadIdx.x & 31) == 0 && bits) atomicMax(ws.maxgrad + f, bits);
+}
+
+// Debug (sslpl_line_debug_ll_table): ll_pixel on every (DA, BC) in [-255, 255]^2, entry (DA + 255) * LL_SPAN + (BC + 255).
+constexpr int LL_SPAN = 511;
+__global__ void k_ll_table(double rho, float* ang, float2* cs, float2* cs0, double* norm) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= LL_SPAN * LL_SPAN) return;
+    const LLPix p = ll_pixel(i / LL_SPAN - 255, i % LL_SPAN - 255, rho);
+    ang[i] = p.ang; cs[i] = p.cs; cs0[i] = p.cs0; norm[i] = p.norm;
 }
 
 __device__ __forceinline__ int lsd_bin(double norm, double max_grad) {
@@ -2879,6 +2902,9 @@ void lmark(sslpl_line* h, const char* name) {
     cudaEventRecord(h->ev[h->ev_n++], h->stream);
 }
 
+// gradient threshold of lsd.cpp: quant / sin(ang_th) with quant 2, ang_th 22.5 degrees
+double lsd_rho() { return 2.0 / std::sin(L_PI * 22.5 / 180); }
+
 void make_geometry(const sslpl_line* h, int W, int H, LineGeom& g, std::vector<int2>* tab) {
     memset(&g, 0, sizeof(g));
     g.w = W; g.h = H; g.pitch = (int)align_up(W, 16);
@@ -2891,7 +2917,7 @@ void make_geometry(const sslpl_line* h, int W, int H, LineGeom& g, std::vector<i
     g.full_stride = (long long)W * H;
     g.kl_cap = h->p.lsdNFeatures;
     // lsd.cpp constants (ANG_TH 22.5, QUANT 2.0); host libm, exactly as the CPU implementation evaluates them
-    g.prec = L_PI * 22.5 / 180; g.p = 22.5 / 180; g.rho = 2.0 / std::sin(g.prec);
+    g.prec = L_PI * 22.5 / 180; g.p = 22.5 / 180; g.rho = lsd_rho();
     g.log_nt = 5 * (std::log10(double(g.sw)) + std::log10(double(g.sh))) / 2 + std::log10(11.0);
     g.min_reg_size = (int)size_t(-g.log_nt / std::log10(g.p));
     g.seg_cap = (int)(g.pix_stride / std::max(g.min_reg_size, 1)) + 16;
@@ -3181,6 +3207,58 @@ int sslpl_line_download_segments(sslpl_line* h, int frame, float* seg4, int cap,
     return SSLPL_OK;
 }
 
+// Region growing changes only LPix.used after k_lsd_prep / k_lsd_seeds, so these planes are still the pre-pass's after a full call.
+int sslpl_line_download_prep(sslpl_line* h, int frame, int* w, int* hgt, int* sw, int* sh, int16_t* dx, int16_t* dy, float* angdeg,
+                             float* pix_cs, float* cs0, double* modgrad, double* maxgrad, uint32_t* seeds, int* nseeds) {
+    SSLPL_REQUIRE(h && frame >= 0 && frame < h->cur_frames, SSLPL_ERR_ARG, "bad argument");
+    SSLPL_CUDA(cudaSetDevice(h->p.device));
+    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
+    const LineGeom& g = h->g;
+    const size_t np = (size_t)g.pix_stride, nf = (size_t)g.full_stride, po = (size_t)frame * np, fo = (size_t)frame * nf;
+    if (w) *w = g.w;
+    if (hgt) *hgt = g.h;
+    if (sw) *sw = g.sw;
+    if (sh) *sh = g.sh;
+    if (dx) SSLPL_CUDA(cudaMemcpy(dx, h->ws.dx + fo, nf * sizeof(int16_t), cudaMemcpyDeviceToHost));
+    if (dy) SSLPL_CUDA(cudaMemcpy(dy, h->ws.dy + fo, nf * sizeof(int16_t), cudaMemcpyDeviceToHost));
+    if (angdeg) SSLPL_CUDA(cudaMemcpy(angdeg, h->ws.angdeg + po, np * sizeof(float), cudaMemcpyDeviceToHost));
+    if (pix_cs) SSLPL_CUDA(cudaMemcpy2D(pix_cs, 2 * sizeof(float), &h->ws.pix[po].cx, sizeof(LPix), 2 * sizeof(float), np, cudaMemcpyDeviceToHost));
+    if (cs0) SSLPL_CUDA(cudaMemcpy(cs0, h->ws.cs0 + po, np * sizeof(float2), cudaMemcpyDeviceToHost));
+    if (modgrad) SSLPL_CUDA(cudaMemcpy(modgrad, h->ws.modgrad + po, np * sizeof(double), cudaMemcpyDeviceToHost));
+    if (maxgrad) {
+        unsigned long long bits = 0;
+        SSLPL_CUDA(cudaMemcpy(&bits, h->ws.maxgrad + frame, sizeof(bits), cudaMemcpyDeviceToHost));
+        memcpy(maxgrad, &bits, sizeof(double));
+    }
+    int cnt = 0;
+    SSLPL_CUDA(cudaMemcpy(&cnt, h->ws.nseeds + frame, sizeof(int), cudaMemcpyDeviceToHost));
+    if (seeds && cnt > 0) SSLPL_CUDA(cudaMemcpy(seeds, h->ws.seeds + po, (size_t)cnt * sizeof(unsigned), cudaMemcpyDeviceToHost));
+    if (nseeds) *nseeds = cnt;
+    return SSLPL_OK;
+}
+
+int sslpl_line_debug_ll_table(sslpl_line* h, float* angdeg, float* cs, float* cs0, double* modgrad) {
+    SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle");
+    SSLPL_CUDA(cudaSetDevice(h->p.device));
+    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
+    constexpr size_t N = (size_t)LL_SPAN * LL_SPAN;
+    uint8_t* buf = nullptr;
+    SSLPL_CUDA(cudaMalloc(&buf, N * (sizeof(float) + 2 * sizeof(float2) + sizeof(double))));
+    double* d_norm = reinterpret_cast<double*>(buf);
+    float2* d_cs = reinterpret_cast<float2*>(d_norm + N);
+    float2* d_cs0 = d_cs + N;
+    float* d_ang = reinterpret_cast<float*>(d_cs0 + N);
+    k_ll_table<<<(unsigned)((N + 255) / 256), 256, 0, h->stream>>>(lsd_rho(), d_ang, d_cs, d_cs0, d_norm);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    if (e == cudaSuccess && angdeg) e = cudaMemcpy(angdeg, d_ang, N * sizeof(float), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && cs) e = cudaMemcpy(cs, d_cs, N * sizeof(float2), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && cs0) e = cudaMemcpy(cs0, d_cs0, N * sizeof(float2), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && modgrad) e = cudaMemcpy(modgrad, d_norm, N * sizeof(double), cudaMemcpyDeviceToHost);
+    cudaFree(buf);
+    SSLPL_CUDA(e);
+    return SSLPL_OK;
+}
 
 /* debug (SSLPL_LINE_TRACE=1 at handle creation): one row of 10 doubles per region that reached region2rect */
 /* Statistics of the last region-walker launch (16 values; collected with SSLPL_WALKER_DBG=32).  For the round-2a multi-warp walker as
