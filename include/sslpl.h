@@ -201,6 +201,24 @@ int  sslpl_search_by_projection_frame(sslpl_matcher* m,
         int n2, const uint8_t* d2, const float* x2, const float* y2, const int32_t* oct2, const float* angle2, const float* uright2,
         const uint8_t* claimed2, const float* Tcw, const float* Tlw, const float* cam, const float* bounds,
         const float* scaleFactors, int nlevels, float th, int bMono, int checkOrientation, int32_t* assign2, int* nmatches);
+/* The same matcher over consecutive frames resident in HBM, monocular (bMono = true), asynchronous on the handle's stream like
+   sslpl_match_bow_batch_device.  Pair p (npairs = nframes - 1) is what Tracking::TrackWithMotionModel (Tracking.cc:1204-1244) runs with
+   frame p as LastFrame and frame p + 1 as CurrentFrame: CurrentFrame.mvpMapPoints starts all NULL (:1219), ORBmatcher::SearchByProjection
+   (ORBmatcher.cc:1331-1473) runs with th, and when retry_below > 0 and it found fewer than retry_below matches (the reference: 20) it runs
+   again from NULL with 2 * th (:1240-1244).
+   Per frame f, `cap` entries each: d_kps = mvKeysUn (e.g. sslpl_orb_device_results, or sslpl_frame_device_keypoints_un with
+   distortion), d_desc, d_n[f] (clamped to cap); d_Xw[f][cap][3] = GetWorldPos() of feature i's MapPoint; d_mpflag[f][cap]: bit0 =
+   mvpMapPoints[i] && !mvbOutlier[i], bit1 = Observations() > 0; d_dmp[f][cap][32] = the MapPoints' descriptors (NULL = the frame's own
+   d_desc); d_Tcw[f][12] = 3x4 row-major pose (pair p projects with frame p + 1's).  Host: cam = {fx, fy, cx, cy}, bounds = {mnMinX,
+   mnMaxX, mnMinY, mnMaxY}, scaleFactors[nlevels] (nlevels <= 32).  A last-frame point whose octave is outside [0, nlevels) is skipped.
+   Result: d_assign[p][cap] as assign2 above for frame p + 1's features (-1 also past d_n), d_nmatch[p] = the final count.
+   Needs nframes <= max_batch + 1 and cap <= max_features + 64; the first call allocates a workspace of that size, freed with the
+   handle.  Bad arguments return SSLPL_ERR_ARG and enqueue nothing. */
+int  sslpl_search_by_projection_frame_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nframes, int cap,
+        const float* d_Xw, const uint8_t* d_mpflag, const uint8_t* d_dmp, const float* d_Tcw,
+        const float* cam, const float* bounds, const float* scaleFactors, int nlevels, float th, int checkOrientation, int retry_below,
+        int32_t* d_assign, int32_t* d_nmatch);
 
 /* ---- ORBmatcher::SearchByProjection(Frame &F, const vector<MapPoint*> &vpMapPoints, th) (ORBmatcher.cc:45-129): the matcher of
    Tracking::SearchLocalPoints (Tracking.cc:1736), run on every frame.  Per MapPoint, in vector order, what Frame::isInFrustum left on
@@ -374,6 +392,10 @@ int  sslpl_frame_extract_batch_begin(sslpl_frame* h, const uint8_t* imgs, int nf
 int  sslpl_frame_sync(sslpl_frame* h);
 void* sslpl_frame_stream(sslpl_frame* h, int which /* 0 = ORB stream, 1 = line stream */);
 int  sslpl_frame_device_gray(sslpl_frame* h, const uint8_t** d_gray, int* pitch, size_t* frame_stride);
+/* mvKeysUn of the last call, in HBM ([nframes][cap], counts as in sslpl_orb_device_results): the undistorted keypoints when the camera
+   has k1 != 0 (they are computed on every call then), the ORB handle's keypoints otherwise (Frame.cc:485).  Written on the ORB stream
+   (sslpl_frame_stream(h, 0)): sync the frame, or order that stream before the consumer's. */
+int  sslpl_frame_device_keypoints_un(sslpl_frame* h, const sslpl_keypoint** d_kps_un, int* cap);
 
 #ifdef __cplusplus
 }

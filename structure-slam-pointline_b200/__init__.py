@@ -434,6 +434,21 @@ class Matcher:
         # -2 = assigned, then removed by the rotation check (the reference writes NULL there, ORBmatcher.cc:1461); -1 = never assigned
         return nm.value, (out[:n2] if raw else np.where(out[:n2] == -2, -1, out[:n2]).astype(np.int32))
 
+    def search_by_projection_frame_batch_device(self, d_kps, d_desc, d_n, nframes, cap, d_Xw, d_mpflag, d_dmp, d_Tcw, cam, bounds,
+                                                scale_factors, th, check_ori=True, retry_below=20, d_assign=0, d_nmatch=0):
+        """SearchByProjection(CurrentFrame, LastFrame, th, bMono=true) (ORBmatcher.cc:1331-1473) over consecutive frames in HBM, with
+        TrackWithMotionModel's 2 * th retry below `retry_below` matches (Tracking.cc:1240-1244; 0 = no retry).  Raw device pointers:
+        d_kps / d_desc / d_n as sslpl_orb_device_results gives them, d_Xw [nframes, cap, 3] f32, d_mpflag [nframes, cap] u8 (bit0 has
+        MapPoint and not outlier, bit1 Observations() > 0), d_dmp [nframes, cap, 32] or 0 (= d_desc), d_Tcw [nframes, 12] f32 ->
+        d_assign [nframes - 1, cap] i32 (-1 never assigned, -2 removed by the rotation check), d_nmatch [nframes - 1] i32.
+        Asynchronous on the matcher's stream."""
+        f32 = lambda a: np.ascontiguousarray(a, np.float32)
+        sf = f32(scale_factors)
+        _check(lib().sslpl_search_by_projection_frame_batch_device(
+            self._h, C.c_void_p(d_kps), C.c_void_p(d_desc), C.c_void_p(d_n), int(nframes), int(cap), C.c_void_p(d_Xw), C.c_void_p(d_mpflag),
+            C.c_void_p(d_dmp or None), C.c_void_p(d_Tcw), _p(f32(cam)[:4].copy()), _p(f32(bounds)), _p(sf), len(sf), C.c_float(th),
+            int(check_ori), int(retry_below), C.c_void_p(d_assign), C.c_void_p(d_nmatch)))
+
     def descriptor_medoid(self, desc, off):
         """ComputeDistinctiveDescriptors (MapPoint.cc:247-312 / MapLine.cpp:246-317) for CSR groups of descriptors."""
         desc = np.ascontiguousarray(desc, np.uint8).reshape(-1, 32); off = np.ascontiguousarray(off, np.int32)
@@ -693,6 +708,13 @@ class Frame:
 
     def sync(self):
         _check(lib().sslpl_frame_sync(self._h))
+
+    def device_keypoints_un(self):
+        """(device pointer, cap) of the last call's mvKeysUn: undistorted keypoints when k1 != 0, else the ORB keypoints (Frame.cc:485).
+        Counts are those of self.orb.device_results(); written on stream(0)."""
+        p = C.c_void_p(); cap = C.c_int()
+        _check(lib().sslpl_frame_device_keypoints_un(self._h, C.byref(p), C.byref(cap)))
+        return p.value, cap.value
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:

@@ -67,6 +67,7 @@ struct sslpl_frame {
     sslpl_keypoint* d_un = nullptr;                        // undistorted keypoints [max_batch][cap]
     Camera cam;
     int cap = 0, last_pitch = 0; size_t last_stride = 0;
+    bool last_undistorted = false;                         // the last call wrote mvKeysUn to d_un (k1 != 0)
     long long launches = 0;
 };
 
@@ -194,7 +195,10 @@ int sslpl_frame_extract_batch_begin(sslpl_frame* h, const uint8_t* imgs, int nfr
     const sslpl_keypoint* d_kps; const uint8_t* d_desc; const int* d_n; int c2;
     rc = sslpl_orb_device_results(h->orb, &d_kps, &d_desc, &d_n, &c2);
     if (rc != SSLPL_OK) return rc;
-    if (kps_un) {
+    // mvKeysUn: always computed with k1 != 0 (the device consumers read it through sslpl_frame_device_keypoints_un); with k1 == 0 it
+    // equals the ORB keypoints and is only copied for the host output
+    h->last_undistorted = h->cam.distorted != 0;
+    if (kps_un || h->last_undistorted) {
         k_undistort<<<dim3((c2 + 255) / 256, nframes), 256, 0, h->s_orb>>>(d_kps, d_n, c2, h->cam, h->d_un);
         h->launches++;
     }
@@ -251,6 +255,17 @@ int sslpl_frame_extract(sslpl_frame* h, const uint8_t* img, int width, int heigh
 int sslpl_frame_device_gray(sslpl_frame* h, const uint8_t** d_gray, int* pitch, size_t* frame_stride) {
     SSLPL_REQUIRE(h && d_gray, SSLPL_ERR_ARG, "null argument");
     *d_gray = h->d_gray; if (pitch) *pitch = h->last_pitch; if (frame_stride) *frame_stride = h->last_stride;
+    return SSLPL_OK;
+}
+
+/* mvKeysUn of the last call (device): d_un when it was undistorted, the ORB handle's keypoints when k1 == 0 (Frame.cc:485) */
+int sslpl_frame_device_keypoints_un(sslpl_frame* h, const sslpl_keypoint** d_kps_un, int* cap) {
+    SSLPL_REQUIRE(h && d_kps_un, SSLPL_ERR_ARG, "null argument");
+    const sslpl_keypoint* d_kps; const uint8_t* d_desc; const int* d_n; int c2;
+    const int rc = sslpl_orb_device_results(h->orb, &d_kps, &d_desc, &d_n, &c2);
+    if (rc != SSLPL_OK) return rc;
+    *d_kps_un = h->last_undistorted ? h->d_un : d_kps;
+    if (cap) *cap = c2;
     return SSLPL_OK;
 }
 
