@@ -50,6 +50,7 @@ struct __align__(16) LPix { float ang, cx, cy; unsigned used; };   // `used` = t
 struct LineWs {
     float* angdeg; LPix* pix; float2* cs0; double* modgrad;
     unsigned long long* maxgrad; unsigned* seeds; int* nseeds;
+    int* prep_next;             // k_lsd_prep's tile counter (zeroed before every launch)
     unsigned* reg;              // region pixel list (x | y << 16) of the turn holder (whole-frame capacity)
     unsigned* sreg;             // per frame: WALK_RING speculation slots x WALK_SLOT_CAP list entries (v3: one list of V3_LIST entries per worker)
     unsigned* dlist;            // v3, per frame: V3_DPOOL entries (see V3Shared::dl_off)
@@ -174,143 +175,169 @@ __device__ __forceinline__ LLPix ll_pixel(int DA, int BC, double rho) {
     return o;
 }
 
+// Stage the input box of tile (X0, Y0) of frame f into s_in: aligned words where the view allows and the word lies inside the row, as
+// 4-byte cp.async copies that complete at the next cp.async.wait_all; reflected bytes elsewhere, loaded and stored synchronously.
+// Not unrolled: a copy in flight holds no register, and unrolling took the kernel past 70 registers.
+__device__ __forceinline__ void prep_stage(unsigned* s_in, const LineGeom& g, const LView& v, int f, int X0, int Y0) {
+    const uint8_t* img = v.base + f * v.frame_stride;
+    const bool aligned = (((size_t)img | (size_t)v.pitch) & 3) == 0;
+#pragma unroll 1
+    for (int i = threadIdx.x; i < PI_H * (PI_W / 4); i += PT_NT) {
+        const int r = i / (PI_W / 4), x = X0 - PI_X + 4 * (i - r * (PI_W / 4));
+        const uint8_t* src = img + (long long)reflect101(Y0 - PI_Y + r, g.h) * v.pitch;
+        if (aligned && x >= 0 && x + 3 < g.w)
+            asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((unsigned)__cvta_generic_to_shared(s_in + i)), "l"(src + x) : "memory");
+        else s_in[i] = (unsigned)__ldg(src + reflect101(x, g.w)) | (unsigned)__ldg(src + reflect101(x + 1, g.w)) << 8 |
+                       (unsigned)__ldg(src + reflect101(x + 2, g.w)) << 16 | (unsigned)__ldg(src + reflect101(x + 3, g.w)) << 24;
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+}
+
+// A persistent tile loop: the grid holds as many CTAs as fit on the device at once (fewer when the tiles are fewer), and every CTA
+// takes tile after tile (frame-major) from the counter ws.prep_next (zeroed before every launch) until they run out.  A CTA that
+// becomes resident late finds the work taken and exits.  The next tile's input box is requested as soon as the current tile's last
+// read of s_in (blur7's horizontal pass) is done, so its load overlaps blur7's vertical pass, the resize and ll_angle.  Outputs go to
+// fixed places and maxgrad is an atomicMax: which CTA runs a tile, and in what order, changes no result.
 // ll_angle over the tile: 2x2 gradient, level-line angle, gradient norm, max over defined pixels.  Four horizontally adjacent pixels
 // per thread and item: 9 vector stores per 4 pixels (the scalar form was limited by the memory-instruction queue, not by HBM or by
 // the trigonometry).
-__global__ void __launch_bounds__(PT_NT) k_lsd_prep(const __grid_constant__ LineGeom g, LView v, LineWs ws) {
+__global__ void __launch_bounds__(PT_NT) k_lsd_prep(const __grid_constant__ LineGeom g, LView v, LineWs ws, int nframes) {
     __shared__ __align__(16) unsigned s_in[PI_H * (PI_W / 4)];     // staged input, reflected at the frame's borders
     __shared__ __align__(16) unsigned short s_h[PH_H * PB_W];      // horizontal pass; then the resized box (PS_H x PS_W bytes)
     __shared__ __align__(16) uint8_t s_b[PB_H * PB_W];             // blur5, then blur7
+    __shared__ int s_next;
     unsigned* s_sc = reinterpret_cast<unsigned*>(s_h);
-    const int tile = blockIdx.x, f = blockIdx.y, tid = threadIdx.x;
-    const int trow = tile / g.tiles_x, tcol = tile - trow * g.tiles_x;
-    const int X0 = tcol * PT_W, Y0 = trow * PT_H, SX0 = tcol * PT_SW, SY0 = trow * PT_SH;
-    {   // stage: aligned words where the view allows and the word lies inside the row, reflected bytes elsewhere
-        const uint8_t* img = v.base + f * v.frame_stride;
-        const bool aligned = (((size_t)img | (size_t)v.pitch) & 3) == 0;
-#pragma unroll 4
-        for (int i = tid; i < PI_H * (PI_W / 4); i += PT_NT) {
-            const int r = i / (PI_W / 4), x = X0 - PI_X + 4 * (i - r * (PI_W / 4));
-            const uint8_t* src = img + (long long)reflect101(Y0 - PI_Y + r, g.h) * v.pitch;
-            unsigned wv;
-            if (aligned && x >= 0 && x + 3 < g.w) wv = __ldg(reinterpret_cast<const unsigned*>(src + x));
-            else wv = (unsigned)__ldg(src + reflect101(x, g.w)) | (unsigned)__ldg(src + reflect101(x + 1, g.w)) << 8 |
-                      (unsigned)__ldg(src + reflect101(x + 2, g.w)) << 16 | (unsigned)__ldg(src + reflect101(x + 3, g.w)) << 24;
-            s_in[i] = wv;
-        }
-    }
+    const int tid = threadIdx.x, per_frame = g.tiles_x * g.tiles_y, ntiles = per_frame * nframes;
+    if (tid == 0) s_next = atomicAdd(ws.prep_next, 1);
     __syncthreads();
-    prep_hpass<1, 0>(s_in, s_h, BL5_T0, BL5_T4);     // blur5 column c = input column X0-1+c: window X0-3+c .. X0+1+c = staged c+1 ..
-    __syncthreads();
-    prep_vpass(s_h, s_b, BL5_T0, BL5_T4);
-    __syncthreads();
-    // Sobel 3x3 of blur5 with BORDER_REFLECT_101 -> dx, dy; four pixels per item
-    for (int i = tid; i < PT_H * (PT_W / 4); i += PT_NT) {
-        const int r = i / (PT_W / 4), q = i - r * (PT_W / 4);
-        const int y = Y0 + r, x0 = X0 + 4 * q;
-        if (y >= g.h || x0 >= g.w) continue;
-        const int rows[3] = {reflect101(y - 1, g.h) - Y0 + 1, r + 1, reflect101(y + 1, g.h) - Y0 + 1};
-        int vv[3][6];                                            // columns x0-1 .. x0+4 of the three rows (blur5 column c is s_b column c-X0+1)
+    int t = s_next;
+    if (t >= ntiles) return;
+    prep_stage(s_in, g, v, t / per_frame, (t % per_frame % g.tiles_x) * PT_W, (t % per_frame / g.tiles_x) * PT_H);
+    for (;;) {
+        const int f = t / per_frame, tile = t - f * per_frame;
+        const int trow = tile / g.tiles_x, tcol = tile - trow * g.tiles_x;
+        const int X0 = tcol * PT_W, Y0 = trow * PT_H, SX0 = tcol * PT_SW, SY0 = trow * PT_SH;
+        asm volatile("cp.async.wait_all;" ::: "memory");
+        __syncthreads();                                 // the staged box is complete; the previous tile is done with s_h and s_next
+        if (tid == 0) s_next = atomicAdd(ws.prep_next, 1);
+        prep_hpass<1, 0>(s_in, s_h, BL5_T0, BL5_T4);     // blur5 column c = input column X0-1+c: window X0-3+c .. X0+1+c = staged c+1 ..
+        __syncthreads();
+        prep_vpass(s_h, s_b, BL5_T0, BL5_T4);
+        __syncthreads();
+        // Sobel 3x3 of blur5 with BORDER_REFLECT_101 -> dx, dy; four pixels per item
+        for (int i = tid; i < PT_H * (PT_W / 4); i += PT_NT) {
+            const int r = i / (PT_W / 4), q = i - r * (PT_W / 4);
+            const int y = Y0 + r, x0 = X0 + 4 * q;
+            if (y >= g.h || x0 >= g.w) continue;
+            const int rows[3] = {reflect101(y - 1, g.h) - Y0 + 1, r + 1, reflect101(y + 1, g.h) - Y0 + 1};
+            int vv[3][6];                                            // columns x0-1 .. x0+4 of the three rows (blur5 column c is s_b column c-X0+1)
 #pragma unroll
-        for (int k = 0; k < 3; k++) {
-            const unsigned* p = reinterpret_cast<const unsigned*>(s_b + rows[k] * PB_W) + q;
-            const unsigned a = p[0], b = p[1];
-            vv[k][0] = x0 ? a & 0xff : (a >> 16) & 0xff;         // column -1 reflects to column 1
-            vv[k][1] = (a >> 8) & 0xff; vv[k][2] = (a >> 16) & 0xff; vv[k][3] = a >> 24; vv[k][4] = b & 0xff; vv[k][5] = (b >> 8) & 0xff;
-        }
-        short dxs[4], dys[4];
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-            const int x = x0 + k;
-            int m0 = vv[0][k], m1 = vv[1][k], m2 = vv[2][k], c0 = vv[0][k + 1], c2 = vv[2][k + 1], p0 = vv[0][k + 2], p1 = vv[1][k + 2], p2 = vv[2][k + 2];
-            if (x == g.w - 1) { p0 = m0; p1 = m1; p2 = m2; }    // reflect101(w) = w - 2 = x - 1
-            dxs[k] = (short)((p0 - m0) + 2 * (p1 - m1) + (p2 - m2));
-            dys[k] = (short)((m2 - m0) + 2 * (c2 - c0) + (p2 - p0));
-        }
-        const long long o = f * g.full_stride + (long long)y * g.w + x0;
-        if ((g.w & 3) == 0 && (g.full_stride & 3) == 0) {
-            *reinterpret_cast<short4*>(ws.dx + o) = make_short4(dxs[0], dxs[1], dxs[2], dxs[3]);
-            *reinterpret_cast<short4*>(ws.dy + o) = make_short4(dys[0], dys[1], dys[2], dys[3]);
-        } else {
-#pragma unroll
-            for (int k = 0; k < 4; k++) if (x0 + k < g.w) { ws.dx[o + k] = dxs[k]; ws.dy[o + k] = dys[k]; }
-        }
-    }
-    prep_hpass<2, 1>(s_in, s_h, BL7_T0, BL7_T4);     // blur7 column c = input column X0+c: window X0-2+c .. X0+2+c = staged c+2 ..
-    __syncthreads();
-    prep_vpass(s_h, s_b, BL7_T0, BL7_T4);
-    __syncthreads();
-    // cv::resize(INTER_LINEAR_EXACT) 8U, 8.8 fixed point (SURVEY.md A.6 iii): the tables hold (i0, w1).  Resized columns past the tile's
-    // one-column halo or the image are never read: they are written as 0.
-    for (int i = tid; i < PS_H * (PS_W / 4); i += PT_NT) {
-        const int r = i / (PS_W / 4), c4 = (i - r * (PS_W / 4)) * 4, y = SY0 + r;
-        unsigned o = 0;
-        if (y < g.sh) {
-            const int2 ty = __ldg(&ws.tab[g.ytab_off + y]);
-            const uint8_t* S0 = s_b + (ty.x - Y0) * PB_W;
-            const uint8_t* S1 = s_b + (min(ty.x + 1, g.h - 1) - Y0) * PB_W;
-            const int v1 = ty.y, v0 = 256 - v1;
+            for (int k = 0; k < 3; k++) {
+                const unsigned* p = reinterpret_cast<const unsigned*>(s_b + rows[k] * PB_W) + q;
+                const unsigned a = p[0], b = p[1];
+                vv[k][0] = x0 ? a & 0xff : (a >> 16) & 0xff;         // column -1 reflects to column 1
+                vv[k][1] = (a >> 8) & 0xff; vv[k][2] = (a >> 16) & 0xff; vv[k][3] = a >> 24; vv[k][4] = b & 0xff; vv[k][5] = (b >> 8) & 0xff;
+            }
+            short dxs[4], dys[4];
 #pragma unroll
             for (int k = 0; k < 4; k++) {
-                const int x = SX0 + c4 + k;
-                if (c4 + k > PT_SW || x >= g.sw) continue;
-                const int2 tx = __ldg(&ws.tab[g.xtab_off + x]);
-                const int i0 = tx.x - X0, i1 = min(tx.x + 1, g.w - 1) - X0, w1 = tx.y, w0 = 256 - w1;
-                const int r0 = w0 * S0[i0] + w1 * S0[i1], r1 = w0 * S1[i0] + w1 * S1[i1];
-                o |= (unsigned)((v0 * r0 + v1 * r1 + 32768) >> 16) << (8 * k);
+                const int x = x0 + k;
+                int m0 = vv[0][k], m1 = vv[1][k], m2 = vv[2][k], c0 = vv[0][k + 1], c2 = vv[2][k + 1], p0 = vv[0][k + 2], p1 = vv[1][k + 2], p2 = vv[2][k + 2];
+                if (x == g.w - 1) { p0 = m0; p1 = m1; p2 = m2; }    // reflect101(w) = w - 2 = x - 1
+                dxs[k] = (short)((p0 - m0) + 2 * (p1 - m1) + (p2 - m2));
+                dys[k] = (short)((m2 - m0) + 2 * (c2 - c0) + (p2 - p0));
+            }
+            const long long o = f * g.full_stride + (long long)y * g.w + x0;
+            if ((g.w & 3) == 0 && (g.full_stride & 3) == 0) {
+                *reinterpret_cast<short4*>(ws.dx + o) = make_short4(dxs[0], dxs[1], dxs[2], dxs[3]);
+                *reinterpret_cast<short4*>(ws.dy + o) = make_short4(dys[0], dys[1], dys[2], dys[3]);
+            } else {
+#pragma unroll
+                for (int k = 0; k < 4; k++) if (x0 + k < g.w) { ws.dx[o + k] = dxs[k]; ws.dy[o + k] = dys[k]; }
             }
         }
-        s_sc[i] = o;
-    }
-    __syncthreads();
-    unsigned long long bits = 0ull;                    // max gradient norm of the defined pixels (positive doubles order like integers)
-    for (int i = tid; i < PT_SH * (PT_SW / 4); i += PT_NT) {
-        const int r = i / (PT_SW / 4), q = i - r * (PT_SW / 4);
-        const int x0 = SX0 + 4 * q, y = SY0 + r;
-        if (x0 >= g.sw || y >= g.sh) continue;
-        float ang[4]; float2 cs[4], cs0[4]; double norm[4];
-        unsigned r0 = 0, r1 = 0; int e0 = 0, e1 = 0;    // rows y, y+1: bytes x0..x0+3 and x0+4
-        const bool row_ok = y < g.sh - 1;
-        if (row_ok) {
-            const unsigned* p = s_sc + r * (PS_W / 4) + q;
-            r0 = p[0]; r1 = p[PS_W / 4]; e0 = p[1] & 0xff; e1 = p[PS_W / 4 + 1] & 0xff;
+        prep_hpass<2, 1>(s_in, s_h, BL7_T0, BL7_T4);     // blur7 column c = input column X0+c: window X0-2+c .. X0+2+c = staged c+2 ..
+        __syncthreads();                                 // s_in is free: request the next tile's box
+        {
+            const int tn = s_next;
+            if (tn < ntiles) prep_stage(s_in, g, v, tn / per_frame, (tn % per_frame % g.tiles_x) * PT_W, (tn % per_frame / g.tiles_x) * PT_H);
         }
+        prep_vpass(s_h, s_b, BL7_T0, BL7_T4);
+        __syncthreads();
+        // cv::resize(INTER_LINEAR_EXACT) 8U, 8.8 fixed point (SURVEY.md A.6 iii): the tables hold (i0, w1).  Resized columns past the tile's
+        // one-column halo or the image are never read: they are written as 0.
+        for (int i = tid; i < PS_H * (PS_W / 4); i += PT_NT) {
+            const int r = i / (PS_W / 4), c4 = (i - r * (PS_W / 4)) * 4, y = SY0 + r;
+            unsigned o = 0;
+            if (y < g.sh) {
+                const int2 ty = __ldg(&ws.tab[g.ytab_off + y]);
+                const uint8_t* S0 = s_b + (ty.x - Y0) * PB_W;
+                const uint8_t* S1 = s_b + (min(ty.x + 1, g.h - 1) - Y0) * PB_W;
+                const int v1 = ty.y, v0 = 256 - v1;
 #pragma unroll
-        for (int k = 0; k < 4; k++) {
-            ang[k] = NOTDEF_F; cs[k] = make_float2(0.f, 0.f); cs0[k] = make_float2(0.f, 0.f); norm[k] = 0;
-            if (row_ok && x0 + k < g.sw - 1) {      // the last row and column stay NOTDEF with norm 0 (lsd.cpp)
-                const int A = (r0 >> (8 * k)) & 0xff, C = (r1 >> (8 * k)) & 0xff;
-                const int Bv = (k < 3) ? (int)((r0 >> (8 * k + 8)) & 0xff) : e0, D = (k < 3) ? (int)((r1 >> (8 * k + 8)) & 0xff) : e1;
-                const LLPix p = ll_pixel(D - A, Bv - C, g.rho);
-                norm[k] = p.norm; ang[k] = p.ang; cs[k] = p.cs; cs0[k] = p.cs0;
-                if (p.norm > g.rho) {
-                    const unsigned long long nb = (unsigned long long)__double_as_longlong(p.norm);
-                    bits = nb > bits ? nb : bits;
+                for (int k = 0; k < 4; k++) {
+                    const int x = SX0 + c4 + k;
+                    if (c4 + k > PT_SW || x >= g.sw) continue;
+                    const int2 tx = __ldg(&ws.tab[g.xtab_off + x]);
+                    const int i0 = tx.x - X0, i1 = min(tx.x + 1, g.w - 1) - X0, w1 = tx.y, w0 = 256 - w1;
+                    const int r0 = w0 * S0[i0] + w1 * S0[i1], r1 = w0 * S1[i0] + w1 * S1[i1];
+                    o |= (unsigned)((v0 * r0 + v1 * r1 + 32768) >> 16) << (8 * k);
+                }
+            }
+            s_sc[i] = o;
+        }
+        __syncthreads();
+        unsigned long long bits = 0ull;                    // max gradient norm of the defined pixels (positive doubles order like integers)
+        for (int i = tid; i < PT_SH * (PT_SW / 4); i += PT_NT) {
+            const int r = i / (PT_SW / 4), q = i - r * (PT_SW / 4);
+            const int x0 = SX0 + 4 * q, y = SY0 + r;
+            if (x0 >= g.sw || y >= g.sh) continue;
+            float ang[4]; float2 cs[4], cs0[4]; double norm[4];
+            unsigned r0 = 0, r1 = 0; int e0 = 0, e1 = 0;    // rows y, y+1: bytes x0..x0+3 and x0+4
+            const bool row_ok = y < g.sh - 1;
+            if (row_ok) {
+                const unsigned* p = s_sc + r * (PS_W / 4) + q;
+                r0 = p[0]; r1 = p[PS_W / 4]; e0 = p[1] & 0xff; e1 = p[PS_W / 4 + 1] & 0xff;
+            }
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                ang[k] = NOTDEF_F; cs[k] = make_float2(0.f, 0.f); cs0[k] = make_float2(0.f, 0.f); norm[k] = 0;
+                if (row_ok && x0 + k < g.sw - 1) {      // the last row and column stay NOTDEF with norm 0 (lsd.cpp)
+                    const int A = (r0 >> (8 * k)) & 0xff, C = (r1 >> (8 * k)) & 0xff;
+                    const int Bv = (k < 3) ? (int)((r0 >> (8 * k + 8)) & 0xff) : e0, D = (k < 3) ? (int)((r1 >> (8 * k + 8)) & 0xff) : e1;
+                    const LLPix p = ll_pixel(D - A, Bv - C, g.rho);
+                    norm[k] = p.norm; ang[k] = p.ang; cs[k] = p.cs; cs0[k] = p.cs0;
+                    if (p.norm > g.rho) {
+                        const unsigned long long nb = (unsigned long long)__double_as_longlong(p.norm);
+                        bits = nb > bits ? nb : bits;
+                    }
+                }
+            }
+            const long long pi = f * g.pix_stride + (long long)y * g.sw + x0;
+            if ((g.sw & 3) == 0 && (g.pix_stride & 3) == 0) {                  // rows start 16-byte aligned in every per-pixel array
+                *reinterpret_cast<float4*>(ws.angdeg + pi) = make_float4(ang[0], ang[1], ang[2], ang[3]);
+                float4* c4 = reinterpret_cast<float4*>(ws.cs0 + pi);
+                c4[0] = make_float4(cs0[0].x, cs0[0].y, cs0[1].x, cs0[1].y); c4[1] = make_float4(cs0[2].x, cs0[2].y, cs0[3].x, cs0[3].y);
+                double2* m2 = reinterpret_cast<double2*>(ws.modgrad + pi);
+                m2[0] = make_double2(norm[0], norm[1]); m2[1] = make_double2(norm[2], norm[3]);
+                uint4* px = reinterpret_cast<uint4*>(ws.pix + pi);
+#pragma unroll
+                for (int k = 0; k < 4; k++) px[k] = make_uint4(__float_as_uint(ang[k]), __float_as_uint(cs[k].x), __float_as_uint(cs[k].y), 0u);
+            } else {
+#pragma unroll
+                for (int k = 0; k < 4; k++) if (x0 + k < g.sw) {
+                    ws.angdeg[pi + k] = ang[k]; ws.cs0[pi + k] = cs0[k]; ws.modgrad[pi + k] = norm[k];
+                    LPix px; px.ang = ang[k]; px.cx = cs[k].x; px.cy = cs[k].y; px.used = 0u;
+                    ws.pix[pi + k] = px;
                 }
             }
         }
-        const long long pi = f * g.pix_stride + (long long)y * g.sw + x0;
-        if ((g.sw & 3) == 0 && (g.pix_stride & 3) == 0) {                  // rows start 16-byte aligned in every per-pixel array
-            *reinterpret_cast<float4*>(ws.angdeg + pi) = make_float4(ang[0], ang[1], ang[2], ang[3]);
-            float4* c4 = reinterpret_cast<float4*>(ws.cs0 + pi);
-            c4[0] = make_float4(cs0[0].x, cs0[0].y, cs0[1].x, cs0[1].y); c4[1] = make_float4(cs0[2].x, cs0[2].y, cs0[3].x, cs0[3].y);
-            double2* m2 = reinterpret_cast<double2*>(ws.modgrad + pi);
-            m2[0] = make_double2(norm[0], norm[1]); m2[1] = make_double2(norm[2], norm[3]);
-            uint4* px = reinterpret_cast<uint4*>(ws.pix + pi);
 #pragma unroll
-            for (int k = 0; k < 4; k++) px[k] = make_uint4(__float_as_uint(ang[k]), __float_as_uint(cs[k].x), __float_as_uint(cs[k].y), 0u);
-        } else {
-#pragma unroll
-            for (int k = 0; k < 4; k++) if (x0 + k < g.sw) {
-                ws.angdeg[pi + k] = ang[k]; ws.cs0[pi + k] = cs0[k]; ws.modgrad[pi + k] = norm[k];
-                LPix px; px.ang = ang[k]; px.cx = cs[k].x; px.cy = cs[k].y; px.used = 0u;
-                ws.pix[pi + k] = px;
-            }
-        }
+        for (int o = 16; o > 0; o >>= 1) { const unsigned long long b = __shfl_xor_sync(0xffffffffu, bits, o); bits = b > bits ? b : bits; }
+        if ((threadIdx.x & 31) == 0 && bits) atomicMax(ws.maxgrad + f, bits);
+        t = s_next;                                      // unchanged since the read above: it is rewritten only after the loop's first barrier
+        if (t >= ntiles) break;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) { const unsigned long long t = __shfl_xor_sync(0xffffffffu, bits, o); bits = t > bits ? t : bits; }
-    if ((threadIdx.x & 31) == 0 && bits) atomicMax(ws.maxgrad + f, bits);
 }
 
 // Debug (sslpl_line_debug_ll_table): ll_pixel on every (DA, BC) in [-255, 255]^2, entry (DA + 255) * LL_SPAN + (BC + 255).
@@ -2880,6 +2907,7 @@ struct sslpl_line {
     bool trace = false;
     int used_smem = 0;
     int sm_count = 132;         // replaced by the device's count at creation
+    int prep_ctas = 0;          // k_lsd_prep CTAs resident on the whole device at once (occupancy x SMs), at creation
     int max_walkers = 0;        // 0 = one walker CTA per frame
     int walker_warps = 0;       // 0 = automatic (8 or 16 warps per frame)
     int walker_v3 = 0;          // multi-warp walker: 0 = the round-2a form (shipped), 1 = v3 (control warps + workers, O(1) retire), -1 = v3 by frame size
@@ -2947,7 +2975,7 @@ void carve(sslpl_line* h, Arena& A, const LineGeom& g, int B) {
     h->d_input = A.take<uint8_t>((size_t)B * g.in_stride + 256);
     ws.angdeg = A.take<float>((size_t)B * g.pix_stride); ws.pix = A.take<LPix>((size_t)B * g.pix_stride);
     ws.modgrad = A.take<double>((size_t)B * g.pix_stride); ws.cs0 = A.take<float2>((size_t)B * g.pix_stride);
-    ws.maxgrad = A.take<unsigned long long>(B);
+    ws.maxgrad = A.take<unsigned long long>(B); ws.prep_next = A.take<int>(1);
     ws.seeds = A.take<unsigned>((size_t)B * g.pix_stride); ws.nseeds = A.take<int>(B);
     ws.reg = A.take<unsigned>((size_t)B * g.pix_stride);
     ws.sreg = A.take<unsigned>((size_t)B * WALK_RING * WALK_SLOT_CAP); ws.sjob = A.take<double>((size_t)B * V3_RING * 13); ws.rcode = A.take<unsigned char>((size_t)B * V3_RANKS); ws.dlist = A.take<unsigned>((size_t)B * V3_DPOOL);
@@ -3003,7 +3031,8 @@ int run_pipeline(sslpl_line* h, int B) {
     h->ev_n = 0;
     lmark(h, "start");
     SSLPL_CUDA(cudaMemsetAsync(h->ws.maxgrad, 0, sizeof(unsigned long long) * B, st));
-    k_lsd_prep<<<dim3(g.tiles_x * g.tiles_y, B), PT_NT, 0, st>>>(g, h->view, h->ws);      // blurs, resize, ll_angle, Sobel
+    SSLPL_CUDA(cudaMemsetAsync(h->ws.prep_next, 0, sizeof(int), st));
+    k_lsd_prep<<<std::min(h->prep_ctas, g.tiles_x * g.tiles_y * B), PT_NT, 0, st>>>(g, h->view, h->ws, B);      // blurs, resize, ll_angle, Sobel
     lmark(h, "lsd_prep");
     k_lsd_seeds<<<B, SEED_WARPS * 32, 0, st>>>(g, h->ws);
     lmark(h, "lsd_seeds");
@@ -3072,6 +3101,12 @@ int sslpl_line_create(const sslpl_line_params* p, sslpl_line** out) {
     sslpl_line* h = new sslpl_line();
     h->p = *p;
     { int v = 0; if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, p->device) == cudaSuccess && v > 0) h->sm_count = v; }
+    {   // the persistent pre-pass fills the device once; tiles beyond that are taken from its counter
+        int occ = 0;
+        const cudaError_t oe = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_lsd_prep, PT_NT, 0);
+        if (oe != cudaSuccess || occ < 1) { set_error("k_lsd_prep occupancy query failed: %s", cudaGetErrorString(oe)); delete h; return SSLPL_ERR_CUDA; }
+        h->prep_ctas = occ * h->sm_count;
+    }
     h->trace = getenv("SSLPL_LINE_TRACE") != nullptr;
     if (const char* e = getenv("SSLPL_WALKER_LANES")) h->walker_lanes = atoi(e) != 0;
     if (const char* e = getenv("SSLPL_WALKER_V3")) h->walker_v3 = atoi(e) < 0 ? -1 : (atoi(e) != 0 ? 1 : 0);
