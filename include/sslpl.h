@@ -309,6 +309,38 @@ int  sslpl_match_bow_batch_device_vocab(sslpl_matcher* m, const uint8_t* d_desc,
 int  sslpl_match_lines_batch_device(sslpl_matcher* m, const uint8_t* d_ldesc, const int* d_nl, int nframes, int capl,
                                     int32_t* d_lmatch, int32_t* d_nlmatch);
 
+/* ---- LocalMapping's triangulation matchers over keyframe pairs resident in HBM (SURVEY.md 8(f) rows 2/3), asynchronous on the
+   handle's stream like the other *_batch_device calls; no caller-visible allocation.  LocalMapping::CreateNewMapPoints (LocalMapping.cc:
+   371-440) runs ORBmatcher::SearchForTriangulation(KF, KF2, F12, pairs, false) against each covisible neighbour, CreateNewMapLines2
+   (:911-988) LSDmatcher::SearchForTriangulation(KF, KF2, pairs); here one call runs a whole list of such pairs.
+   The keyframe set: nkf keyframes, `cap` (lines: `capl`) rows each, the layout of sslpl_orb_device_results / sslpl_line_device_results:
+   d_kps[k][cap] = mvKeysUn, d_desc[k][cap][32], d_n[k] (clamped to cap).  The pair list: d_pair[p] = (kf1, kf2) int32, kf1 in the
+   pKF1 role, kf2 in the pKF2 role.  A pair with an index outside [0, nkf) gets the count -1 and no rows.
+   Needs nkf in [1, max_batch + 1] and npairs in [1, max_batch]; bad arguments return SSLPL_ERR_ARG and enqueue nothing.  Every pair's
+   rows and count equal what sslpl_search_for_triangulation / sslpl_line_match(mode 3) return for it.
+
+   ORBmatcher::SearchForTriangulation(pKF1, pKF2, F12, vMatchedPairs, bOnlyStereo = false) (ORBmatcher.cc:660-826), monocular.
+   d_has_mp[k][cap] = KeyFrame::GetMapPoint(i) != NULL.  The FeatureVectors are KeyFrame::ComputeBoW's (KeyFrame.cc:71-80), computed here
+   from the descriptors with the vocabulary v at levelsup.  d_geom[p][11] = F12 (3x3 row-major, LocalMapping::ComputeF12 :1286-1300) then
+   the epipole ex, ey (ORBmatcher.cc:666-673), f32.  scale / sigma2 = mvScaleFactors / mvLevelSigma2 (HOST, nlevels <= SSLPL_MAX_LEVELS); a
+   KF2 feature whose octave is outside [0, nlevels) is never a candidate.  Result: d_pairs[p][cap][2] = (idx1, idx2) in ascending idx1,
+   (-1, -1) after the count; d_nmatch[p].  Needs cap <= max_features + 64 and the vocabulary's level nodes <= max_nodes; the first call
+   allocates a [max_batch][max_features + 64] int32 table, freed with the handle. */
+int  sslpl_search_for_triangulation_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nkf, int cap,
+        const uint8_t* d_has_mp, const sslpl_vocab* v, int levelsup,
+        int npairs, const int32_t* d_pair, const float* d_geom,
+        const float* scale, const float* sigma2, int nlevels, int checkOrientation,
+        int32_t* d_pairs, int32_t* d_nmatch);
+/* LSDmatcher::SearchForTriangulation(pKF1, pKF2, vMatchedPairs) (LSDmatcher.cpp:382-415), with KeyFrame::lineDescriptorMAD
+   (KeyFrame.cc:820-846) on the device.  d_ldesc[k][capl][32], d_nl[k], d_has_ml[k][capl] = KeyFrame::GetMapLine(i) != NULL.
+   Result: d_lpairs[p][capl][2] = (qdx, tdx) in ascending qdx, (-1, -1) after the count; d_nlmatch[p].  When KF1 has lines and KF2 fewer
+   than 2 (the reference reads lmatches[i][1] out of bounds there; the single call returns SSLPL_ERR_ARG) d_nlmatch[p] = -1; when KF1 has
+   none it is 0.  Needs capl <= max_lines + 64. */
+int  sslpl_line_search_for_triangulation_batch_device(sslpl_matcher* m,
+        const uint8_t* d_ldesc, const int* d_nl, int nkf, int capl, const uint8_t* d_has_ml,
+        int npairs, const int32_t* d_pair, int32_t* d_lpairs, int32_t* d_nlmatch);
+
 /* =====================================================================================
  * (2) Line segments — replaces LineSegment::ExtractLineSegment (src/ExtractLineSegment.cpp:18-69)
  * ===================================================================================== */

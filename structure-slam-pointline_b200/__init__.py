@@ -461,6 +461,29 @@ class Matcher:
         _check(lib().sslpl_match_lines_batch_device(self._h, C.c_void_p(d_ldesc), C.c_void_p(d_nl), nframes, capl,
                                                     C.c_void_p(d_lmatch), C.c_void_p(d_nlmatch)))
 
+    def search_for_triangulation_batch_device(self, d_kps, d_desc, d_n, nkf, cap, d_has_mp, vocab, levelsup, npairs, d_pair, d_geom,
+                                              scale, sigma2, check_ori, d_pairs, d_nmatch):
+        """ORBmatcher::SearchForTriangulation(pKF1, pKF2, F12, pairs, false) (ORBmatcher.cc:660-826) for npairs keyframe pairs in HBM.
+        Raw device pointers: d_kps / d_desc / d_n the keyframe set (mvKeysUn, cap rows each), d_has_mp [nkf, cap] u8, d_pair [npairs, 2]
+        i32 (kf1, kf2), d_geom [npairs, 11] f32 (F12 row-major, ex, ey); scale / sigma2 host arrays (nlevels = len(scale)) ->
+        d_pairs [npairs, cap, 2] i32 ((idx1, idx2) ascending idx1, -1 after the count), d_nmatch [npairs] i32 (-1: pair index out of
+        range).  Asynchronous on the matcher's stream."""
+        sc = np.ascontiguousarray(scale, np.float32); s2 = np.ascontiguousarray(sigma2, np.float32)
+        assert len(s2) >= len(sc)
+        _check(lib().sslpl_search_for_triangulation_batch_device(
+            self._h, C.c_void_p(d_kps), C.c_void_p(d_desc), C.c_void_p(d_n), int(nkf), int(cap), C.c_void_p(d_has_mp), vocab._h,
+            int(levelsup), int(npairs), C.c_void_p(d_pair), C.c_void_p(d_geom), _p(sc), _p(s2), len(sc), int(check_ori),
+            C.c_void_p(d_pairs), C.c_void_p(d_nmatch)))
+
+    def line_search_for_triangulation_batch_device(self, d_ldesc, d_nl, nkf, capl, d_has_ml, npairs, d_pair, d_lpairs, d_nlmatch):
+        """LSDmatcher::SearchForTriangulation(pKF1, pKF2, pairs) (LSDmatcher.cpp:382-415) for npairs keyframe pairs in HBM, with
+        KeyFrame::lineDescriptorMAD on the device.  d_ldesc [nkf, capl, 32], d_nl [nkf], d_has_ml [nkf, capl] u8, d_pair [npairs, 2] ->
+        d_lpairs [npairs, capl, 2] ((qdx, tdx) ascending qdx, -1 after the count), d_nlmatch [npairs] (-1: pair index out of range, or
+        KF1 has lines and KF2 fewer than 2).  Asynchronous on the matcher's stream."""
+        _check(lib().sslpl_line_search_for_triangulation_batch_device(
+            self._h, C.c_void_p(d_ldesc), C.c_void_p(d_nl), int(nkf), int(capl), C.c_void_p(d_has_ml), int(npairs), C.c_void_p(d_pair),
+            C.c_void_p(d_lpairs), C.c_void_p(d_nlmatch)))
+
 
 class Vocabulary:
     """DBoW2 ORB vocabulary tree on the device (the reference's ORBVocabulary = TemplatedVocabulary<FORB::TDescriptor, FORB>,
@@ -656,6 +679,9 @@ class LSDmatcher:
 
     def SearchByDescriptorKF(self, ldesc1, ldesc2, has_mapline_KF2):    # LSDmatcher.cpp:329
         return self._run(2, ldesc1, ldesc2, None, has_mapline_KF2)
+
+    def SearchForTriangulation(self, ldesc1, has_mapline_KF1, ldesc2, has_mapline_KF2):    # LSDmatcher.cpp:382 -> (n, pairs[n, 2])
+        return self._run(3, ldesc1, ldesc2, has_mapline_KF1, has_mapline_KF2)
 
     def SearchForTriangulation(self, ldesc1, has_ml1, ldesc2, has_ml2):  # LSDmatcher.cpp:382
         return self._run(3, ldesc1, ldesc2, has_ml1, has_ml2)

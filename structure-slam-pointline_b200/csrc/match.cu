@@ -26,7 +26,16 @@ struct FrameSet {
     const uint8_t* flag; long long flag_fs;                  // valid / has-MapPoint mask (may be null)
     const float* angle; int angle_es; long long angle_fs;    // keypoint angle: element stride / frame stride in floats
     const float* x; const float* y; const int* oct;          // same strides as angle (fields of sslpl_keypoint)
+    const int2* pmap; int nframes;                           // pair p = frames (pmap[p].x, pmap[p].y) of [0, nframes); NULL: (p, p + 1)
 };
+
+// the frames of pair p; false when a mapped index lies outside [0, nframes) (the pair is then left empty)
+__device__ __forceinline__ bool pair_frames(const int2* pmap, int nframes, int pair, int& f1, int& f2) {
+    if (!pmap) { f1 = pair; f2 = pair + 1; return true; }
+    const int2 q = pmap[pair];
+    f1 = q.x; f2 = q.y;
+    return (unsigned)f1 < (unsigned)nframes && (unsigned)f2 < (unsigned)nframes;
+}
 
 __device__ __forceinline__ void load_desc(const uint8_t* p, uint4& a, uint4& b) {
     const uint4* q = reinterpret_cast<const uint4*>(p);
@@ -35,20 +44,26 @@ __device__ __forceinline__ void load_desc(const uint8_t* p, uint4& a, uint4& b) 
 
 // -------------------------------------------------------------------------------------------------
 // knnMatch(k=2): one warp per query.  key = dist << 20 | trainIdx  => ascending distance, ties -> lower index
+// Pair p queries frame p of q against frame p of t (t already points at the train frames), or, with a pair map, frame
+// pmap[p].x of q against frame pmap[p].y of t (both arrays then start at frame 0).  kMap = false compiles the map out: the
+// consecutive-pair instance keeps its registers (and occupancy) on bench.py's line path.
 // -------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void top2_insert(unsigned& k0, unsigned& k1, unsigned k) {
     if (k < k0) { k1 = k0; k0 = k; } else if (k < k1) k1 = k;
 }
 
+template <bool kMap>
 __global__ void __launch_bounds__(256) k_knn2(const uint8_t* q, long long q_fs, const int* nq_arr, int nq_const,
                                                const uint8_t* t, long long t_fs, const int* nt_arr, int nt_const,
-                                               int32_t* out, long long out_fs, int qcap) {
+                                               int32_t* out, long long out_fs, int qcap, const int2* pmap, int nframes) {
     const int pair = blockIdx.y, lane = threadIdx.x & 31, qi = blockIdx.x * 8 + (threadIdx.x >> 5);
-    const int nq = nq_arr ? min(nq_arr[pair], qcap) : nq_const, nt = nt_arr ? min(nt_arr[pair + 1], qcap) : nt_const;
+    int fq, ft;
+    if (!pair_frames(kMap ? pmap : nullptr, nframes, pair, fq, ft)) return;
+    const int nq = nq_arr ? min(nq_arr[fq], qcap) : nq_const, nt = nt_arr ? min(nt_arr[ft], qcap) : nt_const;
     if (qi >= nq) return;
     uint4 a0, a1;
-    load_desc(q + pair * q_fs + (long long)qi * 32, a0, a1);
-    const uint8_t* T = t + pair * t_fs;
+    load_desc(q + fq * q_fs + (long long)qi * 32, a0, a1);
+    const uint8_t* T = t + (kMap ? ft : pair) * t_fs;
     unsigned k0 = 0xffffffffu, k1 = 0xffffffffu;
     for (int j = lane; j < nt; j += 32) {
         uint4 b0, b1;
@@ -249,13 +264,23 @@ __global__ void __launch_bounds__(128) k_bow_match(FrameSet S, int mode, float n
 
 // SearchForTriangulation (ORBmatcher.cc:660-826, monocular): warp per node of set 1; no dependency between
 // idx1's (vbMatched2 is never set), so the lanes only cooperate on the scan of the node's idx2 list.
-struct TriArgs { float F[9]; float ex, ey; float scale[SSLPL_MAX_LEVELS]; float sigma2[SSLPL_MAX_LEVELS]; };
+// F12 and the epipole of pair p are geom[11 p ..] (F row-major, ex, ey) when geom != NULL, else T's.  A KF2 feature whose octave is
+// outside [0, nlevels) is never a candidate (mvScaleFactors / mvLevelSigma2 have no entry for it).  kMap = false (the single-pair
+// call) compiles S.pmap and geom out.
+struct TriArgs { float F[9]; float ex, ey; int nlevels; float scale[SSLPL_MAX_LEVELS]; float sigma2[SSLPL_MAX_LEVELS]; };
 
-__global__ void __launch_bounds__(128) k_tri_match(FrameSet S, TriArgs T, int32_t* out, long long out_fs, uint8_t* rot, long long rot_fs) {
+template <bool kMap>
+__global__ void __launch_bounds__(128) k_tri_match(FrameSet S, TriArgs T, const float* geom, int32_t* out, long long out_fs, uint8_t* rot, long long rot_fs) {
     const int pair = blockIdx.y, lane = threadIdx.x & 31, a = blockIdx.x * 4 + (threadIdx.x >> 5);
-    const int f1 = pair, f2 = pair + 1;
+    int f1, f2;
+    if (!pair_frames(kMap ? S.pmap : nullptr, S.nframes, pair, f1, f2)) return;
     const int nn1 = S.nn ? S.nn[f1] : S.nn_const, nn2 = S.nn ? S.nn[f2] : S.nn_const;
     if (a >= nn1) return;
+    const float* G = kMap ? geom : nullptr;
+    float F[9], ex, ey;
+#pragma unroll
+    for (int k = 0; k < 9; k++) F[k] = G ? G[11LL * pair + k] : T.F[k];
+    ex = G ? G[11LL * pair + 9] : T.ex; ey = G ? G[11LL * pair + 10] : T.ey;
     const int* nodes1 = S.nodes + f1 * S.nodes_fs; const int* nodes2 = S.nodes + f2 * S.nodes_fs;
     const int b = find_node(nodes2, nn2, nodes1[a]);
     if (b < 0) return;
@@ -276,9 +301,9 @@ __global__ void __launch_bounds__(128) k_tri_match(FrameSet S, TriArgs T, int32_
         load_desc(D1 + (long long)id1 * 32, a0, a1);
         const float x1 = X1[id1 * es], y1 = Y1[id1 * es];
         // epipolar line l = x1' F12 (CheckDistEpipolarLine :143-145), f32 without contraction
-        const float la = __fadd_rn(__fadd_rn(__fmul_rn(x1, T.F[0]), __fmul_rn(y1, T.F[3])), T.F[6]);
-        const float lb = __fadd_rn(__fadd_rn(__fmul_rn(x1, T.F[1]), __fmul_rn(y1, T.F[4])), T.F[7]);
-        const float lc = __fadd_rn(__fadd_rn(__fmul_rn(x1, T.F[2]), __fmul_rn(y1, T.F[5])), T.F[8]);
+        const float la = __fadd_rn(__fadd_rn(__fmul_rn(x1, F[0]), __fmul_rn(y1, F[3])), F[6]);
+        const float lb = __fadd_rn(__fadd_rn(__fmul_rn(x1, F[1]), __fmul_rn(y1, F[4])), F[7]);
+        const float lc = __fadd_rn(__fadd_rn(__fmul_rn(x1, F[2]), __fmul_rn(y1, F[5])), F[8]);
         const float den = __fadd_rn(__fmul_rn(la, la), __fmul_rn(lb, lb));
         unsigned best = 0xffffffffu;              // min over (dist << 20 | (0xfffff - position)): min distance, LAST wins (:741)
         for (int i2 = b2 + lane; i2 < e2; i2 += 32) {
@@ -290,7 +315,8 @@ __global__ void __launch_bounds__(128) k_tri_match(FrameSet S, TriArgs T, int32_
             if (dist > TH_LOW) continue;
             const float x2 = X2[id2 * es], y2 = Y2[id2 * es];
             const int oc = OC2[id2 * es];
-            const float dex = __fsub_rn(T.ex, x2), dey = __fsub_rn(T.ey, y2);
+            if ((unsigned)oc >= (unsigned)T.nlevels) continue;
+            const float dex = __fsub_rn(ex, x2), dey = __fsub_rn(ey, y2);
             if (__fadd_rn(__fmul_rn(dex, dex), __fmul_rn(dey, dey)) < __fmul_rn(100.f, T.scale[oc])) continue;    // :749-751
             const float num = __fadd_rn(__fadd_rn(__fmul_rn(la, x2), __fmul_rn(lb, y2)), lc);
             if (den == 0.f) continue;
@@ -928,6 +954,73 @@ __global__ void __launch_bounds__(128) k_line_ratio(const int32_t* knn, long lon
     }
 }
 
+// A pair of the batched triangulation matcher whose keyframe indices lie outside [0, nframes) gets the count -1 (its rows stay empty)
+__global__ void k_bad_pairs(const int2* pmap, int npairs, int nframes, int32_t* nmatch) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    int f1, f2;
+    if (p < npairs && !pair_frames(pmap, nframes, p, f1, f2)) nmatch[p] = -1;
+}
+
+// LSDmatcher::SearchForTriangulation (LSDmatcher.cpp:382-415), one CTA per keyframe pair, on the knn2 table of (KF1 lines, KF2 lines):
+//   KeyFrame::lineDescriptorMAD's nn12_mad (KeyFrame.cc:820-846; the host form is line_mad() below) over all n1 query rows.  The
+//   distances are integers in [0, 256], so both medians are exact selections over a 257-bin histogram: med12 = element nq / 2 of the
+//   d1 - d0 sorted in DESCENDING order (conpare_descriptor_by_NN12_dist), then element nq / 2 of |d1 - d0 - med12| in ascending order;
+//   then the filter of :398-410 (skip rows whose KF1 or KF2 line has a MapLine, accept d1 - d0 > 0.1 nn12_mad) and an ordered
+//   compaction: lpairs[p][k] = (qdx, tdx) in ascending qdx, (-1, -1) past the count.
+// nlmatch[p] = -1 when an index is outside [0, nframes) or when KF1 has lines and KF2 fewer than 2 (the reference would read
+// lmatches[i][1] out of bounds, :402); 0 when KF1 has none.
+__global__ void __launch_bounds__(256) k_line_tri(const int32_t* knn, long long knn_fs, const int* nl, int capl, const int2* pmap, int nframes,
+                                                   const uint8_t* has_ml, int32_t* lpairs, int32_t* nlmatch) {
+    __shared__ int s_hist[257];
+    __shared__ int s_warp[33];
+    __shared__ int s_sel;
+    const int p = blockIdx.x, tid = threadIdx.x;
+    int f1, f2, n1 = 0, total = 0;
+    bool ok = pair_frames(pmap, nframes, p, f1, f2);
+    if (ok) {
+        n1 = max(0, min(nl[f1], capl));
+        ok = n1 == 0 || min(nl[f2], capl) >= 2;
+    }
+    const int4* K = reinterpret_cast<const int4*>(knn + p * knn_fs);
+    int32_t* O = lpairs + 2LL * capl * p;
+    if (ok && n1 > 0) {                                        // CTA-uniform
+        const int k = n1 / 2;
+        for (int i = tid; i < 257; i += 256) s_hist[i] = 0;
+        __syncthreads();
+        for (int i = tid; i < n1; i += 256) { const int4 r = K[i]; atomicAdd(&s_hist[r.w - r.y], 1); }
+        __syncthreads();
+        if (tid == 0) {                                        // descending order: count down from 256
+            int c = 0, v = 256;
+            for (; v > 0; v--) { c += s_hist[v]; if (c > k) break; }
+            s_sel = v;
+        }
+        __syncthreads();
+        const int med12 = s_sel;
+        for (int i = tid; i < 257; i += 256) s_hist[i] = 0;
+        __syncthreads();
+        for (int i = tid; i < n1; i += 256) { const int4 r = K[i]; atomicAdd(&s_hist[abs(r.w - r.y - med12)], 1); }
+        __syncthreads();
+        if (tid == 0) {                                        // ascending order
+            int c = 0, v = 0;
+            for (; v < 256; v++) { c += s_hist[v]; if (c > k) break; }
+            s_sel = v;
+        }
+        __syncthreads();
+        const double thr = __dmul_rn(__dmul_rn(1.4826, (double)s_sel), 0.1);      // nn12_mad * 0.1 (:406)
+        const uint8_t* h1 = has_ml + (long long)f1 * capl; const uint8_t* h2 = has_ml + (long long)f2 * capl;
+        const int chunk = (n1 + 255) / 256, pb = min(n1, tid * chunk), pe = min(n1, pb + chunk);
+        int c = 0;
+        for (int i = pb; i < pe; i++) { const int4 r = K[i]; c += !h1[i] && !h2[r.x] && (double)(r.w - r.y) > thr; }
+        int o = block_exclusive_scan(c, s_warp, &total);
+        for (int i = pb; i < pe; i++) {
+            const int4 r = K[i];
+            if (!h1[i] && !h2[r.x] && (double)(r.w - r.y) > thr) { O[2 * o] = i; O[2 * o + 1] = r.x; o++; }
+        }
+    }
+    for (int i = total + tid; i < capl; i += 256) { O[2 * i] = -1; O[2 * i + 1] = -1; }
+    if (tid == 0) nlmatch[p] = ok ? total : -1;
+}
+
 }  // namespace sslpl
 
 // =================================================================================================
@@ -957,6 +1050,8 @@ struct sslpl_matcher {
     // feature and the grid CSR, per pair the walker's claimed / sel / rbin tables ([max_batch + 1][max_features + 64] each)
     uint8_t* pw = nullptr;
     int32_t* pw_cell = nullptr; int* pw_off = nullptr; int* pw_idx = nullptr; int32_t* pw_sel = nullptr; uint8_t* pw_claimed = nullptr; uint8_t* pw_rbin = nullptr;
+    // per-pair match table of sslpl_search_for_triangulation_batch_device ([max_batch][max_features + 64]), allocated by its first call
+    int32_t* tw = nullptr;
     int32_t* h_small = nullptr;      // pinned scratch
     long long launches = 0;
 };
@@ -1074,7 +1169,7 @@ int run_knn2(sslpl_matcher* m, const uint8_t* q, int nq, const uint8_t* t, int n
     cudaStream_t st = m->stream;
     SSLPL_CUDA(cudaMemcpyAsync(m->desc, q, (size_t)nq * 32, cudaMemcpyHostToDevice, st));
     if (nt) SSLPL_CUDA(cudaMemcpyAsync(m->desc + (size_t)m->cap * 32, t, (size_t)nt * 32, cudaMemcpyHostToDevice, st));
-    k_knn2<<<dim3((nq + 7) / 8, 1), 256, 0, st>>>(m->desc, 0, nullptr, nq, m->desc + (size_t)m->cap * 32, 0, nullptr, nt, m->knn, 0, nq);
+    k_knn2<false><<<dim3((nq + 7) / 8, 1), 256, 0, st>>>(m->desc, 0, nullptr, nq, m->desc + (size_t)m->cap * 32, 0, nullptr, nt, m->knn, 0, nq, nullptr, 0);
     m->launches++;
     SSLPL_CUDA(cudaGetLastError());
     if (out_host) {
@@ -1149,6 +1244,7 @@ void sslpl_matcher_destroy(sslpl_matcher* m) {
     if (m->arena) cudaFree(m->arena);
     if (m->scratch) cudaFree(m->scratch);
     if (m->pw) cudaFree(m->pw);
+    if (m->tw) cudaFree(m->tw);
     if (m->h_small) cudaFreeHost(m->h_small);
     delete m;
 }
@@ -1247,9 +1343,9 @@ int sslpl_search_for_triangulation(sslpl_matcher* m, const uint8_t* d1, int n1, 
     FrameSet S = staging_set(m, fv1->nn, fv2->nn, true);
     TriArgs T;
     for (int i = 0; i < 9; i++) T.F[i] = F12[i];
-    T.ex = ex; T.ey = ey;
+    T.ex = ex; T.ey = ey; T.nlevels = nlevels;
     for (int i = 0; i < SSLPL_MAX_LEVELS; i++) { T.scale[i] = i < nlevels ? scale[i] : 0.f; T.sigma2[i] = i < nlevels ? sigma2[i] : 0.f; }
-    if (fv1->nn > 0 && fv2->nn > 0) { k_tri_match<<<dim3((fv1->nn + 3) / 4, 1), 128, 0, st>>>(S, T, m->out, 0, m->rot, 0); m->launches++; }
+    if (fv1->nn > 0 && fv2->nn > 0) { k_tri_match<false><<<dim3((fv1->nn + 3) / 4, 1), 128, 0, st>>>(S, T, nullptr, m->out, 0, m->rot, 0); m->launches++; }
     k_rot_filter<<<1, 256, 0, st>>>(m->out, 0, m->rot, 0, nullptr, 0, n1, cap, checkOri, m->nmatch, m->pairs, 0); m->launches++;
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(m->h_small + 8, m->nmatch, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -1896,13 +1992,85 @@ int sslpl_match_lines_batch_device(sslpl_matcher* m, const uint8_t* d_ldesc, con
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
     const int npairs = nframes - 1, lc = m->p.max_lines + 64;
-    k_knn2<<<dim3((capl + 7) / 8, npairs), 256, 0, st>>>(d_ldesc, (long long)capl * 32, d_nl, 0, d_ldesc + (size_t)capl * 32, (long long)capl * 32,
-                                                          d_nl, 0, m->b_knn, (long long)lc * 4, capl);
+    k_knn2<false><<<dim3((capl + 7) / 8, npairs), 256, 0, st>>>(d_ldesc, (long long)capl * 32, d_nl, 0, d_ldesc + (size_t)capl * 32, (long long)capl * 32,
+                                                          d_nl, 0, m->b_knn, (long long)lc * 4, capl, nullptr, 0);
     m->launches++;
     fill(m, d_lmatch, (long long)npairs * capl, -1);
     SSLPL_CUDA(cudaMemsetAsync(d_nlmatch, 0, sizeof(int32_t) * npairs, st));
     k_line_ratio<<<dim3((capl + 127) / 128, npairs), 128, 0, st>>>(m->b_knn, (long long)lc * 4, d_nl, 0, capl, nullptr, 0, d_lmatch, capl, d_nlmatch);
     m->launches++;
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+// ---------------- LocalMapping's matchers over keyframe pairs in HBM (SURVEY.md 8(f) rows 2/3) ----------------
+// SearchForTriangulation for a list of (KF1, KF2) pairs of one keyframe set: the FeatureVector of every keyframe (KeyFrame::ComputeBoW's,
+// from the descriptors), then k_tri_match over the pair map with per-pair F12 / epipole, the rotation filter and the ordered compaction.
+int sslpl_search_for_triangulation_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nkf, int cap, const uint8_t* d_has_mp,
+        const sslpl_vocab* v, int levelsup, int npairs, const int32_t* d_pair, const float* d_geom,
+        const float* scale, const float* sigma2, int nlevels, int checkOrientation, int32_t* d_pairs, int32_t* d_nmatch) {
+    SSLPL_REQUIRE(m && d_kps && d_desc && d_n && d_has_mp && v && d_pair && d_geom && scale && sigma2 && d_pairs && d_nmatch,
+                  SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nkf >= 1 && nkf <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nkf outside [1, max_batch + 1]");
+    SSLPL_REQUIRE(npairs >= 1 && npairs <= m->p.max_batch, SSLPL_ERR_ARG, "npairs outside [1, max_batch]");
+    SSLPL_REQUIRE(cap >= 1 && cap <= m->p.max_features + 64, SSLPL_ERR_ARG, "cap outside [1, max_features + 64]");
+    SSLPL_REQUIRE(nlevels >= 1 && nlevels <= SSLPL_MAX_LEVELS, SSLPL_ERR_ARG, "nlevels out of range");
+    const int nc = vocab_level_nodes(v, levelsup);
+    SSLPL_REQUIRE(nc <= m->p.max_nodes, SSLPL_ERR_ARG, "the vocabulary level exceeds the matcher capacity (max_nodes)");
+    SSLPL_REQUIRE(v->device == m->p.device, SSLPL_ERR_ARG, "vocabulary and matcher live on different devices");
+    SSLPL_REQUIRE((size_t)((nc + 1 + cap) * sizeof(int)) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "nodes + features exceed the shared memory of one CTA ((nc + 1 + cap) * 4 <= 200 KB)");
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    const int fc = m->p.max_features + 64, NN = m->p.max_nodes + 1;
+    if (!m->tw) {                                                        // first call: a handle that never gets here never pays for it
+        const size_t bytes = sizeof(int32_t) * (size_t)m->p.max_batch * fc;
+        cudaError_t e = cudaMalloc(&m->tw, bytes);
+        if (e != cudaSuccess) { m->tw = nullptr; set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return SSLPL_ERR_CUDA; }
+    }
+    cudaStream_t st = m->stream;
+    const int2* pmap = reinterpret_cast<const int2*>(d_pair);
+    k_vocab_transform<<<dim3((cap + 127) / 128, nkf), 128, 0, st>>>(d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup,
+                                                                     nullptr, nullptr, m->b_node, nullptr, fc);
+    k_build_csr<<<nkf, 128, (nc + 1 + cap) * sizeof(int), st>>>(m->b_node, fc, d_n, cap, nc, m->b_off, NN + 1, m->b_idx, fc);
+    m->launches += 2;
+    fill(m, m->tw, (long long)npairs * cap, -1);
+    fill(m, d_pairs, 2LL * npairs * cap, -1);
+    FrameSet S; memset(&S, 0, sizeof(S));
+    S.desc = d_desc; S.desc_fs = (long long)cap * 32;
+    S.nodes = m->iota; S.nodes_fs = 0; S.nn = nullptr; S.nn_const = nc;            // dense node ranks: every keyframe lists 0..nc-1
+    S.off = m->b_off; S.idx = m->b_idx; S.off_fs = NN + 1; S.idx_fs = fc;
+    S.flag = d_has_mp; S.flag_fs = cap;
+    const float* kf = reinterpret_cast<const float*>(d_kps);
+    S.angle = kf + 3; S.x = kf; S.y = kf + 1; S.oct = reinterpret_cast<const int*>(kf + 5); S.angle_es = 7; S.angle_fs = (long long)cap * 7;
+    S.pmap = pmap; S.nframes = nkf;
+    TriArgs T; memset(&T, 0, sizeof(T));
+    T.nlevels = nlevels;
+    for (int i = 0; i < nlevels; i++) { T.scale[i] = scale[i]; T.sigma2[i] = sigma2[i]; }
+    // b_rot is only read where the table holds a match, and k_tri_match writes both together
+    k_tri_match<true><<<dim3((nc + 3) / 4, npairs), 128, 0, st>>>(S, T, d_geom, m->tw, cap, m->b_rot, fc);
+    k_rot_filter<<<npairs, 256, 0, st>>>(m->tw, cap, m->b_rot, fc, nullptr, 0, cap, cap, checkOrientation, d_nmatch, d_pairs, 2LL * cap);
+    k_bad_pairs<<<(npairs + 127) / 128, 128, 0, st>>>(pmap, npairs, nkf, d_nmatch);
+    m->launches += 3;
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+// LSDmatcher::SearchForTriangulation for a list of (KF1, KF2) pairs: k_knn2 over the pair map (query = KF1's lines, train = KF2's), then
+// k_line_tri (lineDescriptorMAD, the filter and the compaction) per pair.
+int sslpl_line_search_for_triangulation_batch_device(sslpl_matcher* m, const uint8_t* d_ldesc, const int* d_nl, int nkf, int capl,
+        const uint8_t* d_has_ml, int npairs, const int32_t* d_pair, int32_t* d_lpairs, int32_t* d_nlmatch) {
+    SSLPL_REQUIRE(m && d_ldesc && d_nl && d_has_ml && d_pair && d_lpairs && d_nlmatch, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nkf >= 1 && nkf <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nkf outside [1, max_batch + 1]");
+    SSLPL_REQUIRE(npairs >= 1 && npairs <= m->p.max_batch, SSLPL_ERR_ARG, "npairs outside [1, max_batch]");
+    SSLPL_REQUIRE(capl >= 1 && capl <= m->p.max_lines + 64, SSLPL_ERR_ARG, "capl outside [1, max_lines + 64]");
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    cudaStream_t st = m->stream;
+    const int lc = m->p.max_lines + 64;
+    const int2* pmap = reinterpret_cast<const int2*>(d_pair);
+    k_knn2<true><<<dim3((capl + 7) / 8, npairs), 256, 0, st>>>(d_ldesc, (long long)capl * 32, d_nl, 0, d_ldesc, (long long)capl * 32, d_nl, 0,
+                                                          m->b_knn, (long long)lc * 4, capl, pmap, nkf);
+    k_line_tri<<<npairs, 256, 0, st>>>(m->b_knn, (long long)lc * 4, d_nl, capl, pmap, nkf, d_has_ml, d_lpairs, d_nlmatch);
+    m->launches += 2;
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
