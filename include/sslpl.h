@@ -341,6 +341,59 @@ int  sslpl_line_search_for_triangulation_batch_device(sslpl_matcher* m,
         const uint8_t* d_ldesc, const int* d_nl, int nkf, int capl, const uint8_t* d_has_ml,
         int npairs, const int32_t* d_pair, int32_t* d_lpairs, int32_t* d_nlmatch);
 
+/* ---- MapPoint::PredictScale / MapLine::PredictScale (MapPoint.cc:390-405, MapLine.cpp:386-395) on the device, exact against the host's
+   logf: level = (int)ceil(logf(ratio) / logScaleFactor), ratio = mfMaxDistance / dist.  The level is a monotone step function of the float
+   ratio; thr[k] (k = 0 .. nlevels, nlevels + 1 floats) is the smallest positive float whose level is >= k, found by bisection over the
+   float bit patterns with this process's logf (+inf when no finite ratio gets there).  Host-only, needs no device.  The device counts
+   the thresholds <= ratio.  A ratio that is not finite and positive (NaN, +-inf, <= 0: dist = 0, 0 / 0) gives INT_MIN on x86-64, i.e.
+   level 0 for a MapPoint (clamped to [0, nlevels - 1]) and outside the pyramid for a MapLine (not clamped: dropped).
+   Needs nlevels in [1, SSLPL_MAX_LEVELS] and logScaleFactor positive and finite. ---- */
+int  sslpl_predict_scale_table(float logScaleFactor, int nlevels, float* thr);
+/* The device function the batched Fuse calls use, on n HOST ratios: clamp != 0 gives the MapPoint level in [0, nlevels - 1]; clamp = 0
+   gives INT_MIN for a ratio that is not finite and positive, else the level when it lies in [0, nlevels), -1 for any level below 0
+   and nlevels for any level >= nlevels.  Synchronous. */
+int  sslpl_matcher_debug_predict_scale(sslpl_matcher* m, int n, const float* ratio, float logScaleFactor, int nlevels, int clamp,
+                                       int32_t* level);
+
+/* ---- LocalMapping::SearchInNeighbors' Fuse calls (LocalMapping.cc:1178-1279) over keyframes resident in HBM, monocular, asynchronous on
+   the handle's stream; no caller-visible allocation.  ORBmatcher::Fuse(pKF, vpMapPoints, th) (ORBmatcher.cc:828-973) and
+   LSDmatcher::Fuse(pKF, vpMapLines, th) (LSDmatcher.cpp:417-548) are one call per target keyframe in the reference; here one call runs a
+   flat list of (keyframe, element) entries over many keyframes, projection stage included.
+   The keyframe set: nkf in [1, max_batch + 1] keyframes, the layout of sslpl_orb_device_results / sslpl_line_device_results (d_kps[k][cap] =
+   mvKeysUn, d_desc[k][cap][32], d_n[k]; d_kl[k][capl] = mvKeyLines, d_ldesc[k][capl][32], d_nl[k]; counts clamped to cap / capl), and
+   d_kfpose[k][15] = Tcw (3x4 row-major) then Ow (GetCameraCenter), f32.  The entries: d_entry[e] = (kf, element) int32, element -1 =
+   a NULL pointer in the vector; d_skip[e] (u8, NULL = none) = what the reference tests before projecting, as the caller sees it at the
+   call: points isBad() || IsInKeyFrame(kf), lines isBad() (line Fuse has no IsInKeyFrame test).  cam = fx fy cx cy, bounds = mnMinX
+   mnMaxX mnMinY mnMaxY, scaleFactors = mvScaleFactors, nlevels <= SSLPL_MAX_LEVELS, logScaleFactor = mfLogScaleFactor (all HOST).
+   Result per entry: d_best_idx[e], d_best_dist[e] = what the projection stage followed by sslpl_fuse_points_search /
+   sslpl_fuse_lines_search give for that keyframe (the caller fuses when best_dist <= 50): (-1, 256) for a point and (-1, INT_MAX) for
+   a line without a candidate (skipped, NULL, failed gate, a line whose level falls outside the pyramid).  An entry whose kf is outside
+   [0, nkf) or whose element is outside [-1, nel) gets (-1, -1) and reads nothing.  nentries = 0 enqueues nothing; bad arguments
+   return SSLPL_ERR_ARG and enqueue nothing.
+   Order dependence: the results are exact for the inputs as given.  Within one reference Fuse call a Replace recomputes the surviving
+   element's descriptor (MapPoint.cc:217, MapLine.cpp:216), which later iterations read; Replace leaves position, normal and distances
+   alone, so a descriptor change is the only way a result goes stale.  SearchInNeighbors is two dependent calls: phase A (the current
+   keyframe's elements into every target) and phase B (the candidates, collected from the targets after phase A's bookkeeping
+   :1209-1224, into the current keyframe).  The caller applies Replace / AddObservation in entry order, re-tests isBad / IsInKeyFrame
+   there, and re-submits any entry whose element's descriptor a Replace recomputed since the call.
+
+   Points: d_mp[m][9] = Xw, normal, GetMinDistanceInvariance(), GetMaxDistanceInvariance(), mfMaxDistance; d_mpdesc[m][32].
+   invLevelSigma2 = mvInvLevelSigma2 (HOST).  Every keyframe's 64 x 48 grid (AssignFeaturesToGrid) is built per call in a workspace of
+   max_batch + 1 grids allocated by the first call that needs it (shared with sslpl_search_by_projection_frame_batch_device) and freed
+   with the handle.  A keyframe octave below 0 is never a candidate.  Stereo (mvuRight >= 0) stays with the single call. */
+int  sslpl_fuse_points_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nkf, int cap, const float* d_kfpose,
+        int nmp, const float* d_mp, const uint8_t* d_mpdesc, int nentries, const int32_t* d_entry, const uint8_t* d_skip,
+        const float* cam, const float* bounds, const float* scaleFactors, const float* invLevelSigma2, int nlevels, float logScaleFactor,
+        float th, int32_t* d_best_idx, int32_t* d_best_dist);
+/* Lines: d_ml[m][12] = SP, EP (GetWorldPos, narrowed to float), GetNormal() (narrowed to float), minInv, maxInv, mfMaxDistance;
+   d_mldesc[m][32].  Needs capl <= max_lines + 64. */
+int  sslpl_fuse_lines_batch_device(sslpl_matcher* m,
+        const sslpl_keyline* d_kl, const uint8_t* d_ldesc, const int* d_nl, int nkf, int capl, const float* d_kfpose,
+        int nml, const float* d_ml, const uint8_t* d_mldesc, int nentries, const int32_t* d_entry, const uint8_t* d_skip,
+        const float* cam, const float* bounds, const float* scaleFactors, int nlevels, float logScaleFactor, float th,
+        int32_t* d_best_idx, int32_t* d_best_dist);
+
 /* =====================================================================================
  * (2) Line segments — replaces LineSegment::ExtractLineSegment (src/ExtractLineSegment.cpp:18-69)
  * ===================================================================================== */

@@ -484,6 +484,50 @@ class Matcher:
             self._h, C.c_void_p(d_ldesc), C.c_void_p(d_nl), int(nkf), int(capl), C.c_void_p(d_has_ml), int(npairs), C.c_void_p(d_pair),
             C.c_void_p(d_lpairs), C.c_void_p(d_nlmatch)))
 
+    def fuse_points_batch_device(self, d_kps, d_desc, d_n, nkf, cap, d_kfpose, nmp, d_mp, d_mpdesc, nentries, d_entry, d_skip,
+                                 cam, bounds, scale_factors, inv_level_sigma2, log_scale_factor, th, d_best_idx, d_best_dist):
+        """ORBmatcher::Fuse(pKF, vpMapPoints, th) (ORBmatcher.cc:828-973, monocular) for a flat list of (keyframe, MapPoint) entries in
+        HBM, projection stage (with PredictScale) included.  Raw device pointers: d_kps / d_desc / d_n the keyframe set (mvKeysUn, cap rows
+        each), d_kfpose [nkf, 15] f32 (Tcw 3x4, Ow), d_mp [nmp, 9] f32 (Xw, normal, minInv, maxInv, maxRaw), d_mpdesc [nmp, 32] u8,
+        d_entry [nentries, 2] i32 (kf, mp; mp = -1 NULL), d_skip [nentries] u8 or 0; cam = fx fy cx cy, bounds, scale_factors (nlevels =
+        len), inv_level_sigma2 host arrays -> d_best_idx / d_best_dist [nentries] i32 ((-1, 256) no candidate, (-1, -1) index out of
+        range).  Asynchronous on the matcher's stream."""
+        f32 = lambda a: np.ascontiguousarray(a, np.float32)
+        sf = f32(scale_factors); isg = f32(inv_level_sigma2)
+        assert len(isg) >= len(sf)
+        _check(lib().sslpl_fuse_points_batch_device(
+            self._h, C.c_void_p(d_kps), C.c_void_p(d_desc), C.c_void_p(d_n), int(nkf), int(cap), C.c_void_p(d_kfpose), int(nmp),
+            C.c_void_p(d_mp), C.c_void_p(d_mpdesc), int(nentries), C.c_void_p(d_entry), C.c_void_p(d_skip or None), _p(f32(cam)[:4].copy()),
+            _p(f32(bounds)), _p(sf), _p(isg), len(sf), C.c_float(log_scale_factor), C.c_float(th), C.c_void_p(d_best_idx), C.c_void_p(d_best_dist)))
+
+    def fuse_lines_batch_device(self, d_kl, d_ldesc, d_nl, nkf, capl, d_kfpose, nml, d_ml, d_mldesc, nentries, d_entry, d_skip,
+                                cam, bounds, scale_factors, log_scale_factor, th, d_best_idx, d_best_dist):
+        """LSDmatcher::Fuse(pKF, vpMapLines, th) (LSDmatcher.cpp:417-548) for a flat list of (keyframe, MapLine) entries in HBM.  d_kl /
+        d_ldesc / d_nl as sslpl_line_device_results gives them, d_ml [nml, 12] f32 (SP, EP, normal, minInv, maxInv, maxRaw), d_mldesc
+        [nml, 32]; the rest as fuse_points_batch_device -> (-1, INT_MAX) no candidate (a level outside the pyramid included), (-1, -1)
+        index out of range.  Asynchronous on the matcher's stream."""
+        f32 = lambda a: np.ascontiguousarray(a, np.float32)
+        sf = f32(scale_factors)
+        _check(lib().sslpl_fuse_lines_batch_device(
+            self._h, C.c_void_p(d_kl), C.c_void_p(d_ldesc), C.c_void_p(d_nl), int(nkf), int(capl), C.c_void_p(d_kfpose), int(nml),
+            C.c_void_p(d_ml), C.c_void_p(d_mldesc), int(nentries), C.c_void_p(d_entry), C.c_void_p(d_skip or None), _p(f32(cam)[:4].copy()),
+            _p(f32(bounds)), _p(sf), len(sf), C.c_float(log_scale_factor), C.c_float(th), C.c_void_p(d_best_idx), C.c_void_p(d_best_dist)))
+
+    def debug_predict_scale(self, ratio, log_scale_factor, nlevels, clamp=True):
+        """MapPoint / MapLine::PredictScale on the device for host ratios (see sslpl_matcher_debug_predict_scale) -> int32 levels."""
+        r = np.ascontiguousarray(ratio, np.float32).reshape(-1)
+        out = np.empty(max(len(r), 1), np.int32)
+        _check(lib().sslpl_matcher_debug_predict_scale(self._h, len(r), _p(r), C.c_float(log_scale_factor), int(nlevels), int(clamp), _p(out)))
+        return out[:len(r)]
+
+
+def predict_scale_table(log_scale_factor, nlevels):
+    """The nlevels + 1 PredictScale thresholds of sslpl_predict_scale_table (host only, no device): thr[k] = the smallest positive float
+    ratio whose level (int)ceil(logf(ratio) / log_scale_factor) is >= k."""
+    thr = np.empty(int(nlevels) + 1, np.float32)
+    _check(lib().sslpl_predict_scale_table(C.c_float(log_scale_factor), int(nlevels), _p(thr)))
+    return thr
+
 
 class Vocabulary:
     """DBoW2 ORB vocabulary tree on the device (the reference's ORBVocabulary = TemplatedVocabulary<FORB::TDescriptor, FORB>,

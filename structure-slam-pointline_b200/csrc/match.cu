@@ -7,6 +7,7 @@
 // vector and optional masks; pair p matches frame p (KeyFrame role) against frame p+1 (Frame role).
 #include "common.cuh"
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <vector>
@@ -679,22 +680,140 @@ __global__ void __launch_bounds__(32) k_line_window_search(int nml, const uint8_
     if (lane == 0) *nmatch = nmatches;
 }
 
-// Search stage of LSDmatcher::Fuse (LSDmatcher.cpp:499-523): independent per MapLine, one warp each
+// -------------------------------------------------------------------------------------------------
+// MapPoint::PredictScale / MapLine::PredictScale (MapPoint.cc:390-405, MapLine.cpp:386-395): (int)ceil(logf(ratio) / logScaleFactor).
+// The level is a monotone step function of the float ratio, so the host finds, with its own logf, the smallest positive float t_k
+// whose level is >= k for k = 0 .. nlevels (sslpl_predict_scale_table) and the device counts the thresholds <= ratio: the same levels
+// as the host's libm by construction.  A ratio that is not finite and positive (NaN, +-inf, <= 0) has logf = NaN or -inf, which
+// x86-64 converts to INT_MIN: clamped to level 0 (points), outside the pyramid (lines).
+// clamp: [0, nlevels - 1];  !clamp: INT_MIN as above, else -1 for any level below 0, nlevels for any level >= nlevels.
+// -------------------------------------------------------------------------------------------------
+struct PredictTable { float thr[SSLPL_MAX_LEVELS + 1]; int nlevels; };
+
+__device__ __forceinline__ int predict_scale(float ratio, const float* thr, int nlevels, bool clamp) {
+    int c = 0;
+    for (int k = 0; k <= nlevels; k++) c += thr[k] <= ratio;
+    if (!(ratio > 0.f && ratio < INFINITY)) return clamp ? 0 : INT_MIN;
+    return clamp ? min(max(c - 1, 0), nlevels - 1) : c - 1;
+}
+
+__global__ void k_predict_scale(int n, const float* ratio, const __grid_constant__ PredictTable T, int clamp, int32_t* level) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) level[i] = predict_scale(ratio[i], T.thr, T.nlevels, clamp != 0);
+}
+
+// Rcw * x + tcw of a KeyFrame pose (Tcw 3x4 row-major): cv::gemm's float path, products summed left to right, the addend last
+__device__ __forceinline__ float rt_row(const float* T, float x0, float x1, float x2) {
+    return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[0], x0), __fmul_rn(T[1], x1)), __fmul_rn(T[2], x2)), T[3]);
+}
+// (float)cv::norm(d) (double accumulation) and the double dot product with the normal of the viewing-angle gate
+__device__ __forceinline__ float norm3d(float d0, float d1, float d2) {
+    return __double2float_rn(__dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn((double)d0, (double)d0), __dmul_rn((double)d1, (double)d1)),
+                                                  __dmul_rn((double)d2, (double)d2))));
+}
+__device__ __forceinline__ bool view_ok(float d0, float d1, float d2, float n0, float n1, float n2, float dist) {
+    const double dot = __dadd_rn(__dadd_rn(__dmul_rn((double)d0, (double)n0), __dmul_rn((double)d1, (double)n1)), __dmul_rn((double)d2, (double)n2));
+    return !(dot < __dmul_rn(0.5, (double)dist));
+}
+
+// Where the batched Fuse calls read: entry e = (keyframe, element) pair, the keyframe set (strides in elements of its arrays), the
+// element table and the keyframe poses pose[k][15] = Tcw (3x4 row-major), Ow.  Unused (zero) in the single-call instances.
+struct FuseMap {
+    const int2* entry; const uint8_t* skip; int nkf, nel;
+    const float* kp; long long kp_fs; const uint8_t* desc; long long desc_fs; const int* n; int cap;
+    const float* pose; const float* el; const uint8_t* eldesc;
+    const int* goff; const int* gidx; long long goff_fs, gidx_fs;      // points: the 64 x 48 grid CSR of every keyframe
+    float fx, fy, cx, cy, minX, maxX, minY, maxY;
+    PredictTable T;
+    float invSigma2[SSLPL_MAX_LEVELS];
+    float scale[SSLPL_MAX_LEVELS];
+};
+
+// entry e of a batched call: false (and (-1, -1) written) when its keyframe or element index is out of range
+__device__ __forceinline__ bool fuse_entry(const FuseMap& M, int e, int lane, int& k, int& p, int32_t* best_idx, int32_t* best_dist) {
+    const int2 q = M.entry[e];
+    k = q.x; p = q.y;
+    if ((unsigned)k < (unsigned)M.nkf && p >= -1 && p < M.nel) return true;
+    if (lane == 0) { best_idx[e] = -1; best_dist[e] = -1; }
+    return false;
+}
+
+// Projection stage of ORBmatcher::Fuse (ORBmatcher.cc:828-894) for MapPoint p in keyframe k, with the reference's operation order.
+// el[p][9] = Xw, normal, minInv, maxInv, maxRaw.
+__device__ __forceinline__ bool fuse_project_point(const FuseMap& M, int k, int p, float& u, float& v, int& lvl) {
+    const float* T = M.pose + 15LL * k;
+    const float* P = M.el + 9LL * p;
+    const float X0 = P[0], X1 = P[1], X2 = P[2];
+    const float zc = rt_row(T + 8, X0, X1, X2);
+    if (zc < 0.0f) return false;
+    const float invz = __fdiv_rn(1.0f, zc);
+    u = __fadd_rn(__fmul_rn(M.fx, __fmul_rn(rt_row(T, X0, X1, X2), invz)), M.cx);
+    v = __fadd_rn(__fmul_rn(M.fy, __fmul_rn(rt_row(T + 4, X0, X1, X2), invz)), M.cy);
+    if (!(u >= M.minX && u < M.maxX && v >= M.minY && v < M.maxY)) return false;     // KeyFrame::IsInImage KeyFrame.cc:686-689
+    const float d0 = __fsub_rn(X0, T[12]), d1 = __fsub_rn(X1, T[13]), d2 = __fsub_rn(X2, T[14]);
+    const float dist = norm3d(d0, d1, d2);
+    if (dist < P[6] || dist > P[7]) return false;
+    if (!view_ok(d0, d1, d2, P[3], P[4], P[5], dist)) return false;
+    lvl = predict_scale(__fdiv_rn(P[8], dist), M.T.thr, M.T.nlevels, true);
+    return true;
+}
+
+// Projection stage of LSDmatcher::Fuse (LSDmatcher.cpp:417-497) for MapLine p in keyframe k, with the reference's operation order.
+// el[p][12] = SP, EP, normal, minInv, maxInv, maxRaw.  A level outside the pyramid drops the line.
+__device__ __forceinline__ bool fuse_project_line(const FuseMap& M, int k, int p, float4& q, int& lvl) {
+    const float* T = M.pose + 15LL * k;
+    const float* L = M.el + 12LL * p;
+    const float s0 = L[0], s1 = L[1], s2 = L[2], e0 = L[3], e1 = L[4], e2 = L[5];
+    const float sz = rt_row(T + 8, s0, s1, s2), ez = rt_row(T + 8, e0, e1, e2);
+    if (sz < 0.0f || ez < 0.0f) return false;
+    const float iz1 = __fdiv_rn(1.0f, sz), iz2 = __fdiv_rn(1.0f, ez);
+    q.x = __fadd_rn(__fmul_rn(__fmul_rn(M.fx, rt_row(T, s0, s1, s2)), iz1), M.cx);
+    q.y = __fadd_rn(__fmul_rn(__fmul_rn(M.fy, rt_row(T + 4, s0, s1, s2)), iz1), M.cy);
+    if (q.x < M.minX || q.x > M.maxX || q.y < M.minY || q.y > M.maxY) return false;
+    q.z = __fadd_rn(__fmul_rn(__fmul_rn(M.fx, rt_row(T, e0, e1, e2)), iz2), M.cx);
+    q.w = __fadd_rn(__fmul_rn(__fmul_rn(M.fy, rt_row(T + 4, e0, e1, e2)), iz2), M.cy);
+    if (q.z < M.minX || q.z > M.maxX || q.w < M.minY || q.w > M.maxY) return false;
+    const float d0 = __fsub_rn(__fmul_rn(0.5f, __fadd_rn(s0, e0)), T[12]), d1 = __fsub_rn(__fmul_rn(0.5f, __fadd_rn(s1, e1)), T[13]),
+                d2 = __fsub_rn(__fmul_rn(0.5f, __fadd_rn(s2, e2)), T[14]);
+    const float dist = norm3d(d0, d1, d2);
+    if (dist < L[9] || dist > L[10]) return false;
+    if (!view_ok(d0, d1, d2, L[6], L[7], L[8], dist)) return false;
+    lvl = predict_scale(__fdiv_rn(L[11], dist), M.T.thr, M.T.nlevels, false);
+    return lvl >= 0 && lvl < M.T.nlevels;
+}
+
+// Search stage of LSDmatcher::Fuse (LSDmatcher.cpp:499-523): independent per MapLine, one warp each.  kMap: warp i runs entry i of a
+// batched call (fuse_project_line, then the same search over keyframe k's sslpl_keyline rows); false compiles the map out.
+template <bool kMap>
 __global__ void __launch_bounds__(128) k_line_fuse_search(int nml, const uint8_t* active, const float4* proj, const int* level, const uint8_t* dml,
                                                            int nl2, const uint8_t* ld2, const float* kl2, const int* oct2, const float* scale, float th,
-                                                           int32_t* best_idx, int32_t* best_dist) {
+                                                           int32_t* best_idx, int32_t* best_dist, const __grid_constant__ FuseMap M) {
     const int i = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (i >= nml) return;
+    // keyline fields: (pt.x, pt.y, angle) rows and a separate octave array, or sslpl_keyline (angle, class_id, octave, pt_x, pt_y, ...)
+    constexpr int es = kMap ? 17 : 3, ox = kMap ? 3 : 0, oy = kMap ? 4 : 1, oa = kMap ? 0 : 2, oes = kMap ? 17 : 1;
     unsigned long long b = ~0ull;
-    if (active[i]) {
-        const int lvl = level[i];
-        const float4 p = proj[i];
+    bool act;
+    int lvl;
+    float4 p;
+    if (kMap) {
+        int k, e;
+        if (!fuse_entry(M, i, lane, k, e, best_idx, best_dist)) return;
+        act = e >= 0 && !(M.skip && M.skip[i]) && fuse_project_line(M, k, e, p, lvl);
+        nl2 = min(M.n[k], M.cap); ld2 = M.desc + k * M.desc_fs; kl2 = M.kp + k * M.kp_fs;
+        oct2 = reinterpret_cast<const int*>(kl2 + 2); scale = M.scale; dml = M.eldesc + (long long)e * 32;
+    } else {
+        act = active[i];
+        dml += (long long)i * 32;
+    }
+    if (act) {
+        if (!kMap) { lvl = level[i]; p = proj[i]; }
         const LineWin w = line_win(p.x, p.y, p.z, p.w, __fmul_rn(th, scale[lvl]), -1, -1);
         uint4 a0, a1;
-        load_desc(dml + (long long)i * 32, a0, a1);
+        load_desc(dml, a0, a1);
         for (int j = lane; j < nl2; j += 32) {
-            const int o = oct2[j];
-            if (!line_in_area(w, kl2[3 * j], kl2[3 * j + 1], kl2[3 * j + 2], o)) continue;
+            const int o = oct2[oes * j];
+            if (!line_in_area(w, kl2[es * j + ox], kl2[es * j + oy], kl2[es * j + oa], o)) continue;
             if (o < lvl - 1 || o > lvl) continue;
             uint4 c0, c1;
             load_desc(ld2 + (long long)j * 32, c0, c1);
@@ -707,32 +826,50 @@ __global__ void __launch_bounds__(128) k_line_fuse_search(int nml, const uint8_t
     if (lane == 0) { best_idx[i] = b == ~0ull ? -1 : (int)(b & 0xffffffffu); best_dist[i] = b == ~0ull ? 0x7fffffff : (int)(b >> 32); }
 }
 
-// Search stage of ORBmatcher::Fuse (ORBmatcher.cc:896-950): independent per MapPoint, one warp each over the grid cells of the window
+// Search stage of ORBmatcher::Fuse (ORBmatcher.cc:896-950): independent per MapPoint, one warp each over the grid cells of the window.
+// kMap: warp i runs entry i of a batched call (fuse_project_point, then the same search over keyframe k's sslpl_keypoint rows and grid;
+// monocular, a keyframe octave below 0 is never a candidate); false compiles the map out.
+template <bool kMap>
 __global__ void __launch_bounds__(128) k_point_fuse_search(const __grid_constant__ WinArgs A, int nmp, const uint8_t* active, const float* pu, const float* pv, const float* pur,
                                                             const int* level, const uint8_t* dmp, const uint8_t* d2, const float* x2, const float* y2, const int* oct2,
                                                             const float* uright2, const float* invSigma2, const int* goff, const int* gidx,
-                                                            int32_t* best_idx, int32_t* best_dist) {
+                                                            int32_t* best_idx, int32_t* best_dist, const __grid_constant__ FuseMap M) {
     const int i = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (i >= nmp) return;
+    constexpr int es = kMap ? 7 : 1;                     // keypoint fields: separate arrays or sslpl_keypoint rows
     unsigned long long b = ~0ull;
     int cx0 = 0, cx1 = -1, cy0 = 0, cy1 = -1;
-    if (active[i]) {
-        const int lvl = level[i];
-        const float u = pu[i], v = pv[i], ur = pur[i];
+    bool act;
+    int lvl;
+    float u, v, ur;
+    if (kMap) {
+        int k, e;
+        if (!fuse_entry(M, i, lane, k, e, best_idx, best_dist)) return;
+        act = e >= 0 && !(M.skip && M.skip[i]) && fuse_project_point(M, k, e, u, v, lvl);
+        ur = 0.f;
+        d2 = M.desc + k * M.desc_fs; x2 = M.kp + k * M.kp_fs; y2 = x2 + 1; oct2 = reinterpret_cast<const int*>(x2 + 5);
+        goff = M.goff + k * M.goff_fs; gidx = M.gidx + k * M.gidx_fs; invSigma2 = M.invSigma2; dmp = M.eldesc + (long long)e * 32;
+    } else {
+        act = active[i];
+        dmp += (long long)i * 32;
+    }
+    if (act) {
+        if (!kMap) { lvl = level[i]; u = pu[i]; v = pv[i]; ur = pur[i]; }
         const float rad = __fmul_rn(A.th, A.scale[lvl]);
         if (grid_window(A, u, v, rad, cx0, cx1, cy0, cy1)) {
             const int ny = cy1 - cy0 + 1, ncell = (cx1 - cx0 + 1) * ny;
             uint4 a0, a1;
-            load_desc(dmp + (long long)i * 32, a0, a1);
+            load_desc(dmp, a0, a1);
             for (int c = lane; c < ncell; c += 32) {
                 const int ix = cx0 + c / ny, iy = cy0 + c % ny, cell = ix * GRID_ROWS + iy;
                 const int qb = goff[cell], qe = goff[cell + 1];
                 for (int q = qb; q < qe; q++) {
                     const int j = gidx[q];
-                    const float kx = x2[j], ky = y2[j];
+                    const float kx = x2[es * j], ky = y2[es * j];
                     if (!(fabsf(__fsub_rn(kx, u)) < rad && fabsf(__fsub_rn(ky, v)) < rad)) continue;     // KeyFrame::GetFeaturesInArea KeyFrame.cc:642
-                    const int o = oct2[j];
+                    const int o = oct2[es * j];
                     if (o < lvl - 1 || o > lvl) continue;                                                 // :905
+                    if (kMap && o < 0) continue;
                     const float ex = __fsub_rn(u, kx), ey = __fsub_rn(v, ky);
                     float e2 = __fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey));
                     const float kr = A.use_right ? uright2[j] : -1.f;
@@ -1515,6 +1652,25 @@ int sslpl_search_by_projection_frame(sslpl_matcher* m,
     return SSLPL_OK;
 }
 
+// The per-frame grid workspace of the batched projection matchers ([max_batch + 1] frames), allocated by the first call that needs it
+// (a handle that never gets there never pays for it) and freed with the handle: per frame the grid cell of every feature and the grid
+// CSR, and the motion-model walker's claimed / sel / rbin tables.
+static int ensure_grid_ws(sslpl_matcher* m) {
+    if (m->pw) return SSLPL_OK;
+    const int B = m->p.max_batch + 1, fc = m->p.max_features + 64, nc = GRID_COLS * GRID_ROWS;
+    Arena W;
+    for (int k = 0; k < 2; k++) {
+        m->pw_cell = W.take<int32_t>((size_t)B * fc); m->pw_off = W.take<int>((size_t)B * (nc + 1)); m->pw_idx = W.take<int>((size_t)B * fc);
+        m->pw_sel = W.take<int32_t>((size_t)B * fc); m->pw_claimed = W.take<uint8_t>((size_t)B * fc); m->pw_rbin = W.take<uint8_t>((size_t)B * fc);
+        if (k == 0) {
+            cudaError_t e = cudaMalloc(&m->pw, W.used);
+            if (e != cudaSuccess) { m->pw = nullptr; set_error("cudaMalloc(%zu) failed: %s", W.used, cudaGetErrorString(e)); return SSLPL_ERR_CUDA; }
+            W.base = m->pw; W.size = W.used; W.used = 0;
+        }
+    }
+    return SSLPL_OK;
+}
+
 // The same matcher over consecutive frames in HBM (monocular: bMono = true, as Tracking passes it for a monocular sensor): pair p
 // projects frame p's MapPoints with frame p + 1's pose.  Grid cells of every current frame (frame on grid.y), one k_build_csr
 // launch for all of them, then one walker warp per pair, which also runs TrackWithMotionModel's 2 * th retry (Tracking.cc:1240-1244).
@@ -1532,19 +1688,8 @@ int sslpl_search_by_projection_frame_batch_device(sslpl_matcher* m, const sslpl_
     const int nc = GRID_COLS * GRID_ROWS, npairs = nframes - 1;
     SSLPL_REQUIRE((size_t)((nc + 1 + cap) * sizeof(int)) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "grid cells + features exceed the shared memory of one CTA ((3073 + cap) * 4 <= 200 KB)");
     SSLPL_CUDA(cudaSetDevice(m->p.device));
-    const int B = m->p.max_batch + 1, fc = m->p.max_features + 64;
-    if (!m->pw) {                                                        // first call: a handle that never gets here never pays for it
-        Arena W;
-        for (int k = 0; k < 2; k++) {
-            m->pw_cell = W.take<int32_t>((size_t)B * fc); m->pw_off = W.take<int>((size_t)B * (nc + 1)); m->pw_idx = W.take<int>((size_t)B * fc);
-            m->pw_sel = W.take<int32_t>((size_t)B * fc); m->pw_claimed = W.take<uint8_t>((size_t)B * fc); m->pw_rbin = W.take<uint8_t>((size_t)B * fc);
-            if (k == 0) {
-                cudaError_t e = cudaMalloc(&m->pw, W.used);
-                if (e != cudaSuccess) { m->pw = nullptr; set_error("cudaMalloc(%zu) failed: %s", W.used, cudaGetErrorString(e)); return SSLPL_ERR_CUDA; }
-                W.base = m->pw; W.size = W.used; W.used = 0;
-            }
-        }
-    }
+    const int fc = m->p.max_features + 64;
+    if (int rc = ensure_grid_ws(m)) return rc;
     cudaStream_t st = m->stream;
     ProjArgs A; memset(&A, 0, sizeof(A));
     A.fx = cam[0]; A.fy = cam[1]; A.cx = cam[2]; A.cy = cam[3];
@@ -1760,7 +1905,8 @@ int sslpl_fuse_lines_search(sslpl_matcher* m, int nml, const uint8_t* active, co
     int32_t* d_bi = A.take<int32_t>(nml + 8); int32_t* d_bd = A.take<int32_t>(nml + 8);
     SSLPL_CUDA(e);
     SSLPL_CUDA(cudaStreamSynchronize(st));
-    k_line_fuse_search<<<(nml + 3) / 4, 128, 0, st>>>(nml, d_act, reinterpret_cast<const float4*>(d_proj), d_lvl, d_dml, nl2, d_ld2, d_kl2, d_oct, d_sc, th, d_bi, d_bd);
+    FuseMap Z; memset(&Z, 0, sizeof(Z));
+    k_line_fuse_search<false><<<(nml + 3) / 4, 128, 0, st>>>(nml, d_act, reinterpret_cast<const float4*>(d_proj), d_lvl, d_dml, nl2, d_ld2, d_kl2, d_oct, d_sc, th, d_bi, d_bd, Z);
     m->launches++;
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(best_idx, d_bi, sizeof(int32_t) * nml, cudaMemcpyDeviceToHost, st));
@@ -1805,7 +1951,8 @@ int sslpl_fuse_points_search(sslpl_matcher* m, int nmp, const uint8_t* active, c
     k_grid_cells<<<(n2 + 127) / 128, 128, 0, st>>>(d_x2, d_y2, 1, 0, nullptr, n2, n2, A.minX, A.minY, A.invW, A.invH, m->node, 0);
     SSLPL_REQUIRE((size_t)((nc + 1 + cap) * sizeof(int)) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "nodes + features exceed the shared memory of one CTA ((nc + 1 + cap) * 4 <= 200 KB)");
     k_build_csr<<<1, 128, (nc + 1 + cap) * sizeof(int), st>>>(m->node, 0, m->ncnt, cap, nc, goff, 0, gidx, 0);
-    k_point_fuse_search<<<(nmp + 3) / 4, 128, 0, st>>>(A, nmp, d_act, d_u, d_v, d_ur, d_lvl, d_dmp, d_d2, d_x2, d_y2, d_oct, d_ur2, d_is2, goff, gidx, d_bi, d_bd);
+    FuseMap Z; memset(&Z, 0, sizeof(Z));
+    k_point_fuse_search<false><<<(nmp + 3) / 4, 128, 0, st>>>(A, nmp, d_act, d_u, d_v, d_ur, d_lvl, d_dmp, d_d2, d_x2, d_y2, d_oct, d_ur2, d_is2, goff, gidx, d_bi, d_bd, Z);
     m->launches += 3;
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(best_idx, d_bi, sizeof(int32_t) * nmp, cudaMemcpyDeviceToHost, st));
@@ -2071,6 +2218,124 @@ int sslpl_line_search_for_triangulation_batch_device(sslpl_matcher* m, const uin
                                                           m->b_knn, (long long)lc * 4, capl, pmap, nkf);
     k_line_tri<<<npairs, 256, 0, st>>>(m->b_knn, (long long)lc * 4, d_nl, capl, pmap, nkf, d_has_ml, d_lpairs, d_nlmatch);
     m->launches += 2;
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+// ---------------- PredictScale thresholds and LocalMapping::SearchInNeighbors' Fuse over keyframes in HBM (SURVEY.md 8(f) rows 2/3) ----------------
+// t_k = the smallest positive float r with (int)ceil(logf(r) / logScaleFactor) >= k, by bisection over the bit patterns of the positive
+// floats with this process's logf (+inf when no finite r gets there).  The level is compared in float: for any logScaleFactor of a float
+// scale factor > 1 (>= 1.19e-7) |ceil(logf(r) / s)| < 2^31, where the float compare and the int conversion agree.
+int sslpl_predict_scale_table(float logScaleFactor, int nlevels, float* thr) {
+    SSLPL_REQUIRE(thr, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nlevels >= 1 && nlevels <= SSLPL_MAX_LEVELS, SSLPL_ERR_ARG, "nlevels outside [1, SSLPL_MAX_LEVELS]");
+    SSLPL_REQUIRE(logScaleFactor > 0.f && logScaleFactor < INFINITY, SSLPL_ERR_ARG, "logScaleFactor must be positive and finite");
+    for (int k = 0; k <= nlevels; k++) {
+        uint32_t lo = 1, hi = 0x7f800000u;                                // hi = +inf: never evaluated
+        while (lo < hi) {
+            const uint32_t mid = lo + (hi - lo) / 2;
+            float r; memcpy(&r, &mid, 4);
+            if (std::ceil(logf(r) / logScaleFactor) >= (float)k) hi = mid; else lo = mid + 1;
+        }
+        memcpy(&thr[k], &lo, 4);
+    }
+    return SSLPL_OK;
+}
+
+static int predict_table(PredictTable& T, float logScaleFactor, int nlevels) {
+    memset(&T, 0, sizeof(T));
+    T.nlevels = nlevels;
+    return sslpl_predict_scale_table(logScaleFactor, nlevels, T.thr);
+}
+
+int sslpl_matcher_debug_predict_scale(sslpl_matcher* m, int n, const float* ratio, float logScaleFactor, int nlevels, int clamp, int32_t* level) {
+    SSLPL_REQUIRE(m && n >= 0 && (n == 0 || (ratio && level)), SSLPL_ERR_ARG, "null argument");
+    PredictTable T;
+    if (int rc = predict_table(T, logScaleFactor, nlevels)) return rc;
+    if (n == 0) return SSLPL_OK;
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    cudaStream_t st = m->stream;
+    if (int rc = ensure_scratch(m, (size_t)n * 8 + 1024)) return rc;
+    Arena A; A.base = m->scratch; A.used = 0;
+    cudaError_t e = cudaSuccess;
+    float* d_r = stage(A, ratio, n, st, e); int32_t* d_l = A.take<int32_t>(n + 8);
+    SSLPL_CUDA(e);
+    k_predict_scale<<<(n + 255) / 256, 256, 0, st>>>(n, d_r, T, clamp, d_l);
+    m->launches++;
+    SSLPL_CUDA(cudaGetLastError());
+    SSLPL_CUDA(cudaMemcpyAsync(level, d_l, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
+    SSLPL_CUDA(cudaStreamSynchronize(st));
+    return SSLPL_OK;
+}
+
+static int fuse_map_common(FuseMap& M, sslpl_matcher* m, int nkf, int nel, int nentries, const int32_t* d_entry, const uint8_t* d_skip,
+                           const float* d_kfpose, const float* d_el, const uint8_t* d_eldesc, const float* cam, const float* bounds,
+                           const float* scaleFactors, int nlevels, float logScaleFactor) {
+    SSLPL_REQUIRE(d_entry && d_kfpose && d_el && d_eldesc && cam && bounds && scaleFactors, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nkf >= 1 && nkf <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nkf outside [1, max_batch + 1]");
+    SSLPL_REQUIRE(nel >= 0 && nentries >= 0, SSLPL_ERR_ARG, "negative count");
+    SSLPL_REQUIRE(nlevels >= 1 && nlevels <= SSLPL_MAX_LEVELS, SSLPL_ERR_ARG, "nlevels outside [1, SSLPL_MAX_LEVELS]");
+    SSLPL_REQUIRE(bounds[1] > bounds[0] && bounds[3] > bounds[2], SSLPL_ERR_ARG, "degenerate image bounds");
+    memset(&M, 0, sizeof(M));
+    if (int rc = predict_table(M.T, logScaleFactor, nlevels)) return rc;
+    M.entry = reinterpret_cast<const int2*>(d_entry); M.skip = d_skip; M.nkf = nkf; M.nel = nel;
+    M.pose = d_kfpose; M.el = d_el; M.eldesc = d_eldesc;
+    M.fx = cam[0]; M.fy = cam[1]; M.cx = cam[2]; M.cy = cam[3];
+    M.minX = bounds[0]; M.maxX = bounds[1]; M.minY = bounds[2]; M.maxY = bounds[3];
+    for (int k = 0; k < nlevels; k++) M.scale[k] = scaleFactors[k];
+    return SSLPL_OK;
+}
+
+// ORBmatcher::Fuse(pKF, vpMapPoints, th) for a flat list of (keyframe, MapPoint) entries: the 64 x 48 grid of every keyframe (frame on
+// grid.y, one k_build_csr CTA per keyframe), then one warp per entry: projection stage and search (k_point_fuse_search<true>).
+int sslpl_fuse_points_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nkf, int cap, const float* d_kfpose,
+        int nmp, const float* d_mp, const uint8_t* d_mpdesc, int nentries, const int32_t* d_entry, const uint8_t* d_skip,
+        const float* cam, const float* bounds, const float* scaleFactors, const float* invLevelSigma2, int nlevels, float logScaleFactor, float th,
+        int32_t* d_best_idx, int32_t* d_best_dist) {
+    SSLPL_REQUIRE(m && d_kps && d_desc && d_n && invLevelSigma2 && d_best_idx && d_best_dist, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(cap >= 1 && cap <= m->p.max_features + 64, SSLPL_ERR_ARG, "cap outside [1, max_features + 64]");
+    const int nc = GRID_COLS * GRID_ROWS;
+    SSLPL_REQUIRE((size_t)((nc + 1 + cap) * sizeof(int)) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "grid cells + features exceed the shared memory of one CTA ((3073 + cap) * 4 <= 200 KB)");
+    FuseMap M;
+    if (int rc = fuse_map_common(M, m, nkf, nmp, nentries, d_entry, d_skip, d_kfpose, d_mp, d_mpdesc, cam, bounds, scaleFactors, nlevels, logScaleFactor)) return rc;
+    if (nentries == 0) return SSLPL_OK;
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    if (int rc = ensure_grid_ws(m)) return rc;
+    const int fc = m->p.max_features + 64;
+    for (int k = 0; k < nlevels; k++) M.invSigma2[k] = invLevelSigma2[k];
+    const float* kf = reinterpret_cast<const float*>(d_kps);              // sslpl_keypoint = 7 x 4 B: x y size angle response octave class_id
+    M.kp = kf; M.kp_fs = 7LL * cap; M.desc = d_desc; M.desc_fs = 32LL * cap; M.n = d_n; M.cap = cap;
+    M.goff = m->pw_off; M.gidx = m->pw_idx; M.goff_fs = nc + 1; M.gidx_fs = fc;
+    WinArgs A; fill_win(A, bounds, scaleFactors, nlevels);
+    A.th = th;
+    cudaStream_t st = m->stream;
+    k_grid_cells<<<dim3((cap + 127) / 128, nkf), 128, 0, st>>>(kf, kf + 1, 7, M.kp_fs, d_n, 0, cap, A.minX, A.minY, A.invW, A.invH, m->pw_cell, fc);
+    k_build_csr<<<nkf, 128, (nc + 1 + cap) * sizeof(int), st>>>(m->pw_cell, fc, d_n, cap, nc, m->pw_off, nc + 1, m->pw_idx, fc);
+    k_point_fuse_search<true><<<(nentries + 3) / 4, 128, 0, st>>>(A, nentries, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                                                  nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, d_best_idx, d_best_dist, M);
+    m->launches += 3;
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+// LSDmatcher::Fuse(pKF, vpMapLines, th) for a flat list of (keyframe, MapLine) entries: one warp per entry, projection stage and search
+// over the keyframe's sslpl_keyline rows (k_line_fuse_search<true>).
+int sslpl_fuse_lines_batch_device(sslpl_matcher* m,
+        const sslpl_keyline* d_kl, const uint8_t* d_ldesc, const int* d_nl, int nkf, int capl, const float* d_kfpose,
+        int nml, const float* d_ml, const uint8_t* d_mldesc, int nentries, const int32_t* d_entry, const uint8_t* d_skip,
+        const float* cam, const float* bounds, const float* scaleFactors, int nlevels, float logScaleFactor, float th,
+        int32_t* d_best_idx, int32_t* d_best_dist) {
+    SSLPL_REQUIRE(m && d_kl && d_ldesc && d_nl && d_best_idx && d_best_dist, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(capl >= 1 && capl <= m->p.max_lines + 64, SSLPL_ERR_ARG, "capl outside [1, max_lines + 64]");
+    FuseMap M;
+    if (int rc = fuse_map_common(M, m, nkf, nml, nentries, d_entry, d_skip, d_kfpose, d_ml, d_mldesc, cam, bounds, scaleFactors, nlevels, logScaleFactor)) return rc;
+    if (nentries == 0) return SSLPL_OK;
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    M.kp = reinterpret_cast<const float*>(d_kl); M.kp_fs = 17LL * capl; M.desc = d_ldesc; M.desc_fs = 32LL * capl; M.n = d_nl; M.cap = capl;
+    k_line_fuse_search<true><<<(nentries + 3) / 4, 128, 0, m->stream>>>(nentries, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, th,
+                                                                        d_best_idx, d_best_dist, M);
+    m->launches++;
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
