@@ -424,8 +424,9 @@ long long sslpl_line_launch_count(const sslpl_line* h);
    call keeps resident (0 = one per frame, the default).  Useful when several handles are in flight on one GPU next to wide
    kernels: resident walkers pin registers for milliseconds. */
 int  sslpl_line_set_max_walkers(sslpl_line* h, int max_concurrent);
-/* Statistics of the last region-walker launch, 16 values (see csrc/line.cu): regions grown by the turn holder / as speculated,
-   redo causes, cycles under the commit and claim locks, cycles per frame.  Diagnostic only. */
+/* Statistics of the last multi-warp region-walker launch, 16 values (see csrc/line.cu): regions grown by the turn holder / as
+   speculated, redo causes, cycles under the commit and claim locks, cycles per frame.  The one-warp walker leaves them 0.
+   Diagnostic only. */
 int  sslpl_line_walker_stats(sslpl_line* h, unsigned long long* out16);
 int  sslpl_line_set_profiling(sslpl_line* h, int on);
 int  sslpl_line_stage_ms(sslpl_line* h, float* ms, int cap, const char** names, int* nstages);

@@ -129,8 +129,7 @@ class Coverage:
 
 
 def _trace_env(monkeypatch, env=None):
-    for k in ("SSLPL_WALKER_WARPS", "SSLPL_WALKER_LEAN", "SSLPL_WALKER_V3", "SSLPL_WALKER_LANES"):
-        monkeypatch.delenv(k, raising=False)
+    monkeypatch.delenv("SSLPL_WALKER_WARPS", raising=False)
     monkeypatch.setenv("SSLPL_LINE_TRACE", "1")
     for k, v in (env or {}).items():
         monkeypatch.setenv(k, v)
@@ -154,7 +153,7 @@ def test_single_frames_region_by_region(pkg, oracle, synth, icl_gray, monkeypatc
 
 @pytest.mark.parametrize("name,env", WALKERS, ids=[w[0] for w in WALKERS])
 def test_every_walker_region_by_region(pkg, oracle, synth, icl_gray, monkeypatch, name, env):
-    """Each region-walker form, forced, on a subset: the multi-warp forms are timing dependent, so two runs each."""
+    """Each region-walker form and warp count, forced, on a subset: the multi-warp walker is timing dependent, so two runs each."""
     _trace_env(monkeypatch, env)
     rng = np.random.default_rng(5)
     frames = [("icl", icl_gray), ("syn640/3", synth.frame(640, 480, 3)), ("lines 0.5 deg", _lines(640, 480, 0.5, 1)),
