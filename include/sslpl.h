@@ -341,6 +341,55 @@ int  sslpl_line_search_for_triangulation_batch_device(sslpl_matcher* m,
         const uint8_t* d_ldesc, const int* d_nl, int nkf, int capl, const uint8_t* d_has_ml,
         int npairs, const int32_t* d_pair, int32_t* d_lpairs, int32_t* d_nlmatch);
 
+/* ---- LocalMapping::CreateNewMapPoints (LocalMapping.cc:371-637, monocular) over keyframe pairs in HBM: the matcher and the
+   triangulation of every neighbour, neighbour after neighbour.  Same keyframe set, vocabulary, d_has_mp, pair list and d_geom as
+   sslpl_search_for_triangulation_batch_device (checkOrientation is false, as LocalMapping's ORBmatcher(0.6, false) has it), plus
+   d_kfpose[k][15] = Tcw (3x4 row-major) then Ow, f32 (the pose table of the batched Fuse calls), the HOST cam[6] = fx fy cx cy invfx invfy
+   (as the KeyFrame holds them, one camera for all keyframes), scaleFactors / levelSigma2 = mvScaleFactors / mvLevelSigma2 (HOST, nlevels
+   entries) and scaleFactor = mfScaleFactor.
+   Chains: a maximal run of consecutive pairs with the same kf1 is one keyframe's neighbour loop, in GetBestCovisibilityKeyFrames order.
+   Inside a chain the pairs run strictly in order: the KF1 features that have a MapPoint start as d_has_mp[kf1] and gain the idx1 of
+   every created row (KeyFrame::AddMapPoint(pMP, idx1), :624), which the matcher of the later pairs then skips (ORBmatcher.cc:702-706).
+   Chains are independent, and the inputs are never modified.  The first k pairs of a chain give what a call with only those pairs
+   gives (a neighbour loop that stops at CheckNewKeyFrames, :408).  A pair with an index outside [0, nkf), with kf2 == kf1 or with a kf2
+   that an earlier pair of its chain had gets the count -1, no rows, and leaves the chain's state alone.
+   Results per pair p, `cap` rows each:
+     d_pairs[p][cap][2]  (idx1, idx2) in ascending idx1: what SearchForTriangulation returns under the mask of that neighbour; (-1, -1)
+                         after the count;
+     d_nmatch[p]         the row count (-1: bad pair);
+     d_status[p][cap]    per row SSLPL_CNMP_CREATED (0) or the test that rejected it, SSLPL_CNMP_*; -1 after the count;
+     d_x3d[p][cap][3]    the triangulated point x3D (f32), written for every row that got past the w == 0 test (status 0 or >= 3);
+                         other rows are not written;
+     d_nnew[p]           the rows with status 0.
+   The rows with status 0, in (pair, row) order, are the reference's MapPoint creation order.  Two created rows of one pair may share
+   an idx2 (nothing marks a KF2 feature as taken): KF2's slot then ends with the later one (pKF2->AddMapPoint overwrites), so a caller
+   applies them in order.  Numerics are those of the reference with cv2 4.13 and glibc >= 2.35: the 4x4 cv::SVD is OpenCV's one-sided
+   Jacobi, its hypot glibc's; see DESIGN.md.  A KF1 keypoint whose octave is outside [0, nlevels) gets SSLPL_CNMP_OCTAVE1 (the
+   reference indexes mvLevelSigma2 out of bounds).  Asynchronous on the matcher's stream; bad arguments return SSLPL_ERR_ARG and enqueue
+   nothing. ---- */
+enum {
+    SSLPL_CNMP_CREATED = 0,    /* the MapPoint is created (:619-634) */
+    SSLPL_CNMP_PARALLAX = 1,   /* cosParallaxRays not in (0, 0.9998) (:497, :526) */
+    SSLPL_CNMP_W_ZERO = 2,     /* vt.row(3)(3) == 0 (:511) */
+    SSLPL_CNMP_Z1 = 3,         /* depth in KF1 <= 0 (:533-535) */
+    SSLPL_CNMP_Z2 = 4,         /* depth in KF2 <= 0 (:537-539) */
+    SSLPL_CNMP_OCTAVE1 = 5,    /* KF1 keypoint octave outside [0, nlevels) (:543) */
+    SSLPL_CNMP_REPROJ1 = 6,    /* reprojection chi2 in KF1 > 5.991 sigma2 (:549-559) */
+    SSLPL_CNMP_REPROJ2 = 7,    /* reprojection chi2 in KF2 > 5.991 sigma2 (:578-586) */
+    SSLPL_CNMP_DIST0 = 8,      /* dist1 == 0 || dist2 == 0 (:607) */
+    SSLPL_CNMP_SCALE = 9       /* scale consistency (:615) */
+};
+int  sslpl_create_new_map_points_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nkf, int cap,
+        const uint8_t* d_has_mp, const sslpl_vocab* v, int levelsup,
+        int npairs, const int32_t* d_pair, const float* d_geom, const float* d_kfpose,
+        const float* cam, const float* scaleFactors, const float* levelSigma2, int nlevels, float scaleFactor,
+        int32_t* d_pairs, int32_t* d_nmatch, int32_t* d_status, float* d_x3d, int32_t* d_nnew);
+/* The device functions of that call on HOST tables: the 4x4 SVD of n row-major matrices A[n][16] -> W[n][4] (descending) and
+   Vt[n][16] (cv::SVD::compute(A, w, u, vt, MODIFY_A | FULL_UV) on CV_32F), and glibc's hypot of nh pairs -> h[nh].  Synchronous. */
+int  sslpl_matcher_debug_svd4(sslpl_matcher* m, int n, const float* A, float* W, float* Vt,
+                              int nh, const double* hx, const double* hy, double* h);
+
 /* ---- MapPoint::PredictScale / MapLine::PredictScale (MapPoint.cc:390-405, MapLine.cpp:386-395) on the device, exact against the host's
    logf: level = (int)ceil(logf(ratio) / logScaleFactor), ratio = mfMaxDistance / dist.  The level is a monotone step function of the float
    ratio; thr[k] (k = 0 .. nlevels, nlevels + 1 floats) is the smallest positive float whose level is >= k, found by bisection over the

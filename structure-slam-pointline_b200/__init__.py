@@ -484,6 +484,33 @@ class Matcher:
             self._h, C.c_void_p(d_ldesc), C.c_void_p(d_nl), int(nkf), int(capl), C.c_void_p(d_has_ml), int(npairs), C.c_void_p(d_pair),
             C.c_void_p(d_lpairs), C.c_void_p(d_nlmatch)))
 
+    def create_new_map_points_batch_device(self, d_kps, d_desc, d_n, nkf, cap, d_has_mp, vocab, levelsup, npairs, d_pair, d_geom, d_kfpose,
+                                           cam, scale_factors, level_sigma2, scale_factor, d_pairs, d_nmatch, d_status, d_x3d, d_nnew):
+        """LocalMapping::CreateNewMapPoints (LocalMapping.cc:371-637, monocular) for the chains of a pair list in HBM: per pair the
+        SearchForTriangulation rows under the mask the reference sees at that neighbour, a status per row and the triangulated point
+        (see sslpl_create_new_map_points_batch_device).  Inputs as search_for_triangulation_batch_device, plus d_kfpose [nkf, 15] f32 (Tcw
+        3x4, Ow) and host cam = fx fy cx cy invfx invfy, scale_factors / level_sigma2 (nlevels = len) and scale_factor -> d_pairs [npairs,
+        cap, 2], d_nmatch [npairs], d_status [npairs, cap] i32, d_x3d [npairs, cap, 3] f32, d_nnew [npairs].  Asynchronous."""
+        f32 = lambda a: np.ascontiguousarray(a, np.float32)
+        sc = f32(scale_factors); s2 = f32(level_sigma2); cm = f32(cam)
+        assert len(s2) >= len(sc) and len(cm) == 6
+        _check(lib().sslpl_create_new_map_points_batch_device(
+            self._h, C.c_void_p(d_kps), C.c_void_p(d_desc), C.c_void_p(d_n), int(nkf), int(cap), C.c_void_p(d_has_mp), vocab._h,
+            int(levelsup), int(npairs), C.c_void_p(d_pair), C.c_void_p(d_geom), C.c_void_p(d_kfpose), _p(cm), _p(sc), _p(s2), len(sc),
+            C.c_float(scale_factor), C.c_void_p(d_pairs), C.c_void_p(d_nmatch), C.c_void_p(d_status), C.c_void_p(d_x3d), C.c_void_p(d_nnew)))
+
+    def debug_svd4(self, A, hx=None, hy=None):
+        """The device's 4x4 SVD (cv::SVD::compute on CV_32F) of host matrices A [n, 4, 4] -> (W [n, 4], Vt [n, 4, 4]), and its glibc
+        hypot of hx, hy (float64) -> h.  Synchronous."""
+        A = np.ascontiguousarray(A, np.float32).reshape(-1, 16)
+        hx = np.ascontiguousarray(hx if hx is not None else [], np.float64).reshape(-1)
+        hy = np.ascontiguousarray(hy if hy is not None else [], np.float64).reshape(-1)
+        assert hx.shape == hy.shape
+        n, nh = len(A), len(hx)
+        W = np.empty((max(n, 1), 4), np.float32); Vt = np.empty((max(n, 1), 4, 4), np.float32); h = np.empty(max(nh, 1), np.float64)
+        _check(lib().sslpl_matcher_debug_svd4(self._h, n, _p(A), _p(W), _p(Vt), nh, _p(hx), _p(hy), _p(h)))
+        return W[:n], Vt[:n], h[:nh]
+
     def fuse_points_batch_device(self, d_kps, d_desc, d_n, nkf, cap, d_kfpose, nmp, d_mp, d_mpdesc, nentries, d_entry, d_skip,
                                  cam, bounds, scale_factors, inv_level_sigma2, log_scale_factor, th, d_best_idx, d_best_dist):
         """ORBmatcher::Fuse(pKF, vpMapPoints, th) (ORBmatcher.cc:828-973, monocular) for a flat list of (keyframe, MapPoint) entries in

@@ -6,6 +6,7 @@
 // 2 x uint4 per row.  The batched layout is "a set of frames": frame f owns desc[f*cap..], a CSR feature
 // vector and optional masks; pair p matches frame p (KeyFrame role) against frame p+1 (Frame role).
 #include "common.cuh"
+#include "svd4.cuh"
 #include <algorithm>
 #include <climits>
 #include <cmath>
@@ -706,14 +707,16 @@ __global__ void k_predict_scale(int n, const float* ratio, const __grid_constant
 __device__ __forceinline__ float rt_row(const float* T, float x0, float x1, float x2) {
     return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[0], x0), __fmul_rn(T[1], x1)), __fmul_rn(T[2], x2)), T[3]);
 }
-// (float)cv::norm(d) (double accumulation) and the double dot product with the normal of the viewing-angle gate
-__device__ __forceinline__ float norm3d(float d0, float d1, float d2) {
-    return __double2float_rn(__dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn((double)d0, (double)d0), __dmul_rn((double)d1, (double)d1)),
-                                                  __dmul_rn((double)d2, (double)d2))));
+// Mat::dot of two float rows of 3 (double products and sum; the reference's sum starts from 0.0, which changes only the sign of an
+// exact zero, and no caller reads that sign), cv::norm (double accumulation, the double it returns) and (float)cv::norm(d), and the
+// double dot product with the normal of the viewing-angle gate
+__device__ __forceinline__ double dot3d(float a0, float a1, float a2, float b0, float b1, float b2) {
+    return __dadd_rn(__dadd_rn(__dmul_rn((double)a0, (double)b0), __dmul_rn((double)a1, (double)b1)), __dmul_rn((double)a2, (double)b2));
 }
+__device__ __forceinline__ double norm3d_d(float d0, float d1, float d2) { return __dsqrt_rn(dot3d(d0, d1, d2, d0, d1, d2)); }
+__device__ __forceinline__ float norm3d(float d0, float d1, float d2) { return __double2float_rn(norm3d_d(d0, d1, d2)); }
 __device__ __forceinline__ bool view_ok(float d0, float d1, float d2, float n0, float n1, float n2, float dist) {
-    const double dot = __dadd_rn(__dadd_rn(__dmul_rn((double)d0, (double)n0), __dmul_rn((double)d1, (double)n1)), __dmul_rn((double)d2, (double)n2));
-    return !(dot < __dmul_rn(0.5, (double)dist));
+    return !(dot3d(d0, d1, d2, n0, n1, n2) < __dmul_rn(0.5, (double)dist));
 }
 
 // Where the batched Fuse calls read: entry e = (keyframe, element) pair, the keyframe set (strides in elements of its arrays), the
@@ -1156,6 +1159,160 @@ __global__ void __launch_bounds__(256) k_line_tri(const int32_t* knn, long long 
     }
     for (int i = total + tid; i < capl; i += 256) { O[2 * i] = -1; O[2 * i + 1] = -1; }
     if (tid == 0) nlmatch[p] = ok ? total : -1;
+}
+
+// ---------------- LocalMapping::CreateNewMapPoints' neighbour loop (LocalMapping.cc:371-637, monocular) ----------------
+// Status codes of include/sslpl.h (SSLPL_CNMP_*), one per `continue` of the per-match body in reference order.
+enum { CNMP_CREATED = 0, CNMP_PARALLAX, CNMP_W_ZERO, CNMP_Z1, CNMP_Z2, CNMP_OCTAVE1, CNMP_REPROJ1, CNMP_REPROJ2, CNMP_DIST0, CNMP_SCALE };
+
+struct CreateArgs {
+    float fx, fy, cx, cy, invfx, invfy;   // KeyFrame::fx .. invfy (one camera for both keyframes)
+    float ratioFactor;                    // 1.5f * mfScaleFactor (:400)
+    int nlevels;
+    float scale[SSLPL_MAX_LEVELS], sigma2[SSLPL_MAX_LEVELS];
+};
+
+// cv::addWeighted(a, alpha, b, -1, 0) of CV_32F, as tools/probe_cv_matexpr.py measured it: in double, rounded once
+__device__ __forceinline__ float add_weighted_m1(float a, float alpha, float b) {
+    return __double2float_rn(__dadd_rn(__dadd_rn(__dmul_rn((double)a, (double)alpha), -(double)b), 0.0));
+}
+// float(Rcw.row(r).dot(x3Dt) + tcw.at<float>(r)) for row r = T[0..3] of a pose (:533, :545)
+__device__ __forceinline__ float cam_row(const float* T, const float* X) {
+    return __double2float_rn(__dadd_rn(dot3d(T[0], T[1], T[2], X[0], X[1], X[2]), (double)T[3]));
+}
+// Rwc * xn (cv::gemm's float path) with Rwc = Rcw.t(): column i of Rcw
+__device__ __forceinline__ void ray(const float* T, const float* xn, float* r) {
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+        r[i] = __fadd_rn(__fadd_rn(__fmul_rn(T[i], xn[0]), __fmul_rn(T[4 + i], xn[1])), __fmul_rn(T[8 + i], xn[2]));
+}
+// the monocular reprojection chi-square test (:549-558 / :578-585): true = rejected
+__device__ __forceinline__ bool reproj_bad(const CreateArgs& C, const float* T, const float* X, float z, float kx, float ky, float sigma2) {
+    const float x = cam_row(T, X), y = cam_row(T + 4, X);
+    const float invz = __double2float_rn(__ddiv_rn(1.0, (double)z));                                   // const float invz = 1.0 / z
+    const float u = __fadd_rn(__fmul_rn(__fmul_rn(C.fx, x), invz), C.cx), v = __fadd_rn(__fmul_rn(__fmul_rn(C.fy, y), invz), C.cy);
+    const float ex = __fsub_rn(u, kx), ey = __fsub_rn(v, ky);
+    return (double)__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)) > __dmul_rn(5.991, (double)sigma2);
+}
+
+// The per-match body of CreateNewMapPoints (:459-634) for KF1 keypoint (x1, y1, o1) and KF2 keypoint (x2, y2, o2) with poses T1 / T2
+// (pose[15] = Tcw 3x4 row-major, Ow) -> status; X is set when the row gets past the w == 0 test (*written = true).
+__device__ __forceinline__ int create_point(const CreateArgs& C, const float* T1, const float* T2, float x1, float y1, int o1,
+                                            float x2, float y2, int o2, float* X, bool* written) {
+    *written = false;
+    const float xn1[3] = {__fmul_rn(__fsub_rn(x1, C.cx), C.invfx), __fmul_rn(__fsub_rn(y1, C.cy), C.invfy), 1.f};   // :475-476
+    const float xn2[3] = {__fmul_rn(__fsub_rn(x2, C.cx), C.invfx), __fmul_rn(__fsub_rn(y2, C.cy), C.invfy), 1.f};
+    float r1[3], r2[3];
+    ray(T1, xn1, r1); ray(T2, xn2, r2);                                                                          // :479-480
+    const float cosp = __double2float_rn(__ddiv_rn(dot3d(r1[0], r1[1], r1[2], r2[0], r2[1], r2[2]),
+                                                   __dmul_rn(norm3d_d(r1[0], r1[1], r1[2]), norm3d_d(r2[0], r2[1], r2[2]))));   // :482
+    if (!(cosp < __fadd_rn(cosp, 1.f) && cosp > 0.f && (double)cosp < 0.9998)) return CNMP_PARALLAX;             // :484-497, :526
+    float A[16], W[4], Vt[16];
+#pragma unroll
+    for (int k = 0; k < 4; k++) {                                                                                // :500-504
+        A[k] = add_weighted_m1(T1[8 + k], xn1[0], T1[k]);
+        A[4 + k] = add_weighted_m1(T1[8 + k], xn1[1], T1[4 + k]);
+        A[8 + k] = add_weighted_m1(T2[8 + k], xn2[0], T2[k]);
+        A[12 + k] = add_weighted_m1(T2[8 + k], xn2[1], T2[4 + k]);
+    }
+    svd4_jacobi(A, W, Vt);                                                                                       // :506-509
+    if (Vt[15] == 0.f) return CNMP_W_ZERO;                                                                       // :511
+    const float inv = __double2float_rn(__ddiv_rn(1.0, (double)Vt[15]));                                         // :515, convertTo
+#pragma unroll
+    for (int k = 0; k < 3; k++) X[k] = __fadd_rn(__fmul_rn(Vt[12 + k], inv), 0.f);
+    *written = true;
+    const float z1 = cam_row(T1 + 8, X);                                                                         // :533-539
+    if (z1 <= 0.f) return CNMP_Z1;
+    const float z2 = cam_row(T2 + 8, X);
+    if (z2 <= 0.f) return CNMP_Z2;
+    if ((unsigned)o1 >= (unsigned)C.nlevels) return CNMP_OCTAVE1;                                                // mvLevelSigma2[kp1.octave]
+    if (reproj_bad(C, T1, X, z1, x1, y1, C.sigma2[o1])) return CNMP_REPROJ1;
+    if (reproj_bad(C, T2, X, z2, x2, y2, C.sigma2[o2])) return CNMP_REPROJ2;
+    const float dist1 = norm3d(__fsub_rn(X[0], T1[12]), __fsub_rn(X[1], T1[13]), __fsub_rn(X[2], T1[14]));       // :601-605
+    const float dist2 = norm3d(__fsub_rn(X[0], T2[12]), __fsub_rn(X[1], T2[13]), __fsub_rn(X[2], T2[14]));
+    if (dist1 == 0.f || dist2 == 0.f) return CNMP_DIST0;
+    const float ratioDist = __fdiv_rn(dist2, dist1), ratioOctave = __fdiv_rn(C.scale[o1], C.scale[o2]);           // :610-616
+    if (__fmul_rn(ratioDist, C.ratioFactor) < ratioOctave || ratioDist > __fmul_rn(ratioOctave, C.ratioFactor)) return CNMP_SCALE;
+    return CNMP_CREATED;
+}
+
+// One CTA per chain (a maximal run of consecutive pairs with the same kf1: one keyframe's neighbour loop); CTAs that do not start a chain
+// return at once.  The KF1 features that have a MapPoint are a bitmap in shared memory, loaded from has_mp; for each pair in order the
+// CTA drops the unfiltered SearchForTriangulation rows (tw[p][idx1] = idx2 or -1) whose idx1 is set, compacts the rest in ascending idx1
+// (block scan), triangulates one row per thread and sets the bits of the created rows (AddMapPoint(pMP, idx1), :624) before the next pair.
+// A pair with an index outside [0, nkf), kf2 == kf1 or a kf2 repeated in its chain gets count -1 and leaves the bitmap alone.
+__global__ void __launch_bounds__(256, 1) k_create_points_chain(const int2* pmap, int npairs, int nkf, const int32_t* tw, int cap,
+        const float* kp, const int* n_arr, const uint8_t* has_mp, const float* pose, const __grid_constant__ CreateArgs C,
+        int32_t* rows, int32_t* nmatch, int32_t* status, float* x3d, int32_t* nnew) {
+    extern __shared__ unsigned s_bits[];
+    __shared__ int s_warp[33];
+    const int c0 = blockIdx.x, tid = threadIdx.x;
+    const int kf1 = pmap[c0].x;
+    if (c0 > 0 && pmap[c0 - 1].x == kf1) return;
+    int c1 = c0 + 1;
+    while (c1 < npairs && pmap[c1].x == kf1) c1++;
+    const bool ok1 = (unsigned)kf1 < (unsigned)nkf;
+    const int n1 = ok1 ? max(0, min(n_arr[kf1], cap)) : 0, words = (cap + 31) / 32;
+    for (int w = tid; w < words; w += 256) {
+        unsigned b = 0;
+        for (int k = 0; k < 32 && ok1 && 32 * w + k < cap; k++) b |= (has_mp[(long long)kf1 * cap + 32 * w + k] != 0) << k;
+        s_bits[w] = b;
+    }
+    __syncthreads();
+    const float* K1 = kp + 7LL * cap * (ok1 ? kf1 : 0);
+    for (int p = c0; p < c1; p++) {
+        const int kf2 = pmap[p].y;
+        bool bad = !ok1 || (unsigned)kf2 >= (unsigned)nkf || kf2 == kf1;
+        for (int q = c0; q < p && !bad; q++) bad = pmap[q].y == kf2;
+        int32_t* R = rows + 2LL * cap * p; int32_t* S = status + (long long)cap * p; float* X3 = x3d + 3LL * cap * p;
+        int total = 0, created = 0;
+        if (!bad) {                                                              // CTA-uniform
+            const int32_t* Tw = tw + (long long)cap * p;
+            const int chunk = (n1 + 255) / 256, pb = min(n1, tid * chunk), pe = min(n1, pb + chunk);
+            int c = 0;
+            for (int i = pb; i < pe; i++) c += Tw[i] >= 0 && !((s_bits[i >> 5] >> (i & 31)) & 1u);
+            int o = block_exclusive_scan(c, s_warp, &total);
+            for (int i = pb; i < pe; i++)
+                if (Tw[i] >= 0 && !((s_bits[i >> 5] >> (i & 31)) & 1u)) { R[2 * o] = i; R[2 * o + 1] = Tw[i]; o++; }
+            __syncthreads();                                                     // the rows (global) and every bitmap read are done
+            const float* K2 = kp + 7LL * cap * kf2;
+            const float* T1 = pose + 15LL * kf1; const float* T2 = pose + 15LL * kf2;
+            float t1[15], t2[15];
+#pragma unroll
+            for (int k = 0; k < 15; k++) { t1[k] = T1[k]; t2[k] = T2[k]; }
+            for (int r = tid; r < total; r += 256) {
+                const int i1 = R[2 * r], i2 = R[2 * r + 1];
+                float X[3]; bool written;
+                const int st = create_point(C, t1, t2, K1[7 * i1], K1[7 * i1 + 1], __float_as_int(K1[7 * i1 + 5]),
+                                            K2[7 * i2], K2[7 * i2 + 1], __float_as_int(K2[7 * i2 + 5]), X, &written);
+                S[r] = st;
+                if (written) { X3[3 * r] = X[0]; X3[3 * r + 1] = X[1]; X3[3 * r + 2] = X[2]; }
+                if (st == CNMP_CREATED) { atomicOr(&s_bits[i1 >> 5], 1u << (i1 & 31)); created++; }
+            }
+            int all;
+            block_exclusive_scan(created, s_warp, &all);
+            created = all;
+        }
+        for (int i = total + tid; i < cap; i += 256) { R[2 * i] = -1; R[2 * i + 1] = -1; S[i] = -1; }
+        if (tid == 0) { nmatch[p] = bad ? -1 : total; nnew[p] = created; }
+        __syncthreads();
+    }
+}
+
+// sslpl_matcher_debug_svd4: svd4_jacobi on n row-major 4x4 matrices (W, Vt), glibc_hypot on nh pairs
+__global__ void k_debug_svd4(int n, const float* A, float* W, float* Vt, int nh, const double* hx, const double* hy, double* h) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) {
+        float a[16], w[4], v[16];
+#pragma unroll
+        for (int k = 0; k < 16; k++) a[k] = A[16LL * i + k];
+        svd4_jacobi(a, w, v);
+#pragma unroll
+        for (int k = 0; k < 4; k++) W[4LL * i + k] = w[k];
+#pragma unroll
+        for (int k = 0; k < 16; k++) Vt[16LL * i + k] = v[k];
+    }
+    if (i < nh) h[i] = glibc_hypot(hx[i], hy[i]);
 }
 
 }  // namespace sslpl
@@ -2153,12 +2310,11 @@ int sslpl_match_lines_batch_device(sslpl_matcher* m, const uint8_t* d_ldesc, con
 // ---------------- LocalMapping's matchers over keyframe pairs in HBM (SURVEY.md 8(f) rows 2/3) ----------------
 // SearchForTriangulation for a list of (KF1, KF2) pairs of one keyframe set: the FeatureVector of every keyframe (KeyFrame::ComputeBoW's,
 // from the descriptors), then k_tri_match over the pair map with per-pair F12 / epipole, the rotation filter and the ordered compaction.
-int sslpl_search_for_triangulation_batch_device(sslpl_matcher* m,
+static int tri_match_stage(sslpl_matcher* m,
         const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nkf, int cap, const uint8_t* d_has_mp,
         const sslpl_vocab* v, int levelsup, int npairs, const int32_t* d_pair, const float* d_geom,
-        const float* scale, const float* sigma2, int nlevels, int checkOrientation, int32_t* d_pairs, int32_t* d_nmatch) {
-    SSLPL_REQUIRE(m && d_kps && d_desc && d_n && d_has_mp && v && d_pair && d_geom && scale && sigma2 && d_pairs && d_nmatch,
-                  SSLPL_ERR_ARG, "null argument");
+        const float* scale, const float* sigma2, int nlevels) {
+    SSLPL_REQUIRE(d_kps && d_desc && d_n && d_has_mp && v && d_pair && d_geom && scale && sigma2, SSLPL_ERR_ARG, "null argument");
     SSLPL_REQUIRE(nkf >= 1 && nkf <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nkf outside [1, max_batch + 1]");
     SSLPL_REQUIRE(npairs >= 1 && npairs <= m->p.max_batch, SSLPL_ERR_ARG, "npairs outside [1, max_batch]");
     SSLPL_REQUIRE(cap >= 1 && cap <= m->p.max_features + 64, SSLPL_ERR_ARG, "cap outside [1, max_features + 64]");
@@ -2181,7 +2337,6 @@ int sslpl_search_for_triangulation_batch_device(sslpl_matcher* m,
     k_build_csr<<<nkf, 128, (nc + 1 + cap) * sizeof(int), st>>>(m->b_node, fc, d_n, cap, nc, m->b_off, NN + 1, m->b_idx, fc);
     m->launches += 2;
     fill(m, m->tw, (long long)npairs * cap, -1);
-    fill(m, d_pairs, 2LL * npairs * cap, -1);
     FrameSet S; memset(&S, 0, sizeof(S));
     S.desc = d_desc; S.desc_fs = (long long)cap * 32;
     S.nodes = m->iota; S.nodes_fs = 0; S.nn = nullptr; S.nn_const = nc;            // dense node ranks: every keyframe lists 0..nc-1
@@ -2195,9 +2350,22 @@ int sslpl_search_for_triangulation_batch_device(sslpl_matcher* m,
     for (int i = 0; i < nlevels; i++) { T.scale[i] = scale[i]; T.sigma2[i] = sigma2[i]; }
     // b_rot is only read where the table holds a match, and k_tri_match writes both together
     k_tri_match<true><<<dim3((nc + 3) / 4, npairs), 128, 0, st>>>(S, T, d_geom, m->tw, cap, m->b_rot, fc);
+    m->launches++;
+    return SSLPL_OK;
+}
+
+int sslpl_search_for_triangulation_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nkf, int cap, const uint8_t* d_has_mp,
+        const sslpl_vocab* v, int levelsup, int npairs, const int32_t* d_pair, const float* d_geom,
+        const float* scale, const float* sigma2, int nlevels, int checkOrientation, int32_t* d_pairs, int32_t* d_nmatch) {
+    SSLPL_REQUIRE(m && d_pairs && d_nmatch, SSLPL_ERR_ARG, "null argument");
+    if (int rc = tri_match_stage(m, d_kps, d_desc, d_n, nkf, cap, d_has_mp, v, levelsup, npairs, d_pair, d_geom, scale, sigma2, nlevels)) return rc;
+    cudaStream_t st = m->stream;
+    const int fc = m->p.max_features + 64;
+    fill(m, d_pairs, 2LL * npairs * cap, -1);
     k_rot_filter<<<npairs, 256, 0, st>>>(m->tw, cap, m->b_rot, fc, nullptr, 0, cap, cap, checkOrientation, d_nmatch, d_pairs, 2LL * cap);
-    k_bad_pairs<<<(npairs + 127) / 128, 128, 0, st>>>(pmap, npairs, nkf, d_nmatch);
-    m->launches += 3;
+    k_bad_pairs<<<(npairs + 127) / 128, 128, 0, st>>>(reinterpret_cast<const int2*>(d_pair), npairs, nkf, d_nmatch);
+    m->launches += 2;
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
@@ -2219,6 +2387,54 @@ int sslpl_line_search_for_triangulation_batch_device(sslpl_matcher* m, const uin
     k_line_tri<<<npairs, 256, 0, st>>>(m->b_knn, (long long)lc * 4, d_nl, capl, pmap, nkf, d_has_ml, d_lpairs, d_nlmatch);
     m->launches += 2;
     SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+// LocalMapping::CreateNewMapPoints' neighbour loop over the chains of a pair list: the unfiltered SearchForTriangulation rows of every pair
+// (tri_match_stage, checkOrientation false), then k_create_points_chain, one CTA per chain.
+int sslpl_create_new_map_points_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nkf, int cap, const uint8_t* d_has_mp,
+        const sslpl_vocab* v, int levelsup, int npairs, const int32_t* d_pair, const float* d_geom, const float* d_kfpose,
+        const float* cam, const float* scaleFactors, const float* levelSigma2, int nlevels, float scaleFactor,
+        int32_t* d_pairs, int32_t* d_nmatch, int32_t* d_status, float* d_x3d, int32_t* d_nnew) {
+    SSLPL_REQUIRE(m && d_kfpose && cam && d_pairs && d_nmatch && d_status && d_x3d && d_nnew, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(scaleFactor > 0.f && scaleFactor < INFINITY, SSLPL_ERR_ARG, "scaleFactor must be positive and finite");
+    CreateArgs C; memset(&C, 0, sizeof(C));
+    C.fx = cam[0]; C.fy = cam[1]; C.cx = cam[2]; C.cy = cam[3]; C.invfx = cam[4]; C.invfy = cam[5];
+    C.ratioFactor = 1.5f * scaleFactor;
+    if (int rc = tri_match_stage(m, d_kps, d_desc, d_n, nkf, cap, d_has_mp, v, levelsup, npairs, d_pair, d_geom, scaleFactors, levelSigma2, nlevels)) return rc;
+    C.nlevels = nlevels;
+    for (int i = 0; i < nlevels; i++) { C.scale[i] = scaleFactors[i]; C.sigma2[i] = levelSigma2[i]; }
+    const size_t smem = sizeof(unsigned) * (size_t)((cap + 31) / 32);
+    k_create_points_chain<<<npairs, 256, smem, m->stream>>>(reinterpret_cast<const int2*>(d_pair), npairs, nkf, m->tw, cap,
+                                                            reinterpret_cast<const float*>(d_kps), d_n, d_has_mp, d_kfpose, C,
+                                                            d_pairs, d_nmatch, d_status, d_x3d, d_nnew);
+    m->launches++;
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+int sslpl_matcher_debug_svd4(sslpl_matcher* m, int n, const float* A, float* W, float* Vt, int nh, const double* hx, const double* hy, double* h) {
+    SSLPL_REQUIRE(m && n >= 0 && nh >= 0 && (n == 0 || (A && W && Vt)) && (nh == 0 || (hx && hy && h)), SSLPL_ERR_ARG, "null argument");
+    const int nt = std::max(n, nh);
+    if (nt == 0) return SSLPL_OK;
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    cudaStream_t st = m->stream;
+    if (int rc = ensure_scratch(m, (size_t)n * 36 * sizeof(float) + (size_t)nh * 3 * sizeof(double) + 4096)) return rc;
+    Arena Ar; Ar.base = m->scratch; Ar.used = 0;
+    cudaError_t e = cudaSuccess;
+    const float* d_A = stage(Ar, A, (size_t)16 * n, st, e); float* d_W = Ar.take<float>((size_t)4 * n + 8); float* d_V = Ar.take<float>((size_t)16 * n + 8);
+    const double* d_hx = stage(Ar, hx, nh, st, e); const double* d_hy = stage(Ar, hy, nh, st, e); double* d_h = Ar.take<double>((size_t)nh + 8);
+    SSLPL_CUDA(e);
+    k_debug_svd4<<<(nt + 127) / 128, 128, 0, st>>>(n, d_A, d_W, d_V, nh, d_hx, d_hy, d_h);
+    m->launches++;
+    SSLPL_CUDA(cudaGetLastError());
+    if (n) {
+        SSLPL_CUDA(cudaMemcpyAsync(W, d_W, sizeof(float) * 4 * (size_t)n, cudaMemcpyDeviceToHost, st));
+        SSLPL_CUDA(cudaMemcpyAsync(Vt, d_V, sizeof(float) * 16 * (size_t)n, cudaMemcpyDeviceToHost, st));
+    }
+    if (nh) SSLPL_CUDA(cudaMemcpyAsync(h, d_h, sizeof(double) * (size_t)nh, cudaMemcpyDeviceToHost, st));
+    SSLPL_CUDA(cudaStreamSynchronize(st));
     return SSLPL_OK;
 }
 
