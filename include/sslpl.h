@@ -390,6 +390,55 @@ int  sslpl_create_new_map_points_batch_device(sslpl_matcher* m,
 int  sslpl_matcher_debug_svd4(sslpl_matcher* m, int n, const float* A, float* W, float* Vt,
                               int nh, const double* hx, const double* hy, double* h);
 
+/* ---- LocalMapping::CreateNewMapLines2 (LocalMapping.cc:911-1173, monocular) over keyframe pairs in HBM: the line matcher and the
+   triangulation of both end points of every match, neighbour after neighbour.  The keyframe set is the layout of sslpl_line_device_results:
+   d_kl[k][capl] = KeyFrame::mvKeyLines (F.mvKeylinesUn), d_ldesc[k][capl][32], d_lineeq[k][capl][3] = mvKeyLineFunctions (double),
+   d_nl[k] (clamped to capl); d_has_ml[k][capl] = GetMapLine(i) != NULL.  d_kfpose[k][15] = Tcw (3x4 row-major) then Ow, f32 (the pose
+   table of the points call); d_kfdepth[k] = KeyFrame::ComputeSceneMedianDepth(2) (KeyFrame.cc:711-741) as the caller computes it, f32;
+   the HOST cam[6] = fx fy cx cy invfx invfy, one camera for all keyframes.
+   The pair list is the caller's: it keeps the baseline gate (:955-979, ratioBaselineDepth < 0.1 drops the neighbour) and takes the
+   nn = 10 best covisible keyframes.  Both differ from the points call (gate 0.01, nn = 20), so lines need their own pair list.
+   Chains work as in sslpl_create_new_map_points_batch_device: a maximal run of consecutive pairs with the same kf1 is one neighbour loop,
+   run in order; the KF1 mask starts as d_has_ml[kf1] and gains the qdx of every created row (AddMapLine(pML, idx1), :1159), which the
+   matcher of the later pairs skips (LSDmatcher.cpp:403).  The KF2 masks are used as given (the kf2s of a chain are distinct).  Chains are
+   independent, the inputs are never modified, and the first k pairs of a chain give what a call with only those pairs gives.  A pair
+   with an index outside [0, nkf), with kf2 == kf1, with a kf2 repeated in its chain, or whose KF1 has lines and KF2 fewer than 2 gets
+   the count -1, no rows, and leaves the chain's state alone; a KF1 without lines gives 0.
+   Results per pair p, `capl` rows each:
+     d_lpairs[p][capl][2]  (qdx, tdx) in ascending qdx: what LSDmatcher::SearchForTriangulation returns under the mask of that
+                           neighbour; (-1, -1) after the count;
+     d_nlmatch[p]          the row count (-1: bad pair);
+     d_status[p][capl]     per row SSLPL_CNML_CREATED (0) or the test that rejected it, SSLPL_CNML_*; -1 after the count;
+     d_line3d[p][capl][6]  s3D then e3D (f32), written for the rows with status 0 or >= 4; other rows are not written;
+     d_nnew[p]             the rows with status 0.
+   The rows with status 0, in (pair, row) order, are the reference's MapLine creation order.  Two created rows of one pair may share a
+   tdx: KF2's slot then ends with the later one, so a caller applies them in order.  Numerics are those of the reference with cv2 4.13
+   and glibc >= 2.35 (DESIGN.md).  Concurrency: in the reference CreateNewMapPoints runs in another thread at the same time and adds
+   MapPoints to the same KF2s, so the depth ComputeSceneMedianDepth(2) gives at :973 and at :1098 is not deterministic there; this call
+   takes one depth per keyframe as given.  Asynchronous on the matcher's stream, no caller-visible allocation (the first call allocates a
+   [max_batch][max_lines + 64] int32 table, freed with the handle).  Needs nkf in [1, max_batch + 1], npairs in [1, max_batch] and capl
+   in [1, max_lines + 64]; bad arguments return SSLPL_ERR_ARG and enqueue nothing. ---- */
+enum {
+    SSLPL_CNML_CREATED = 0,    /* the MapLine is created (:1150-1169) */
+    SSLPL_CNML_PARALLAX = 1,   /* !(cos < cos + 1 && cos > 0 && cos < 0.98) (:1041-1053, :1090) */
+    SSLPL_CNML_W_ZERO_S = 2,   /* vt1.row(3)(3) == 0, start point (:1066) */
+    SSLPL_CNML_W_ZERO_E = 3,   /* vt2.row(3)(3) == 0, end point (:1084) */
+    SSLPL_CNML_NEAR_S1 = 4,    /* |s3D - Ow1| / depth2 < 0.3 (:1099-1103) */
+    SSLPL_CNML_NEAR_S2 = 5,    /* |s3D - Ow2| / depth2 < 0.3 (:1105-1109) */
+    SSLPL_CNML_LONG = 6,       /* |e3D - s3D| / depth2 > 0.61 (:1112-1116) */
+    SSLPL_CNML_NEAR_E1 = 7,    /* |e3D - Ow1| / depth2 < 0.3 (:1122-1126) */
+    SSLPL_CNML_NEAR_E2 = 8,    /* |e3D - Ow2| / depth2 < 0.3 (:1127-1131) */
+    SSLPL_CNML_ZS1 = 9,        /* start point depth in KF1 <= 0 (:1134-1136) */
+    SSLPL_CNML_ZS2 = 10,       /* start point depth in KF2 <= 0 (:1138-1140) */
+    SSLPL_CNML_ZE1 = 11,       /* end point depth in KF1 <= 0 (:1142-1144) */
+    SSLPL_CNML_ZE2 = 12        /* end point depth in KF2 <= 0 (:1146-1148) */
+};
+int  sslpl_create_new_map_lines_batch_device(sslpl_matcher* m,
+        const sslpl_keyline* d_kl, const uint8_t* d_ldesc, const double* d_lineeq, const int* d_nl, int nkf, int capl,
+        const uint8_t* d_has_ml, int npairs, const int32_t* d_pair,
+        const float* d_kfpose, const float* d_kfdepth, const float* cam,
+        int32_t* d_lpairs, int32_t* d_nlmatch, int32_t* d_status, float* d_line3d, int32_t* d_nnew);
+
 /* ---- MapPoint::PredictScale / MapLine::PredictScale (MapPoint.cc:390-405, MapLine.cpp:386-395) on the device, exact against the host's
    logf: level = (int)ceil(logf(ratio) / logScaleFactor), ratio = mfMaxDistance / dist.  The level is a monotone step function of the float
    ratio; thr[k] (k = 0 .. nlevels, nlevels + 1 floats) is the smallest positive float whose level is >= k, found by bisection over the

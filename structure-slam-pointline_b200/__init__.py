@@ -499,6 +499,22 @@ class Matcher:
             int(levelsup), int(npairs), C.c_void_p(d_pair), C.c_void_p(d_geom), C.c_void_p(d_kfpose), _p(cm), _p(sc), _p(s2), len(sc),
             C.c_float(scale_factor), C.c_void_p(d_pairs), C.c_void_p(d_nmatch), C.c_void_p(d_status), C.c_void_p(d_x3d), C.c_void_p(d_nnew)))
 
+    def create_new_map_lines_batch_device(self, d_kl, d_ldesc, d_lineeq, d_nl, nkf, capl, d_has_ml, npairs, d_pair, d_kfpose, d_kfdepth,
+                                          cam, d_lpairs, d_nlmatch, d_status, d_line3d, d_nnew):
+        """LocalMapping::CreateNewMapLines2 (LocalMapping.cc:911-1173, monocular) for the chains of a pair list in HBM: per pair the
+        LSDmatcher::SearchForTriangulation rows under the mask the reference sees at that neighbour, a status per row and both
+        triangulated end points (see sslpl_create_new_map_lines_batch_device).  d_kl [nkf, capl] sslpl_keyline, d_ldesc [nkf, capl, 32],
+        d_lineeq [nkf, capl, 3] f64, d_nl [nkf] as sslpl_line_device_results gives them, d_has_ml [nkf, capl] u8, d_pair [npairs, 2]
+        (the caller's pair list: baseline gate 0.1, nn = 10), d_kfpose [nkf, 15] f32 (Tcw 3x4, Ow), d_kfdepth [nkf] f32
+        (ComputeSceneMedianDepth(2)) and host cam = fx fy cx cy invfx invfy -> d_lpairs [npairs, capl, 2], d_nlmatch [npairs],
+        d_status [npairs, capl] i32, d_line3d [npairs, capl, 6] f32 (s3D, e3D), d_nnew [npairs].  Asynchronous."""
+        cm = np.ascontiguousarray(cam, np.float32)
+        assert len(cm) == 6
+        _check(lib().sslpl_create_new_map_lines_batch_device(
+            self._h, C.c_void_p(d_kl), C.c_void_p(d_ldesc), C.c_void_p(d_lineeq), C.c_void_p(d_nl), int(nkf), int(capl), C.c_void_p(d_has_ml),
+            int(npairs), C.c_void_p(d_pair), C.c_void_p(d_kfpose), C.c_void_p(d_kfdepth), _p(cm), C.c_void_p(d_lpairs), C.c_void_p(d_nlmatch),
+            C.c_void_p(d_status), C.c_void_p(d_line3d), C.c_void_p(d_nnew)))
+
     def debug_svd4(self, A, hx=None, hy=None):
         """The device's 4x4 SVD (cv::SVD::compute on CV_32F) of host matrices A [n, 4, 4] -> (W [n, 4], Vt [n, 4, 4]), and its glibc
         hypot of hx, hy (float64) -> h.  Synchronous."""

@@ -1109,6 +1109,38 @@ __global__ void k_bad_pairs(const int2* pmap, int npairs, int nframes, int32_t* 
 //   compaction: lpairs[p][k] = (qdx, tdx) in ascending qdx, (-1, -1) past the count.
 // nlmatch[p] = -1 when an index is outside [0, nframes) or when KF1 has lines and KF2 fewer than 2 (the reference would read
 // lmatches[i][1] out of bounds, :402); 0 when KF1 has none.
+// nn12_mad * 0.1 (:406) of the n1 >= 1 rows of knn table K, computed by the whole CTA (every thread gets it); s_hist[257] and s_sel are
+// the caller's shared memory
+__device__ __forceinline__ double line_mad_thr(const int4* K, int n1, int tid, int* s_hist, int* s_sel) {
+    const int k = n1 / 2;
+    for (int i = tid; i < 257; i += 256) s_hist[i] = 0;
+    __syncthreads();
+    for (int i = tid; i < n1; i += 256) { const int4 r = K[i]; atomicAdd(&s_hist[r.w - r.y], 1); }
+    __syncthreads();
+    if (tid == 0) {                                            // descending order: count down from 256
+        int c = 0, v = 256;
+        for (; v > 0; v--) { c += s_hist[v]; if (c > k) break; }
+        *s_sel = v;
+    }
+    __syncthreads();
+    const int med12 = *s_sel;
+    for (int i = tid; i < 257; i += 256) s_hist[i] = 0;
+    __syncthreads();
+    for (int i = tid; i < n1; i += 256) { const int4 r = K[i]; atomicAdd(&s_hist[abs(r.w - r.y - med12)], 1); }
+    __syncthreads();
+    if (tid == 0) {                                            // ascending order
+        int c = 0, v = 0;
+        for (; v < 256; v++) { c += s_hist[v]; if (c > k) break; }
+        *s_sel = v;
+    }
+    __syncthreads();
+    return __dmul_rn(__dmul_rn(1.4826, (double)*s_sel), 0.1);
+}
+// the KF2 and distance tests of :403-408 for knn row r (the KF1 test is the caller's)
+__device__ __forceinline__ bool line_row_ok(int4 r, const uint8_t* h2, double thr) {
+    return !h2[r.x] && (double)(r.w - r.y) > thr;
+}
+
 __global__ void __launch_bounds__(256) k_line_tri(const int32_t* knn, long long knn_fs, const int* nl, int capl, const int2* pmap, int nframes,
                                                    const uint8_t* has_ml, int32_t* lpairs, int32_t* nlmatch) {
     __shared__ int s_hist[257];
@@ -1124,29 +1156,7 @@ __global__ void __launch_bounds__(256) k_line_tri(const int32_t* knn, long long 
     const int4* K = reinterpret_cast<const int4*>(knn + p * knn_fs);
     int32_t* O = lpairs + 2LL * capl * p;
     if (ok && n1 > 0) {                                        // CTA-uniform
-        const int k = n1 / 2;
-        for (int i = tid; i < 257; i += 256) s_hist[i] = 0;
-        __syncthreads();
-        for (int i = tid; i < n1; i += 256) { const int4 r = K[i]; atomicAdd(&s_hist[r.w - r.y], 1); }
-        __syncthreads();
-        if (tid == 0) {                                        // descending order: count down from 256
-            int c = 0, v = 256;
-            for (; v > 0; v--) { c += s_hist[v]; if (c > k) break; }
-            s_sel = v;
-        }
-        __syncthreads();
-        const int med12 = s_sel;
-        for (int i = tid; i < 257; i += 256) s_hist[i] = 0;
-        __syncthreads();
-        for (int i = tid; i < n1; i += 256) { const int4 r = K[i]; atomicAdd(&s_hist[abs(r.w - r.y - med12)], 1); }
-        __syncthreads();
-        if (tid == 0) {                                        // ascending order
-            int c = 0, v = 0;
-            for (; v < 256; v++) { c += s_hist[v]; if (c > k) break; }
-            s_sel = v;
-        }
-        __syncthreads();
-        const double thr = __dmul_rn(__dmul_rn(1.4826, (double)s_sel), 0.1);      // nn12_mad * 0.1 (:406)
+        const double thr = line_mad_thr(K, n1, tid, s_hist, &s_sel);
         const uint8_t* h1 = has_ml + (long long)f1 * capl; const uint8_t* h2 = has_ml + (long long)f2 * capl;
         const int chunk = (n1 + 255) / 256, pb = min(n1, tid * chunk), pe = min(n1, pb + chunk);
         int c = 0;
@@ -1159,6 +1169,24 @@ __global__ void __launch_bounds__(256) k_line_tri(const int32_t* knn, long long 
     }
     for (int i = total + tid; i < capl; i += 256) { O[2 * i] = -1; O[2 * i + 1] = -1; }
     if (tid == 0) nlmatch[p] = ok ? total : -1;
+}
+
+// The table k_create_lines_chain starts from: for pair p, tw[p][qdx] = tdx when row qdx of LSDmatcher::SearchForTriangulation passes the
+// KF2 and distance tests (the KF1 mask left out), else -1, for qdx < n1.  Pairs that k_line_tri gives no rows or -1 are left unwritten.
+__global__ void __launch_bounds__(256) k_line_tri_table(const int32_t* knn, long long knn_fs, const int* nl, int capl, const int2* pmap,
+                                                         int nframes, const uint8_t* has_ml, int32_t* tw) {
+    __shared__ int s_hist[257];
+    __shared__ int s_sel;
+    const int p = blockIdx.x, tid = threadIdx.x;
+    int f1, f2;
+    if (!pair_frames(pmap, nframes, p, f1, f2)) return;
+    const int n1 = max(0, min(nl[f1], capl));
+    if (n1 == 0 || min(nl[f2], capl) < 2) return;              // CTA-uniform
+    const int4* K = reinterpret_cast<const int4*>(knn + p * knn_fs);
+    const double thr = line_mad_thr(K, n1, tid, s_hist, &s_sel);
+    const uint8_t* h2 = has_ml + (long long)f2 * capl;
+    int32_t* T = tw + (long long)capl * p;
+    for (int i = tid; i < n1; i += 256) { const int4 r = K[i]; T[i] = line_row_ok(r, h2, thr) ? r.x : -1; }
 }
 
 // ---------------- LocalMapping::CreateNewMapPoints' neighbour loop (LocalMapping.cc:371-637, monocular) ----------------
@@ -1299,6 +1327,161 @@ __global__ void __launch_bounds__(256, 1) k_create_points_chain(const int2* pmap
     }
 }
 
+// ---------------- LocalMapping::CreateNewMapLines2's neighbour loop (LocalMapping.cc:911-1173, monocular) ----------------
+// Status codes of include/sslpl.h (SSLPL_CNML_*), one per `continue` of the per-match body in reference order.
+enum { CNML_CREATED = 0, CNML_PARALLAX, CNML_W_ZERO_S, CNML_W_ZERO_E, CNML_NEAR_S1, CNML_NEAR_S2, CNML_LONG, CNML_NEAR_E1, CNML_NEAR_E2,
+       CNML_ZS1, CNML_ZS2, CNML_ZE1, CNML_ZE2 };
+
+struct LineCam { float fx, fy, cx, cy, invfx, invfy; };   // KeyFrame::fx .. invfy (one camera for both keyframes)
+
+// (a + b) / 2 of CV_32F: MatExpr's addWeighted(a, 0.5, b, 0.5, 0), in double, rounded once
+__device__ __forceinline__ float mid_aw(float a, float b) {
+    return __double2float_rn(__dadd_rn(__dadd_rn(__dmul_rn((double)a, 0.5), __dmul_rn((double)b, 0.5)), 0.0));
+}
+// M = K * Tcw (:1047-1048), 3x3 by 3x4: cv::gemm's float path (inner length 3 = output height), K's zeros in the sum order
+__device__ __forceinline__ void proj_mat(const LineCam& C, const float* T, float* M) {
+    const float K[9] = {C.fx, 0.f, C.cx, 0.f, C.fy, C.cy, 0.f, 0.f, 1.f};
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+#pragma unroll
+        for (int j = 0; j < 4; j++)
+            M[4 * i + j] = __fadd_rn(__fadd_rn(__fmul_rn(K[3 * i], T[j]), __fmul_rn(K[3 * i + 1], T[4 + j])), __fmul_rn(K[3 * i + 2], T[8 + j]));
+}
+// row j of klF.t() * M (:1057-1058): cv::gemm 1x3 by 3x4, accumulated in double from 0 and rounded once
+__device__ __forceinline__ float plane_row(const float* l, const float* M, int j) {
+    return __double2float_rn(__dadd_rn(__dadd_rn(__dadd_rn(0.0, __dmul_rn((double)l[0], (double)M[j])), __dmul_rn((double)l[1], (double)M[4 + j])),
+                                       __dmul_rn((double)l[2], (double)M[8 + j])));
+}
+// One end point (:1056-1070 / :1073-1088): A = [P1; P2; x T1.row(2) - T1.row(0); y T1.row(2) - T1.row(1)], its SVD and the
+// dehomogenised null vector X; false when vt(3, 3) == 0
+__device__ __forceinline__ bool tri_end(const float* P1, const float* P2, const float* T1, float x, float y, float* X) {
+    float A[16], W[4], Vt[16];
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        A[k] = P1[k]; A[4 + k] = P2[k];
+        A[8 + k] = add_weighted_m1(T1[8 + k], x, T1[k]);
+        A[12 + k] = add_weighted_m1(T1[8 + k], y, T1[4 + k]);
+    }
+    svd4_jacobi(A, W, Vt);
+    if (Vt[15] == 0.f) return false;
+    const float inv = __double2float_rn(__ddiv_rn(1.0, (double)Vt[15]));                                         // rowRange(0, 3) / w
+#pragma unroll
+    for (int k = 0; k < 3; k++) X[k] = __fadd_rn(__fmul_rn(Vt[12 + k], inv), 0.f);
+    return true;
+}
+// (float)cv::norm(a - b) / depth (:1099-1131)
+__device__ __forceinline__ float dist_ratio(const float* a, const float* b, float depth) {
+    return __fdiv_rn(norm3d(__fsub_rn(a[0], b[0]), __fsub_rn(a[1], b[1]), __fsub_rn(a[2], b[2])), depth);
+}
+
+// The per-match body of CreateNewMapLines2 (:1007-1169) for KF1 segment (s1, e1) with line function l1 and KF2 segment (s2, e2) with l2,
+// poses T1 / T2 (pose[15] = Tcw 3x4 row-major, Ow), projection matrices M1 / M2 and KF2's median depth -> status; X = s3D, e3D is set
+// when both SVDs gave a w != 0 (*written = true).
+__device__ __forceinline__ int create_line(const LineCam& C, const float* T1, const float* T2, const float* M1, const float* M2, float depth2,
+                                           const float* s1, const float* e1, const double* l1, const float* s2, const float* e2,
+                                           const double* l2, float* X, bool* written) {
+    *written = false;
+    const float S1[2] = {__fmul_rn(__fsub_rn(s1[0], C.cx), C.invfx), __fmul_rn(__fsub_rn(s1[1], C.cy), C.invfy)};   // :1025-1036
+    const float E1[2] = {__fmul_rn(__fsub_rn(e1[0], C.cx), C.invfx), __fmul_rn(__fsub_rn(e1[1], C.cy), C.invfy)};
+    const float S2[2] = {__fmul_rn(__fsub_rn(s2[0], C.cx), C.invfx), __fmul_rn(__fsub_rn(s2[1], C.cy), C.invfy)};
+    const float E2[2] = {__fmul_rn(__fsub_rn(e2[0], C.cx), C.invfx), __fmul_rn(__fsub_rn(e2[1], C.cy), C.invfy)};
+    const float m1[3] = {mid_aw(S1[0], E1[0]), mid_aw(S1[1], E1[1]), mid_aw(1.f, 1.f)};
+    const float m2[3] = {mid_aw(S2[0], E2[0]), mid_aw(S2[1], E2[1]), mid_aw(1.f, 1.f)};
+    float r1[3], r2[3];
+    ray(T1, m1, r1); ray(T2, m2, r2);                                                                           // :1038-1039
+    const float cosp = __double2float_rn(__ddiv_rn(dot3d(r1[0], r1[1], r1[2], r2[0], r2[1], r2[2]),
+                                                   __dmul_rn(norm3d_d(r1[0], r1[1], r1[2]), norm3d_d(r2[0], r2[1], r2[2]))));   // :1041
+    if (!(cosp < __fadd_rn(cosp, 1.f) && cosp > 0.f && (double)cosp < 0.98)) return CNML_PARALLAX;             // :1043, :1053, :1090
+    const float f1[3] = {__double2float_rn(l1[0]), __double2float_rn(l1[1]), __double2float_rn(l1[2])};          // klF1, klF2 (:1016-1021)
+    const float f2[3] = {__double2float_rn(l2[0]), __double2float_rn(l2[1]), __double2float_rn(l2[2])};
+    float P1[4], P2[4];
+#pragma unroll
+    for (int j = 0; j < 4; j++) { P1[j] = plane_row(f1, M1, j); P2[j] = plane_row(f2, M2, j); }
+    if (!tri_end(P1, P2, T1, S1[0], S1[1], X)) return CNML_W_ZERO_S;
+    if (!tri_end(P1, P2, T1, E1[0], E1[1], X + 3)) return CNML_W_ZERO_E;
+    *written = true;
+    const float* s3 = X; const float* e3 = X + 3;
+    if ((double)dist_ratio(s3, T1 + 12, depth2) < 0.3) return CNML_NEAR_S1;                                     // :1098-1109
+    if ((double)dist_ratio(s3, T2 + 12, depth2) < 0.3) return CNML_NEAR_S2;
+    if ((double)dist_ratio(e3, s3, depth2) > 0.61) return CNML_LONG;                                            // :1112-1116
+    if ((double)dist_ratio(e3, T1 + 12, depth2) < 0.3) return CNML_NEAR_E1;                                     // :1122-1131
+    if ((double)dist_ratio(e3, T2 + 12, depth2) < 0.3) return CNML_NEAR_E2;
+    if (cam_row(T1 + 8, s3) <= 0.f) return CNML_ZS1;                                                            // :1134-1148
+    if (cam_row(T2 + 8, s3) <= 0.f) return CNML_ZS2;
+    if (cam_row(T1 + 8, e3) <= 0.f) return CNML_ZE1;
+    if (cam_row(T2 + 8, e3) <= 0.f) return CNML_ZE2;
+    return CNML_CREATED;
+}
+
+// One CTA per chain, as k_create_points_chain: the KF1 lines that have a MapLine are a bitmap in shared memory, loaded from has_ml; for
+// each pair in order the CTA drops the k_line_tri_table rows whose qdx is set, compacts the rest in ascending qdx (block scan),
+// triangulates both end points of one row per thread and sets the bits of the created rows (AddMapLine(pML, idx1), :1159) before the
+// next pair.  A pair with an index outside [0, nkf), kf2 == kf1, a kf2 repeated in its chain, or KF1 with lines and KF2 with fewer than
+// 2 gets count -1 and leaves the bitmap alone; KF1 without lines gives 0.  kl = sslpl_keyline rows (17 floats), lineeq 3 doubles per row.
+__global__ void __launch_bounds__(256, 1) k_create_lines_chain(const int2* pmap, int npairs, int nkf, const int32_t* tw, int capl,
+        const float* kl, const double* lineeq, const int* nl, const uint8_t* has_ml, const float* pose, const float* depth,
+        const __grid_constant__ LineCam C, int32_t* rows, int32_t* nmatch, int32_t* status, float* line3d, int32_t* nnew) {
+    extern __shared__ unsigned s_bits[];
+    __shared__ int s_warp[33];
+    __shared__ float s_T[2][15], s_M[2][12];
+    const int c0 = blockIdx.x, tid = threadIdx.x;
+    const int kf1 = pmap[c0].x;
+    if (c0 > 0 && pmap[c0 - 1].x == kf1) return;
+    int c1 = c0 + 1;
+    while (c1 < npairs && pmap[c1].x == kf1) c1++;
+    const bool ok1 = (unsigned)kf1 < (unsigned)nkf;
+    const int n1 = ok1 ? max(0, min(nl[kf1], capl)) : 0, words = (capl + 31) / 32;
+    for (int w = tid; w < words; w += 256) {
+        unsigned b = 0;
+        for (int k = 0; k < 32 && ok1 && 32 * w + k < capl; k++) b |= (has_ml[(long long)kf1 * capl + 32 * w + k] != 0) << k;
+        s_bits[w] = b;
+    }
+    __syncthreads();
+    const long long o1 = (long long)capl * (ok1 ? kf1 : 0);
+    for (int p = c0; p < c1; p++) {
+        const int kf2 = pmap[p].y;
+        bool bad = !ok1 || (unsigned)kf2 >= (unsigned)nkf || kf2 == kf1;
+        for (int q = c0; q < p && !bad; q++) bad = pmap[q].y == kf2;
+        if (!bad) bad = n1 > 0 && min(nl[kf2], capl) < 2;
+        int32_t* R = rows + 2LL * capl * p; int32_t* S = status + (long long)capl * p; float* L3 = line3d + 6LL * capl * p;
+        int total = 0, created = 0;
+        if (!bad && n1 > 0) {                                                    // CTA-uniform
+            const int32_t* Tw = tw + (long long)capl * p;
+            const int chunk = (n1 + 255) / 256, pb = min(n1, tid * chunk), pe = min(n1, pb + chunk);
+            int c = 0;
+            for (int i = pb; i < pe; i++) c += Tw[i] >= 0 && !((s_bits[i >> 5] >> (i & 31)) & 1u);
+            int o = block_exclusive_scan(c, s_warp, &total);
+            for (int i = pb; i < pe; i++)
+                if (Tw[i] >= 0 && !((s_bits[i >> 5] >> (i & 31)) & 1u)) { R[2 * o] = i; R[2 * o + 1] = Tw[i]; o++; }
+            if (tid < 30) s_T[tid / 15][tid % 15] = pose[15LL * (tid < 15 ? kf1 : kf2) + tid % 15];
+            __syncthreads();                                                     // the rows (global), the poses and every bitmap read are done
+            if (tid < 2) proj_mat(C, s_T[tid], s_M[tid]);
+            __syncthreads();
+            const long long o2 = (long long)capl * kf2;
+            const float d2 = depth[kf2];
+            for (int r = tid; r < total; r += 256) {
+                const int i1 = R[2 * r], i2 = R[2 * r + 1];
+                const float* k1 = kl + 17 * (o1 + i1); const float* k2 = kl + 17 * (o2 + i2);
+                float X[6]; bool written;
+                const int st = create_line(C, s_T[0], s_T[1], s_M[0], s_M[1], d2, k1 + 7, k1 + 9, lineeq + 3 * (o1 + i1), k2 + 7, k2 + 9,
+                                           lineeq + 3 * (o2 + i2), X, &written);
+                S[r] = st;
+                if (written) {
+#pragma unroll
+                    for (int k = 0; k < 6; k++) L3[6 * r + k] = X[k];
+                }
+                if (st == CNML_CREATED) { atomicOr(&s_bits[i1 >> 5], 1u << (i1 & 31)); created++; }
+            }
+            int all;
+            block_exclusive_scan(created, s_warp, &all);
+            created = all;
+        }
+        for (int i = total + tid; i < capl; i += 256) { R[2 * i] = -1; R[2 * i + 1] = -1; S[i] = -1; }
+        if (tid == 0) { nmatch[p] = bad ? -1 : total; nnew[p] = created; }
+        __syncthreads();
+    }
+}
+
 // sslpl_matcher_debug_svd4: svd4_jacobi on n row-major 4x4 matrices (W, Vt), glibc_hypot on nh pairs
 __global__ void k_debug_svd4(int n, const float* A, float* W, float* Vt, int nh, const double* hx, const double* hy, double* h) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1346,6 +1529,8 @@ struct sslpl_matcher {
     int32_t* pw_cell = nullptr; int* pw_off = nullptr; int* pw_idx = nullptr; int32_t* pw_sel = nullptr; uint8_t* pw_claimed = nullptr; uint8_t* pw_rbin = nullptr;
     // per-pair match table of sslpl_search_for_triangulation_batch_device ([max_batch][max_features + 64]), allocated by its first call
     int32_t* tw = nullptr;
+    // per-pair row table of sslpl_create_new_map_lines_batch_device ([max_batch][max_lines + 64]), allocated by its first call
+    int32_t* ltw = nullptr;
     int32_t* h_small = nullptr;      // pinned scratch
     long long launches = 0;
 };
@@ -1539,6 +1724,7 @@ void sslpl_matcher_destroy(sslpl_matcher* m) {
     if (m->scratch) cudaFree(m->scratch);
     if (m->pw) cudaFree(m->pw);
     if (m->tw) cudaFree(m->tw);
+    if (m->ltw) cudaFree(m->ltw);
     if (m->h_small) cudaFreeHost(m->h_small);
     delete m;
 }
@@ -2410,6 +2596,39 @@ int sslpl_create_new_map_points_batch_device(sslpl_matcher* m,
                                                             reinterpret_cast<const float*>(d_kps), d_n, d_has_mp, d_kfpose, C,
                                                             d_pairs, d_nmatch, d_status, d_x3d, d_nnew);
     m->launches++;
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+// LocalMapping::CreateNewMapLines2's neighbour loop over the chains of a pair list: k_knn2 over the pair map, the KF1-unmasked rows of
+// every pair (k_line_tri_table), then k_create_lines_chain, one CTA per chain.
+int sslpl_create_new_map_lines_batch_device(sslpl_matcher* m,
+        const sslpl_keyline* d_kl, const uint8_t* d_ldesc, const double* d_lineeq, const int* d_nl, int nkf, int capl,
+        const uint8_t* d_has_ml, int npairs, const int32_t* d_pair, const float* d_kfpose, const float* d_kfdepth, const float* cam,
+        int32_t* d_lpairs, int32_t* d_nlmatch, int32_t* d_status, float* d_line3d, int32_t* d_nnew) {
+    SSLPL_REQUIRE(m && d_kl && d_ldesc && d_lineeq && d_nl && d_has_ml && d_pair && d_kfpose && d_kfdepth && cam && d_lpairs && d_nlmatch &&
+                  d_status && d_line3d && d_nnew, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nkf >= 1 && nkf <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nkf outside [1, max_batch + 1]");
+    SSLPL_REQUIRE(npairs >= 1 && npairs <= m->p.max_batch, SSLPL_ERR_ARG, "npairs outside [1, max_batch]");
+    SSLPL_REQUIRE(capl >= 1 && capl <= m->p.max_lines + 64, SSLPL_ERR_ARG, "capl outside [1, max_lines + 64]");
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    const int lc = m->p.max_lines + 64;
+    if (!m->ltw) {                                                       // first call: a handle that never gets here never pays for it
+        const size_t bytes = sizeof(int32_t) * (size_t)m->p.max_batch * lc;
+        cudaError_t e = cudaMalloc(&m->ltw, bytes);
+        if (e != cudaSuccess) { m->ltw = nullptr; set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return SSLPL_ERR_CUDA; }
+    }
+    LineCam C;
+    C.fx = cam[0]; C.fy = cam[1]; C.cx = cam[2]; C.cy = cam[3]; C.invfx = cam[4]; C.invfy = cam[5];
+    cudaStream_t st = m->stream;
+    const int2* pmap = reinterpret_cast<const int2*>(d_pair);
+    k_knn2<true><<<dim3((capl + 7) / 8, npairs), 256, 0, st>>>(d_ldesc, (long long)capl * 32, d_nl, 0, d_ldesc, (long long)capl * 32, d_nl, 0,
+                                                          m->b_knn, (long long)lc * 4, capl, pmap, nkf);
+    k_line_tri_table<<<npairs, 256, 0, st>>>(m->b_knn, (long long)lc * 4, d_nl, capl, pmap, nkf, d_has_ml, m->ltw);
+    const size_t smem = sizeof(unsigned) * (size_t)((capl + 31) / 32);
+    k_create_lines_chain<<<npairs, 256, smem, st>>>(pmap, npairs, nkf, m->ltw, capl, reinterpret_cast<const float*>(d_kl), d_lineeq, d_nl,
+                                                    d_has_ml, d_kfpose, d_kfdepth, C, d_lpairs, d_nlmatch, d_status, d_line3d, d_nnew);
+    m->launches += 3;
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
