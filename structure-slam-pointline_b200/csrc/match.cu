@@ -53,6 +53,32 @@ __device__ __forceinline__ void load_desc(const uint8_t* p, uint4& a, uint4& b) 
 __device__ __forceinline__ void top2_insert(unsigned& k0, unsigned& k1, unsigned k) {
     if (k < k0) { k1 = k0; k0 = k; } else if (k < k1) k1 = k;
 }
+// the two smallest keys of the warp, in every lane
+__device__ __forceinline__ void top2_warp32(unsigned& k0, unsigned& k1) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned o0 = __shfl_xor_sync(0xffffffffu, k0, o), o1 = __shfl_xor_sync(0xffffffffu, k1, o);
+        top2_insert(k0, k1, o0);
+        top2_insert(k0, k1, o1);
+    }
+}
+__device__ __forceinline__ void top2_push(unsigned long long& a1, unsigned long long& a2, unsigned long long k) {
+    if (k < a1) { a2 = a1; a1 = k; } else if (k < a2) a2 = k;
+}
+__device__ __forceinline__ void top2_warp(unsigned long long& a1, unsigned long long& a2) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long b1 = __shfl_xor_sync(0xffffffffu, a1, o), b2 = __shfl_xor_sync(0xffffffffu, a2, o);
+        const unsigned long long lo = a1 < b1 ? a1 : b1, hi = a1 < b1 ? b1 : a1, m2 = a2 < b2 ? a2 : b2;
+        a1 = lo; a2 = hi < m2 ? hi : m2;
+    }
+}
+// the smallest key of the warp, in every lane
+__device__ __forceinline__ unsigned long long warp_min(unsigned long long b) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { const unsigned long long t = __shfl_xor_sync(0xffffffffu, b, o); b = t < b ? t : b; }
+    return b;
+}
 
 template <bool kMap>
 __global__ void __launch_bounds__(256) k_knn2(const uint8_t* q, long long q_fs, const int* nq_arr, int nq_const,
@@ -72,12 +98,7 @@ __global__ void __launch_bounds__(256) k_knn2(const uint8_t* q, long long q_fs, 
         load_desc(T + (long long)j * 32, b0, b1);
         top2_insert(k0, k1, ((unsigned)popc256(a0, a1, b0, b1) << 20) | (unsigned)j);
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const unsigned o0 = __shfl_xor_sync(0xffffffffu, k0, o), o1 = __shfl_xor_sync(0xffffffffu, k1, o);
-        top2_insert(k0, k1, o0);
-        top2_insert(k0, k1, o1);
-    }
+    top2_warp32(k0, k1);
     if (lane == 0) {
         int4 r;
         r.x = k0 == 0xffffffffu ? -1 : (int)(k0 & 0xfffff); r.y = k0 == 0xffffffffu ? -1 : (int)(k0 >> 20);
@@ -202,6 +223,20 @@ __device__ __forceinline__ int rot_bin(float a1, float a2) {                 // 
     return bin;
 }
 
+// ComputeThreeMaxima (ORBmatcher.cc:1604-1645) over a rotation histogram: the three kept bins, -1 for one it drops
+__device__ __forceinline__ int3 three_maxima(const int* hist) {
+    int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
+    for (int i = 0; i < HISTO_LENGTH; i++) {
+        const int s = hist[i];
+        if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = i; }
+        else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = i; }
+        else if (s > max3) { max3 = s; ind3 = i; }
+    }
+    if ((float)max2 < __fmul_rn(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
+    else if ((float)max3 < __fmul_rn(0.1f, (float)max1)) { ind3 = -1; }
+    return make_int3(ind1, ind2, ind3);
+}
+
 __device__ __forceinline__ int find_node(const int* nodes, int nn, int id) {   // map::find on the ascending CSR node list
     int lo = 0, hi = nn;
     while (lo < hi) { int mid = (lo + hi) >> 1; if (nodes[mid] < id) lo = mid + 1; else hi = mid; }
@@ -241,12 +276,7 @@ __global__ void __launch_bounds__(128) k_bow_match(FrameSet S, int mode, float n
             load_desc(D2 + (long long)id2 * 32, c0, c1);
             top2_insert(k0, k1, ((unsigned)popc256(a0, a1, c0, c1) << 20) | (unsigned)(i2 - b2));
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const unsigned o0 = __shfl_xor_sync(0xffffffffu, k0, o), o1 = __shfl_xor_sync(0xffffffffu, k1, o);
-            top2_insert(k0, k1, o0);
-            top2_insert(k0, k1, o1);
-        }
+        top2_warp32(k0, k1);
         // bestDist1 = smallest distance (first position wins), bestDist2 = second order statistic; both start at 256
         const int best1 = k0 == 0xffffffffu ? 256 : (int)(k0 >> 20);
         const int best2 = k1 == 0xffffffffu ? 256 : (int)(k1 >> 20);
@@ -387,6 +417,24 @@ __global__ void __launch_bounds__(128) k_grid_cells(const float* x, const float*
     cell[f * cell_fs + i] = (px < 0 || px >= GRID_COLS || py < 0 || py >= GRID_ROWS) ? -1 : px * GRID_ROWS + py;
 }
 
+// the cell range of Frame::GetFeaturesInArea(x, y, r) (Frame.cc:375-393) on the grid of k_grid_cells; false when the window misses it
+__device__ __forceinline__ bool grid_window(float minX, float minY, float invW, float invH, float x, float y, float r,
+                                            int& cx0, int& cx1, int& cy0, int& cy1) {
+    cx0 = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(x, minX), r), invW)));
+    if (cx0 >= GRID_COLS) return false;
+    cx1 = min(GRID_COLS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(x, minX), r), invW)));
+    if (cx1 < 0) return false;
+    cy0 = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(y, minY), r), invH)));
+    if (cy0 >= GRID_ROWS) return false;
+    cy1 = min(GRID_ROWS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(y, minY), r), invH)));
+    return cy1 >= 0;
+}
+// the feature of a window key (dist << 40 | cell rank << 20 | position in the cell) over the window from (cx0, cy0), ny cells high
+__device__ __forceinline__ int grid_key_feature(const int* goff, const int* gidx, int cx0, int cy0, int ny, unsigned long long key) {
+    const int c = (int)((key >> 20) & 0xfffff), pos = (int)(key & 0xfffff);
+    return gidx[goff[(cx0 + c / ny) * GRID_ROWS + cy0 + c % ny] + pos];
+}
+
 // One warp per frame pair (blockIdx.x); see ProjPair for the layout.
 __global__ void __launch_bounds__(32) k_proj_match(const __grid_constant__ ProjArgs A, const __grid_constant__ ProjPair P) {
     __shared__ int s_hist[HISTO_LENGTH];
@@ -435,15 +483,8 @@ __global__ void __launch_bounds__(32) k_proj_match(const __grid_constant__ ProjA
             if ((unsigned)lo >= (unsigned)A.nlevels) continue;        // outside mvScaleFactors: never read scale[] out of range
             const float r = __fmul_rn(th, A.scale[lo]);
             const int minLevel = A.forward ? lo : (A.backward ? 0 : lo - 1), maxLevel = A.forward ? -1 : (A.backward ? lo : lo + 1);
-            // GetFeaturesInArea (Frame.cc:368-421)
-            const int cx0 = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(u, A.minX), r), A.invW)));
-            if (cx0 >= GRID_COLS) continue;
-            const int cx1 = min(GRID_COLS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(u, A.minX), r), A.invW)));
-            if (cx1 < 0) continue;
-            const int cy0 = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(v, A.minY), r), A.invH)));
-            if (cy0 >= GRID_ROWS) continue;
-            const int cy1 = min(GRID_ROWS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(v, A.minY), r), A.invH)));
-            if (cy1 < 0) continue;
+            int cx0, cx1, cy0, cy1;                                  // GetFeaturesInArea (Frame.cc:368-421)
+            if (!grid_window(A.minX, A.minY, A.invW, A.invH, u, v, r, cx0, cx1, cy0, cy1)) continue;
             const bool checkLevels = (minLevel > 0) || (maxLevel >= 0);
             const int ny = cy1 - cy0 + 1, ncell = (cx1 - cx0 + 1) * ny;
             uint4 a0, a1;
@@ -469,13 +510,10 @@ __global__ void __launch_bounds__(32) k_proj_match(const __grid_constant__ ProjA
                     if (key < best) best = key;
                 }
             }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) { const unsigned long long t = __shfl_xor_sync(0xffffffffu, best, o); best = t < best ? t : best; }
+            best = warp_min(best);
             const int bestDist = best == ~0ull ? 256 : (int)(best >> 40);
             if (bestDist <= TH_HIGH) {
-                const int c = (int)((best >> 20) & 0xfffff), pos = (int)(best & 0xfffff);
-                const int cell = (cx0 + c / ny) * GRID_ROWS + cy0 + c % ny;
-                const int j = gidx[goff[cell] + pos];
+                const int j = grid_key_feature(goff, gidx, cx0, cy0, ny, best);
                 if (lane == 0) {
                     assign2[j] = i; claimed[j] = (fl >> 1) & 1;
                     sel[i] = j;
@@ -489,18 +527,7 @@ __global__ void __launch_bounds__(32) k_proj_match(const __grid_constant__ ProjA
         }
         __syncwarp();
         if (A.checkOri) {
-            if (lane == 0) {                                         // ComputeThreeMaxima, ORBmatcher.cc:1604-1645
-                int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
-                for (int i = 0; i < HISTO_LENGTH; i++) {
-                    const int sv = s_hist[i];
-                    if (sv > max1) { max3 = max2; max2 = max1; max1 = sv; ind3 = ind2; ind2 = ind1; ind1 = i; }
-                    else if (sv > max2) { max3 = max2; max2 = sv; ind3 = ind2; ind2 = i; }
-                    else if (sv > max3) { max3 = sv; ind3 = i; }
-                }
-                if ((float)max2 < __fmul_rn(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
-                else if ((float)max3 < __fmul_rn(0.1f, (float)max1)) { ind3 = -1; }
-                s_keep[0] = ind1; s_keep[1] = ind2; s_keep[2] = ind3;
-            }
+            if (lane == 0) { const int3 k = three_maxima(s_hist); s_keep[0] = k.x; s_keep[1] = k.y; s_keep[2] = k.z; }
             __syncwarp();
             const int k0 = s_keep[0], k1 = s_keep[1], k2 = s_keep[2];
             for (int i0 = 0; i0 < n1; i0 += 32) {
@@ -528,29 +555,6 @@ __global__ void __launch_bounds__(32) k_proj_match(const __grid_constant__ ProjA
 constexpr int TH_LOW_I = 50;                        // ORBmatcher.cc:38
 struct WinArgs { float minX, minY, invW, invH, th, nnratio; int bFactor, use_right, checkOri, window; float scale[32]; };
 
-__device__ __forceinline__ void top2_push(unsigned long long& a1, unsigned long long& a2, unsigned long long k) {
-    if (k < a1) { a2 = a1; a1 = k; } else if (k < a2) a2 = k;
-}
-__device__ __forceinline__ void top2_warp(unsigned long long& a1, unsigned long long& a2) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const unsigned long long b1 = __shfl_xor_sync(0xffffffffu, a1, o), b2 = __shfl_xor_sync(0xffffffffu, a2, o);
-        const unsigned long long lo = a1 < b1 ? a1 : b1, hi = a1 < b1 ? b1 : a1, m2 = a2 < b2 ? a2 : b2;
-        a1 = lo; a2 = hi < m2 ? hi : m2;
-    }
-}
-// the cell range of Frame::GetFeaturesInArea(x, y, r) (Frame.cc:375-393); false when the window misses the grid
-__device__ __forceinline__ bool grid_window(const WinArgs& A, float x, float y, float r, int& cx0, int& cx1, int& cy0, int& cy1) {
-    cx0 = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(x, A.minX), r), A.invW)));
-    if (cx0 >= GRID_COLS) return false;
-    cx1 = min(GRID_COLS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(x, A.minX), r), A.invW)));
-    if (cx1 < 0) return false;
-    cy0 = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(y, A.minY), r), A.invH)));
-    if (cy0 >= GRID_ROWS) return false;
-    cy1 = min(GRID_ROWS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(y, A.minY), r), A.invH)));
-    return cy1 >= 0;
-}
-
 __global__ void __launch_bounds__(32) k_proj_match_mps(const __grid_constant__ WinArgs A, int nmp, const uint8_t* flag /* bit0 in view && !bad, bit1 obs>0 */,
                                                         const float* px, const float* py, const float* pxr, const int* level, const float* viewcos, const uint8_t* dmp,
                                                         int n2, const uint8_t* d2, const float* x2, const float* y2, const int* oct2, const float* uright2,
@@ -568,8 +572,8 @@ __global__ void __launch_bounds__(32) k_proj_match_mps(const __grid_constant__ W
         const float rad = __fmul_rn(r, A.scale[lvl]);
         const float u = px[i], v = py[i];
         int cx0, cx1, cy0, cy1;
-        if (!grid_window(A, u, v, rad, cx0, cx1, cy0, cy1)) continue;
-        const int minLevel = lvl - 1, maxLevel = lvl;             // GetFeaturesInArea(..., nPredictedLevel-1, nPredictedLevel)
+        if (!grid_window(A.minX, A.minY, A.invW, A.invH, u, v, rad, cx0, cx1, cy0, cy1)) continue;
+        const int minLevel = lvl - 1, maxLevel = lvl;            // GetFeaturesInArea(..., nPredictedLevel-1, nPredictedLevel)
         const bool checkLevels = (minLevel > 0) || (maxLevel >= 0);
         const int ny = cy1 - cy0 + 1, ncell = (cx1 - cx0 + 1) * ny;
         uint4 a0, a1;
@@ -595,13 +599,9 @@ __global__ void __launch_bounds__(32) k_proj_match_mps(const __grid_constant__ W
         if (b1 == ~0ull) continue;
         const int bestDist = (int)(b1 >> 40);
         if (bestDist <= TH_HIGH) {
-            const int c = (int)((b1 >> 20) & 0xfffff), pos = (int)(b1 & 0xfffff);
-            const int j = gidx[goff[(cx0 + c / ny) * GRID_ROWS + cy0 + c % ny] + pos];
+            const int j = grid_key_feature(goff, gidx, cx0, cy0, ny, b1);
             int bestDist2 = 256, bestLevel2 = -1;
-            if (b2 != ~0ull) {
-                const int c2 = (int)((b2 >> 20) & 0xfffff), pos2 = (int)(b2 & 0xfffff);
-                bestDist2 = (int)(b2 >> 40); bestLevel2 = oct2[gidx[goff[(cx0 + c2 / ny) * GRID_ROWS + cy0 + c2 % ny] + pos2]];
-            }
+            if (b2 != ~0ull) { bestDist2 = (int)(b2 >> 40); bestLevel2 = oct2[grid_key_feature(goff, gidx, cx0, cy0, ny, b2)]; }
             if (oct2[j] == bestLevel2 && (float)bestDist > __fmul_rn(A.nnratio, (float)bestDist2)) continue;   // :117
             if (lane == 0) { assign2[j] = i; claimed[j] = (fl >> 1) & 1; }
             nmatches++;
@@ -823,8 +823,7 @@ __global__ void __launch_bounds__(128) k_line_fuse_search(int nml, const uint8_t
             const unsigned long long k = ((unsigned long long)popc256(a0, a1, c0, c1) << 32) | (unsigned)j;
             b = k < b ? k : b;
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) { const unsigned long long t = __shfl_xor_sync(0xffffffffu, b, o); b = t < b ? t : b; }
+        b = warp_min(b);
     }
     if (lane == 0) { best_idx[i] = b == ~0ull ? -1 : (int)(b & 0xffffffffu); best_dist[i] = b == ~0ull ? 0x7fffffff : (int)(b >> 32); }
 }
@@ -859,7 +858,7 @@ __global__ void __launch_bounds__(128) k_point_fuse_search(const __grid_constant
     if (act) {
         if (!kMap) { lvl = level[i]; u = pu[i]; v = pv[i]; ur = pur[i]; }
         const float rad = __fmul_rn(A.th, A.scale[lvl]);
-        if (grid_window(A, u, v, rad, cx0, cx1, cy0, cy1)) {
+        if (grid_window(A.minX, A.minY, A.invW, A.invH, u, v, rad, cx0, cx1, cy0, cy1)) {
             const int ny = cy1 - cy0 + 1, ncell = (cx1 - cx0 + 1) * ny;
             uint4 a0, a1;
             load_desc(dmp, a0, a1);
@@ -889,16 +888,12 @@ __global__ void __launch_bounds__(128) k_point_fuse_search(const __grid_constant
                     b = k < b ? k : b;
                 }
             }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) { const unsigned long long t = __shfl_xor_sync(0xffffffffu, b, o); b = t < b ? t : b; }
+            b = warp_min(b);
         }
     }
     if (lane == 0) {
         int bi = -1, bd = 256;
-        if (b != ~0ull) {
-            const int ny = cy1 - cy0 + 1, c = (int)((b >> 20) & 0xfffff), pos = (int)(b & 0xfffff);
-            bi = gidx[goff[(cx0 + c / ny) * GRID_ROWS + cy0 + c % ny] + pos]; bd = (int)(b >> 40);
-        }
+        if (b != ~0ull) { bi = grid_key_feature(goff, gidx, cx0, cy0, cy1 - cy0 + 1, b); bd = (int)(b >> 40); }
         best_idx[i] = bi; best_dist[i] = bd;
     }
 }
@@ -921,7 +916,7 @@ __global__ void __launch_bounds__(32) k_init_match(const __grid_constant__ WinAr
         if (level1 > 0) continue;                                 // :426
         const float u = prevx[i1], v = prevy[i1];
         int cx0, cx1, cy0, cy1;
-        if (!grid_window(A, u, v, rad, cx0, cx1, cy0, cy1)) continue;
+        if (!grid_window(A.minX, A.minY, A.invW, A.invH, u, v, rad, cx0, cx1, cy0, cy1)) continue;
         const int ny = cy1 - cy0 + 1, ncell = (cx1 - cx0 + 1) * ny;
         uint4 a0, a1;
         load_desc(d1 + (long long)i1 * 32, a0, a1);
@@ -945,8 +940,7 @@ __global__ void __launch_bounds__(32) k_init_match(const __grid_constant__ WinAr
         const int bestDist = (int)(b1 >> 40);
         const float bestDist2 = b2 == ~0ull ? (float)0x7fffffff : (float)(int)(b2 >> 40);
         if (bestDist <= TH_LOW_I && (float)bestDist < __fmul_rn(bestDist2, A.nnratio)) {       // :462-464
-            const int c = (int)((b1 >> 20) & 0xfffff), pos = (int)(b1 & 0xfffff);
-            const int j = gidx[goff[(cx0 + c / ny) * GRID_ROWS + cy0 + c % ny] + pos];
+            const int j = grid_key_feature(goff, gidx, cx0, cy0, ny, b1);
             const int old = matches21[j];
             if (old >= 0) nmatches--;
             if (lane == 0) {
@@ -960,18 +954,7 @@ __global__ void __launch_bounds__(32) k_init_match(const __grid_constant__ WinAr
     }
     __syncwarp();
     if (A.checkOri) {
-        if (lane == 0) {                                         // ComputeThreeMaxima, ORBmatcher.cc:1604-1645
-            int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
-            for (int i = 0; i < HISTO_LENGTH; i++) {
-                const int sv = s_hist[i];
-                if (sv > max1) { max3 = max2; max2 = max1; max1 = sv; ind3 = ind2; ind2 = ind1; ind1 = i; }
-                else if (sv > max2) { max3 = max2; max2 = sv; ind3 = ind2; ind2 = i; }
-                else if (sv > max3) { max3 = sv; ind3 = i; }
-            }
-            if ((float)max2 < __fmul_rn(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
-            else if ((float)max3 < __fmul_rn(0.1f, (float)max1)) { ind3 = -1; }
-            s_keep[0] = ind1; s_keep[1] = ind2; s_keep[2] = ind3;
-        }
+        if (lane == 0) { const int3 k = three_maxima(s_hist); s_keep[0] = k.x; s_keep[1] = k.y; s_keep[2] = k.z; }
         __syncwarp();
         const int k0 = s_keep[0], k1 = s_keep[1], k2 = s_keep[2];
         for (int i0 = 0; i0 < n1; i0 += 32) {
@@ -1043,18 +1026,7 @@ __global__ void __launch_bounds__(256) k_rot_filter(int32_t* out, long long out_
     if (checkOri) {
         for (int i = tid; i < n; i += 256) if (O[i] >= 0) atomicAdd(&s_hist[R[i]], 1);
         __syncthreads();
-        if (tid == 0) {
-            int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
-            for (int i = 0; i < HISTO_LENGTH; i++) {
-                const int s = s_hist[i];
-                if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = i; }
-                else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = i; }
-                else if (s > max3) { max3 = s; ind3 = i; }
-            }
-            if ((float)max2 < __fmul_rn(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
-            else if ((float)max3 < __fmul_rn(0.1f, (float)max1)) { ind3 = -1; }
-            s_keep[0] = ind1; s_keep[1] = ind2; s_keep[2] = ind3;
-        }
+        if (tid == 0) { const int3 k = three_maxima(s_hist); s_keep[0] = k.x; s_keep[1] = k.y; s_keep[2] = k.z; }
         __syncthreads();
         const int k0 = s_keep[0], k1 = s_keep[1], k2 = s_keep[2];
         for (int i = tid; i < n; i += 256)
@@ -1264,6 +1236,50 @@ __device__ __forceinline__ int create_point(const CreateArgs& C, const float* T1
     return CNMP_CREATED;
 }
 
+// The steps both chain kernels below share.  A chain is a maximal run [c0, c1) of consecutive pairs with the same kf1; false when pair c0
+// does not start one.
+__device__ __forceinline__ bool chain_range(const int2* pmap, int npairs, int c0, int& kf1, int& c1) {
+    kf1 = pmap[c0].x;
+    if (c0 > 0 && pmap[c0 - 1].x == kf1) return false;
+    c1 = c0 + 1;
+    while (c1 < npairs && pmap[c1].x == kf1) c1++;
+    return true;
+}
+// s_bits = row kf1 of the mask as a bitmap of cap bits (all clear when !ok1), visible to the whole CTA on return
+__device__ __forceinline__ void chain_load_bits(unsigned* s_bits, const uint8_t* mask, int kf1, bool ok1, int cap, int tid) {
+    const int words = (cap + 31) / 32;
+    for (int w = tid; w < words; w += 256) {
+        unsigned b = 0;
+        for (int k = 0; k < 32 && ok1 && 32 * w + k < cap; k++) b |= (mask[(long long)kf1 * cap + 32 * w + k] != 0) << k;
+        s_bits[w] = b;
+    }
+    __syncthreads();
+}
+// pair p of the chain from c0 gets -1 (and leaves the bitmap alone) for kf1 or kf2 outside [0, nkf), kf2 == kf1 or a kf2 repeated in the chain
+__device__ __forceinline__ bool chain_pair_bad(const int2* pmap, int c0, int p, int kf1, bool ok1, int nkf, int& kf2) {
+    kf2 = pmap[p].y;
+    bool bad = !ok1 || (unsigned)kf2 >= (unsigned)nkf || kf2 == kf1;
+    for (int q = c0; q < p && !bad; q++) bad = pmap[q].y == kf2;
+    return bad;
+}
+// rows R[k] = (i, T[i]) of the i < n1 with T[i] >= 0 and bit i clear, in ascending i (block scan); returns the count
+__device__ __forceinline__ int chain_compact(const int32_t* T, int n1, const unsigned* s_bits, int* s_warp, int32_t* R, int tid) {
+    const int chunk = (n1 + 255) / 256, pb = min(n1, tid * chunk), pe = min(n1, pb + chunk);
+    int c = 0, total;
+    for (int i = pb; i < pe; i++) c += T[i] >= 0 && !((s_bits[i >> 5] >> (i & 31)) & 1u);
+    int o = block_exclusive_scan(c, s_warp, &total);
+    for (int i = pb; i < pe; i++)
+        if (T[i] >= 0 && !((s_bits[i >> 5] >> (i & 31)) & 1u)) { R[2 * o] = i; R[2 * o + 1] = T[i]; o++; }
+    return total;
+}
+// rows and statuses past the count cleared to -1, the pair's counts written; the bitmap bits set for pair p are visible on return
+__device__ __forceinline__ void chain_pair_end(int32_t* R, int32_t* S, int total, int cap, bool bad, int created, int p, int32_t* nmatch,
+                                               int32_t* nnew, int tid) {
+    for (int i = total + tid; i < cap; i += 256) { R[2 * i] = -1; R[2 * i + 1] = -1; S[i] = -1; }
+    if (tid == 0) { nmatch[p] = bad ? -1 : total; nnew[p] = created; }
+    __syncthreads();
+}
+
 // One CTA per chain (a maximal run of consecutive pairs with the same kf1: one keyframe's neighbour loop); CTAs that do not start a chain
 // return at once.  The KF1 features that have a MapPoint are a bitmap in shared memory, loaded from has_mp; for each pair in order the
 // CTA drops the unfiltered SearchForTriangulation rows (tw[p][idx1] = idx2 or -1) whose idx1 is set, compacts the rest in ascending idx1
@@ -1275,33 +1291,19 @@ __global__ void __launch_bounds__(256, 1) k_create_points_chain(const int2* pmap
     extern __shared__ unsigned s_bits[];
     __shared__ int s_warp[33];
     const int c0 = blockIdx.x, tid = threadIdx.x;
-    const int kf1 = pmap[c0].x;
-    if (c0 > 0 && pmap[c0 - 1].x == kf1) return;
-    int c1 = c0 + 1;
-    while (c1 < npairs && pmap[c1].x == kf1) c1++;
+    int kf1, c1;
+    if (!chain_range(pmap, npairs, c0, kf1, c1)) return;
     const bool ok1 = (unsigned)kf1 < (unsigned)nkf;
-    const int n1 = ok1 ? max(0, min(n_arr[kf1], cap)) : 0, words = (cap + 31) / 32;
-    for (int w = tid; w < words; w += 256) {
-        unsigned b = 0;
-        for (int k = 0; k < 32 && ok1 && 32 * w + k < cap; k++) b |= (has_mp[(long long)kf1 * cap + 32 * w + k] != 0) << k;
-        s_bits[w] = b;
-    }
-    __syncthreads();
+    const int n1 = ok1 ? max(0, min(n_arr[kf1], cap)) : 0;
+    chain_load_bits(s_bits, has_mp, kf1, ok1, cap, tid);
     const float* K1 = kp + 7LL * cap * (ok1 ? kf1 : 0);
     for (int p = c0; p < c1; p++) {
-        const int kf2 = pmap[p].y;
-        bool bad = !ok1 || (unsigned)kf2 >= (unsigned)nkf || kf2 == kf1;
-        for (int q = c0; q < p && !bad; q++) bad = pmap[q].y == kf2;
+        int kf2;
+        const bool bad = chain_pair_bad(pmap, c0, p, kf1, ok1, nkf, kf2);
         int32_t* R = rows + 2LL * cap * p; int32_t* S = status + (long long)cap * p; float* X3 = x3d + 3LL * cap * p;
         int total = 0, created = 0;
         if (!bad) {                                                              // CTA-uniform
-            const int32_t* Tw = tw + (long long)cap * p;
-            const int chunk = (n1 + 255) / 256, pb = min(n1, tid * chunk), pe = min(n1, pb + chunk);
-            int c = 0;
-            for (int i = pb; i < pe; i++) c += Tw[i] >= 0 && !((s_bits[i >> 5] >> (i & 31)) & 1u);
-            int o = block_exclusive_scan(c, s_warp, &total);
-            for (int i = pb; i < pe; i++)
-                if (Tw[i] >= 0 && !((s_bits[i >> 5] >> (i & 31)) & 1u)) { R[2 * o] = i; R[2 * o + 1] = Tw[i]; o++; }
+            total = chain_compact(tw + (long long)cap * p, n1, s_bits, s_warp, R, tid);
             __syncthreads();                                                     // the rows (global) and every bitmap read are done
             const float* K2 = kp + 7LL * cap * kf2;
             const float* T1 = pose + 15LL * kf1; const float* T2 = pose + 15LL * kf2;
@@ -1321,9 +1323,7 @@ __global__ void __launch_bounds__(256, 1) k_create_points_chain(const int2* pmap
             block_exclusive_scan(created, s_warp, &all);
             created = all;
         }
-        for (int i = total + tid; i < cap; i += 256) { R[2 * i] = -1; R[2 * i + 1] = -1; S[i] = -1; }
-        if (tid == 0) { nmatch[p] = bad ? -1 : total; nnew[p] = created; }
-        __syncthreads();
+        chain_pair_end(R, S, total, cap, bad, created, p, nmatch, nnew, tid);
     }
 }
 
@@ -1425,34 +1425,20 @@ __global__ void __launch_bounds__(256, 1) k_create_lines_chain(const int2* pmap,
     __shared__ int s_warp[33];
     __shared__ float s_T[2][15], s_M[2][12];
     const int c0 = blockIdx.x, tid = threadIdx.x;
-    const int kf1 = pmap[c0].x;
-    if (c0 > 0 && pmap[c0 - 1].x == kf1) return;
-    int c1 = c0 + 1;
-    while (c1 < npairs && pmap[c1].x == kf1) c1++;
+    int kf1, c1;
+    if (!chain_range(pmap, npairs, c0, kf1, c1)) return;
     const bool ok1 = (unsigned)kf1 < (unsigned)nkf;
-    const int n1 = ok1 ? max(0, min(nl[kf1], capl)) : 0, words = (capl + 31) / 32;
-    for (int w = tid; w < words; w += 256) {
-        unsigned b = 0;
-        for (int k = 0; k < 32 && ok1 && 32 * w + k < capl; k++) b |= (has_ml[(long long)kf1 * capl + 32 * w + k] != 0) << k;
-        s_bits[w] = b;
-    }
-    __syncthreads();
+    const int n1 = ok1 ? max(0, min(nl[kf1], capl)) : 0;
+    chain_load_bits(s_bits, has_ml, kf1, ok1, capl, tid);
     const long long o1 = (long long)capl * (ok1 ? kf1 : 0);
     for (int p = c0; p < c1; p++) {
-        const int kf2 = pmap[p].y;
-        bool bad = !ok1 || (unsigned)kf2 >= (unsigned)nkf || kf2 == kf1;
-        for (int q = c0; q < p && !bad; q++) bad = pmap[q].y == kf2;
+        int kf2;
+        bool bad = chain_pair_bad(pmap, c0, p, kf1, ok1, nkf, kf2);
         if (!bad) bad = n1 > 0 && min(nl[kf2], capl) < 2;
         int32_t* R = rows + 2LL * capl * p; int32_t* S = status + (long long)capl * p; float* L3 = line3d + 6LL * capl * p;
         int total = 0, created = 0;
         if (!bad && n1 > 0) {                                                    // CTA-uniform
-            const int32_t* Tw = tw + (long long)capl * p;
-            const int chunk = (n1 + 255) / 256, pb = min(n1, tid * chunk), pe = min(n1, pb + chunk);
-            int c = 0;
-            for (int i = pb; i < pe; i++) c += Tw[i] >= 0 && !((s_bits[i >> 5] >> (i & 31)) & 1u);
-            int o = block_exclusive_scan(c, s_warp, &total);
-            for (int i = pb; i < pe; i++)
-                if (Tw[i] >= 0 && !((s_bits[i >> 5] >> (i & 31)) & 1u)) { R[2 * o] = i; R[2 * o + 1] = Tw[i]; o++; }
+            total = chain_compact(tw + (long long)capl * p, n1, s_bits, s_warp, R, tid);
             if (tid < 30) s_T[tid / 15][tid % 15] = pose[15LL * (tid < 15 ? kf1 : kf2) + tid % 15];
             __syncthreads();                                                     // the rows (global), the poses and every bitmap read are done
             if (tid < 2) proj_mat(C, s_T[tid], s_M[tid]);
@@ -1476,9 +1462,7 @@ __global__ void __launch_bounds__(256, 1) k_create_lines_chain(const int2* pmap,
             block_exclusive_scan(created, s_warp, &all);
             created = all;
         }
-        for (int i = total + tid; i < capl; i += 256) { R[2 * i] = -1; R[2 * i + 1] = -1; S[i] = -1; }
-        if (tid == 0) { nmatch[p] = bad ? -1 : total; nnew[p] = created; }
-        __syncthreads();
+        chain_pair_end(R, S, total, capl, bad, created, p, nmatch, nnew, tid);
     }
 }
 
@@ -1564,33 +1548,135 @@ template <class T> T* stage(Arena& A, const T* host, size_t count, cudaStream_t 
     return d;
 }
 
-int upload_featvec(sslpl_matcher* m, int slot, const sslpl_featvec* fv, int n) {
-    const int NN = m->p.max_nodes + 1;
+// every kernel launch of the matcher: on its stream, counted by sslpl_matcher_launch_count
+template <class T> struct same_type { using type = T; };
+template <class... KArgs>
+void launch(sslpl_matcher* m, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, typename same_type<KArgs>::type... args) {
+    kernel<<<grid, block, smem, m->stream>>>(args...);
+    m->launches++;
+}
+
+// a workspace of the handle allocated by the first call that needs it (a handle that never gets there never pays for it), freed with it
+template <class T> int first_use(T*& p, size_t bytes) {
+    if (p) return SSLPL_OK;
+    cudaError_t e = cudaMalloc(&p, bytes);
+    if (e != cudaSuccess) { p = nullptr; set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return SSLPL_ERR_CUDA; }
+    return SSLPL_OK;
+}
+
+int featvec_ok(const sslpl_matcher* m, const sslpl_featvec* fv, int n) {
     SSLPL_REQUIRE(fv && fv->nn >= 0 && fv->nn <= m->p.max_nodes, SSLPL_ERR_ARG, "feature vector has more nodes than max_nodes");
     if (fv->nn == 0) return SSLPL_OK;
     SSLPL_REQUIRE(fv->nodes && fv->off && fv->idx, SSLPL_ERR_ARG, "null feature vector arrays");
     SSLPL_REQUIRE(fv->off[fv->nn] <= n, SSLPL_ERR_ARG, "feature vector indexes more features than given");
+    return SSLPL_OK;
+}
+
+// a feature vector that featvec_ok accepted
+int upload_featvec(sslpl_matcher* m, int slot, const sslpl_featvec* fv) {
+    const int NN = m->p.max_nodes + 1;
+    if (fv->nn == 0) return SSLPL_OK;
     SSLPL_CUDA(cudaMemcpyAsync(m->nodes + slot * NN, fv->nodes, sizeof(int) * fv->nn, cudaMemcpyHostToDevice, m->stream));
     SSLPL_CUDA(cudaMemcpyAsync(m->off + slot * (NN + 1), fv->off, sizeof(int) * (fv->nn + 1), cudaMemcpyHostToDevice, m->stream));
     SSLPL_CUDA(cudaMemcpyAsync(m->idx + slot * m->cap, fv->idx, sizeof(int) * fv->off[fv->nn], cudaMemcpyHostToDevice, m->stream));
     return SSLPL_OK;
 }
 
-FrameSet staging_set(sslpl_matcher* m, int nn1, int nn2, bool with_flags) {
+FrameSet staging_set(sslpl_matcher* m) {
     const int NN = m->p.max_nodes + 1;
     FrameSet S; memset(&S, 0, sizeof(S));
     S.desc = m->desc; S.desc_fs = (long long)m->cap * 32;
     S.nodes = m->nodes; S.off = m->off; S.idx = m->idx; S.nodes_fs = NN; S.off_fs = NN + 1; S.idx_fs = m->cap;
-    S.nn = m->nn2; (void)nn1; (void)nn2;
-    S.flag = with_flags ? m->flag : nullptr; S.flag_fs = m->cap;
+    S.nn = m->nn2;
+    S.flag = m->flag; S.flag_fs = m->cap;
     S.angle = m->kpf + 3; S.x = m->kpf; S.y = m->kpf + 1; S.oct = reinterpret_cast<const int*>(m->kpf + 5);
     S.angle_es = 7; S.angle_fs = (long long)m->cap * 7;
     return S;
 }
 
+// A frame set in HBM ([..][cap] descriptors and sslpl_keypoint rows) whose FeatureVectors k_build_csr wrote into b_off / b_idx for a
+// dense vocabulary level: every frame lists the nodes 0..nc-1, so all share the iota array
+FrameSet dense_set(sslpl_matcher* m, const uint8_t* d_desc, const sslpl_keypoint* d_kps, int cap, int nc, const uint8_t* flag) {
+    FrameSet S; memset(&S, 0, sizeof(S));
+    S.desc = d_desc; S.desc_fs = (long long)cap * 32;
+    S.nodes = m->iota; S.nodes_fs = 0; S.nn = nullptr; S.nn_const = nc;
+    S.off = m->b_off; S.idx = m->b_idx; S.off_fs = m->p.max_nodes + 2; S.idx_fs = m->p.max_features + 64;
+    S.flag = flag; S.flag_fs = cap;
+    const float* kf = reinterpret_cast<const float*>(d_kps);
+    S.angle = kf + 3; S.x = kf; S.y = kf + 1; S.oct = reinterpret_cast<const int*>(kf + 5); S.angle_es = 7; S.angle_fs = (long long)cap * 7;
+    return S;
+}
+
 int fill(sslpl_matcher* m, int32_t* p, long long n, int v) {
     if (n <= 0) return SSLPL_OK;
-    k_fill_i32<<<(unsigned)((n + 255) / 256), 256, 0, m->stream>>>(p, n, v); m->launches++;
+    launch(m, k_fill_i32, (unsigned)((n + 255) / 256), 256, 0, p, n, v);
+    return SSLPL_OK;
+}
+
+// k_build_csr keeps nc + 1 counters and a frame's cap node ids in shared memory
+int csr_fits(int nc, int cap) {
+    SSLPL_REQUIRE((size_t)((nc + 1 + cap) * sizeof(int)) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY,
+                  "nodes + features exceed the shared memory of one CTA ((nc + 1 + cap) * 4 <= 200 KB)");
+    return SSLPL_OK;
+}
+
+// The single-pair grid matchers build the 64 x 48 grid CSR of the current frame in staging slot 1 of the node lists (max_nodes >= 3072)
+// with one k_build_csr CTA; at most 8192 features keep that CTA within MAX_DYN_SMEM.
+constexpr int GRID_MAX_FEATURES = 8192;
+static_assert((GRID_COLS * GRID_ROWS + 1 + GRID_MAX_FEATURES + 64) * sizeof(int) <= MAX_DYN_SMEM, "grid CSR of one frame exceeds MAX_DYN_SMEM");
+int grid_staging_ok(const sslpl_matcher* m) {
+    SSLPL_REQUIRE(m->cap <= GRID_MAX_FEATURES + 64, SSLPL_ERR_ARG, "the matcher capacity exceeds 8192 features");
+    SSLPL_REQUIRE(m->p.max_nodes >= GRID_COLS * GRID_ROWS, SSLPL_ERR_ARG, "the matcher needs max_nodes >= 3072 (64 x 48 grid cells)");
+    return SSLPL_OK;
+}
+// Frame::AssignFeaturesToGrid of the n2 features at (x[i], y[i]) into goff / gidx.  h_small is written here: the caller has synchronised
+// the stream since h_small's last asynchronous copy, and does not write it again before its next synchronisation.
+int grid_staging_build(sslpl_matcher* m, const float* x, const float* y, int n2, float minX, float minY, float invW, float invH,
+                       int*& goff, int*& gidx) {
+    const int nc = GRID_COLS * GRID_ROWS;
+    goff = m->off + (m->p.max_nodes + 2); gidx = m->idx + m->cap;
+    m->h_small[0] = n2;
+    SSLPL_CUDA(cudaMemcpyAsync(m->ncnt, m->h_small, sizeof(int), cudaMemcpyHostToDevice, m->stream));
+    launch(m, k_grid_cells, (n2 + 127) / 128, 128, 0, x, y, 1, 0, nullptr, n2, n2, minX, minY, invW, invH, m->node, 0);
+    launch(m, k_build_csr, 1, 128, (nc + 1 + m->cap) * sizeof(int), m->node, 0, m->ncnt, m->cap, nc, goff, 0, gidx, 0);
+    return SSLPL_OK;
+}
+
+// The per-frame grid workspace of the batched projection matchers ([max_batch + 1] frames): per frame the grid cell of every feature
+// and the grid CSR, and the motion-model walker's claimed / sel / rbin tables.
+int ensure_grid_ws(sslpl_matcher* m) {
+    const int B = m->p.max_batch + 1, fc = m->p.max_features + 64, nc = GRID_COLS * GRID_ROWS;
+    Arena W;
+    for (int k = 0; k < 2; k++) {
+        m->pw_cell = W.take<int32_t>((size_t)B * fc); m->pw_off = W.take<int>((size_t)B * (nc + 1)); m->pw_idx = W.take<int>((size_t)B * fc);
+        m->pw_sel = W.take<int32_t>((size_t)B * fc); m->pw_claimed = W.take<uint8_t>((size_t)B * fc); m->pw_rbin = W.take<uint8_t>((size_t)B * fc);
+        if (k == 0) {
+            if (int rc = first_use(m->pw, W.used)) return rc;
+            W.base = m->pw; W.size = W.used; W.used = 0;
+        }
+    }
+    return SSLPL_OK;
+}
+// Frame::AssignFeaturesToGrid of nframes frames in HBM (sslpl_keypoint rows from kp, frame stride 7 cap floats, counts n[f]): the grid CSR
+// of frame f at pw_off + f (nc + 1), pw_idx + f fc; the caller has checked csr_fits(3072, cap)
+int grid_batch_build(sslpl_matcher* m, const float* kp, const int* n, int nframes, int cap, float minX, float minY, float invW, float invH) {
+    if (int rc = ensure_grid_ws(m)) return rc;
+    const int fc = m->p.max_features + 64, nc = GRID_COLS * GRID_ROWS;
+    launch(m, k_grid_cells, dim3((cap + 127) / 128, nframes), 128, 0, kp, kp + 1, 7, 7LL * cap, n, 0, cap, minX, minY, invW, invH, m->pw_cell, fc);
+    launch(m, k_build_csr, nframes, 128, (nc + 1 + cap) * sizeof(int), m->pw_cell, fc, n, cap, nc, m->pw_off, nc + 1, m->pw_idx, fc);
+    return SSLPL_OK;
+}
+
+// the sizes of a batched call over a keyframe set: nkf keyframes of cap rows (cap <= rows + 64: max_features or max_lines)
+int kf_set_ok(const sslpl_matcher* m, int nkf, int cap, int rows) {
+    SSLPL_REQUIRE(nkf >= 1 && nkf <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nkf outside [1, max_batch + 1]");
+    SSLPL_REQUIRE(cap >= 1 && cap <= rows + 64, SSLPL_ERR_ARG, "cap outside [1, max_features + 64] (lines: [1, max_lines + 64])");
+    return SSLPL_OK;
+}
+// ... and npairs keyframe pairs
+int kf_pairs_ok(const sslpl_matcher* m, int nkf, int cap, int rows, int npairs) {
+    if (int rc = kf_set_ok(m, nkf, cap, rows)) return rc;
+    SSLPL_REQUIRE(npairs >= 1 && npairs <= m->p.max_batch, SSLPL_ERR_ARG, "npairs outside [1, max_batch]");
     return SSLPL_OK;
 }
 
@@ -1612,12 +1698,13 @@ int common_bow(sslpl_matcher* m, int mode, const uint8_t* d1, int n1, const uint
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     const int nout = mode == 0 ? n2 : n1;
     if (nout == 0) { *nmatches = 0; return SSLPL_OK; }
+    int rc;
+    if ((rc = featvec_ok(m, fv1, n1)) || (rc = featvec_ok(m, fv2, n2))) return rc;
     cudaStream_t st = m->stream;
     const int cap = m->cap;
     if (n1) SSLPL_CUDA(cudaMemcpyAsync(m->desc, d1, (size_t)n1 * 32, cudaMemcpyHostToDevice, st));
     if (n2) SSLPL_CUDA(cudaMemcpyAsync(m->desc + (size_t)cap * 32, d2, (size_t)n2 * 32, cudaMemcpyHostToDevice, st));
-    int rc;
-    if ((rc = upload_featvec(m, 0, fv1, n1)) || (rc = upload_featvec(m, 1, fv2, n2))) return rc;
+    if ((rc = upload_featvec(m, 0, fv1)) || (rc = upload_featvec(m, 1, fv2))) return rc;
     if ((rc = upload_angles(m, 0, angle1, n1)) || (rc = upload_angles(m, 1, angle2, n2))) return rc;
     if (n1) SSLPL_CUDA(cudaMemcpyAsync(m->flag, valid1, n1, cudaMemcpyHostToDevice, st));
     if (n2 && valid2) SSLPL_CUDA(cudaMemcpyAsync(m->flag + cap, valid2, n2, cudaMemcpyHostToDevice, st));
@@ -1627,12 +1714,9 @@ int common_bow(sslpl_matcher* m, int mode, const uint8_t* d1, int n1, const uint
     fill(m, m->out, nout, -1);
     SSLPL_CUDA(cudaMemsetAsync(m->rot, 255, nout, st));
     SSLPL_CUDA(cudaMemsetAsync(m->taken, 0, std::max(n2, 1), st));
-    FrameSet S = staging_set(m, fv1->nn, fv2->nn, true);
-    if (fv1->nn > 0 && fv2->nn > 0) {
-        k_bow_match<<<dim3((fv1->nn + 3) / 4, 1), 128, 0, st>>>(S, mode, nnratio, cap, m->out, 0, m->rot, 0, m->taken, 0);
-        m->launches++;
-    }
-    k_rot_filter<<<1, 256, 0, st>>>(m->out, 0, m->rot, 0, nullptr, 0, nout, cap, checkOri, m->nmatch, nullptr, 0); m->launches++;
+    if (fv1->nn > 0 && fv2->nn > 0)
+        launch(m, k_bow_match, dim3((fv1->nn + 3) / 4, 1), 128, 0, staging_set(m), mode, nnratio, cap, m->out, 0, m->rot, 0, m->taken, 0);
+    launch(m, k_rot_filter, 1, 256, 0, m->out, 0, m->rot, 0, nullptr, 0, nout, cap, checkOri, m->nmatch, nullptr, 0);
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(match, m->out, sizeof(int32_t) * nout, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaMemcpyAsync(m->h_small + 8, m->nmatch, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -1648,8 +1732,8 @@ int run_knn2(sslpl_matcher* m, const uint8_t* q, int nq, const uint8_t* t, int n
     cudaStream_t st = m->stream;
     SSLPL_CUDA(cudaMemcpyAsync(m->desc, q, (size_t)nq * 32, cudaMemcpyHostToDevice, st));
     if (nt) SSLPL_CUDA(cudaMemcpyAsync(m->desc + (size_t)m->cap * 32, t, (size_t)nt * 32, cudaMemcpyHostToDevice, st));
-    k_knn2<false><<<dim3((nq + 7) / 8, 1), 256, 0, st>>>(m->desc, 0, nullptr, nq, m->desc + (size_t)m->cap * 32, 0, nullptr, nt, m->knn, 0, nq, nullptr, 0);
-    m->launches++;
+    launch(m, k_knn2<false>, dim3((nq + 7) / 8, 1), 256, 0, m->desc, 0, nullptr, nq, m->desc + (size_t)m->cap * 32, 0, nullptr, nt, m->knn, 0, nq,
+           nullptr, 0);
     SSLPL_CUDA(cudaGetLastError());
     if (out_host) {
         SSLPL_CUDA(cudaMemcpyAsync(out_host, m->knn, sizeof(int32_t) * 4 * nq, cudaMemcpyDeviceToHost, st));
@@ -1753,7 +1837,7 @@ int sslpl_descriptor_distance(sslpl_matcher* m, const uint8_t* a, const uint8_t*
     cudaStream_t st = m->stream;
     SSLPL_CUDA(cudaMemcpyAsync(m->desc, a, (size_t)n * 32, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(m->desc + (size_t)m->cap * 32, b, (size_t)n * 32, cudaMemcpyHostToDevice, st));
-    k_pair_distance<<<(n + 127) / 128, 128, 0, st>>>(m->desc, m->desc + (size_t)m->cap * 32, n, m->out); m->launches++;
+    launch(m, k_pair_distance, (n + 127) / 128, 128, 0, m->desc, m->desc + (size_t)m->cap * 32, n, m->out);
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(dist, m->out, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaStreamSynchronize(st));
@@ -1770,12 +1854,12 @@ int sslpl_bow_assign(sslpl_matcher* m, const uint8_t* desc, int n, const uint8_t
     SSLPL_REQUIRE(m && (n == 0 || (desc && node)) && centroids, SSLPL_ERR_ARG, "null argument");
     SSLPL_REQUIRE(n >= 0 && n <= m->cap && nc >= 1 && nc <= m->p.max_nodes, SSLPL_ERR_ARG, "n or nc exceeds the matcher capacity");
     if (n == 0) return SSLPL_OK;
+    SSLPL_REQUIRE((size_t)(nc * 32) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "too many centroids for one shared-memory tile (nc <= 6400)");
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
     SSLPL_CUDA(cudaMemcpyAsync(m->desc, desc, (size_t)n * 32, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(m->cent, centroids, (size_t)nc * 32, cudaMemcpyHostToDevice, st));
-    SSLPL_REQUIRE((size_t)(nc * 32) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "too many centroids for one shared-memory tile (nc <= 6400)");
-    k_bow_assign<<<dim3((n + 127) / 128, 1), 128, nc * 32, st>>>(m->desc, 0, nullptr, n, n, m->cent, nc, m->node, 0); m->launches++;
+    launch(m, k_bow_assign, dim3((n + 127) / 128, 1), 128, nc * 32, m->desc, 0, nullptr, n, n, m->cent, nc, m->node, 0);
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(node, m->node, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaStreamSynchronize(st));
@@ -1805,13 +1889,14 @@ int sslpl_search_for_triangulation(sslpl_matcher* m, const uint8_t* d1, int n1, 
     *nmatches = 0;
     if (n1 == 0 || n2 == 0) return SSLPL_OK;
     for (int i = 0; i < n2; i++) SSLPL_REQUIRE(kp2[i].octave >= 0 && kp2[i].octave < nlevels, SSLPL_ERR_ARG, "keypoint octave out of range");
+    int rc;
+    if ((rc = featvec_ok(m, fv1, n1)) || (rc = featvec_ok(m, fv2, n2))) return rc;
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
     const int cap = m->cap;
     SSLPL_CUDA(cudaMemcpyAsync(m->desc, d1, (size_t)n1 * 32, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(m->desc + (size_t)cap * 32, d2, (size_t)n2 * 32, cudaMemcpyHostToDevice, st));
-    int rc;
-    if ((rc = upload_featvec(m, 0, fv1, n1)) || (rc = upload_featvec(m, 1, fv2, n2))) return rc;
+    if ((rc = upload_featvec(m, 0, fv1)) || (rc = upload_featvec(m, 1, fv2))) return rc;
     SSLPL_CUDA(cudaMemcpyAsync(m->kpf, kp1, (size_t)n1 * 28, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(m->kpf + (size_t)cap * 7, kp2, (size_t)n2 * 28, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(m->flag, has_mp1, n1, cudaMemcpyHostToDevice, st));
@@ -1820,13 +1905,12 @@ int sslpl_search_for_triangulation(sslpl_matcher* m, const uint8_t* d1, int n1, 
     SSLPL_CUDA(cudaMemcpyAsync(m->nn2, m->h_small, 2 * sizeof(int), cudaMemcpyHostToDevice, st));
     fill(m, m->out, n1, -1);
     SSLPL_CUDA(cudaMemsetAsync(m->rot, 255, n1, st));
-    FrameSet S = staging_set(m, fv1->nn, fv2->nn, true);
     TriArgs T;
     for (int i = 0; i < 9; i++) T.F[i] = F12[i];
     T.ex = ex; T.ey = ey; T.nlevels = nlevels;
     for (int i = 0; i < SSLPL_MAX_LEVELS; i++) { T.scale[i] = i < nlevels ? scale[i] : 0.f; T.sigma2[i] = i < nlevels ? sigma2[i] : 0.f; }
-    if (fv1->nn > 0 && fv2->nn > 0) { k_tri_match<false><<<dim3((fv1->nn + 3) / 4, 1), 128, 0, st>>>(S, T, nullptr, m->out, 0, m->rot, 0); m->launches++; }
-    k_rot_filter<<<1, 256, 0, st>>>(m->out, 0, m->rot, 0, nullptr, 0, n1, cap, checkOri, m->nmatch, m->pairs, 0); m->launches++;
+    if (fv1->nn > 0 && fv2->nn > 0) launch(m, k_tri_match<false>, dim3((fv1->nn + 3) / 4, 1), 128, 0, staging_set(m), T, nullptr, m->out, 0, m->rot, 0);
+    launch(m, k_rot_filter, 1, 256, 0, m->out, 0, m->rot, 0, nullptr, 0, n1, cap, checkOri, m->nmatch, m->pairs, 0);
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(m->h_small + 8, m->nmatch, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaStreamSynchronize(st));
@@ -1877,29 +1961,19 @@ int sslpl_line_match(sslpl_matcher* m, int mode, const uint8_t* d1, int n1, cons
     return SSLPL_OK;
 }
 
-// common tail of the batched consecutive-frame SearchByBoW: b_node holds the dense node index (or -1) of every feature
+// common tail of the batched consecutive-frame SearchByBoW: b_node holds the dense node index (or -1) of every feature; the caller has
+// checked csr_fits(nc, cap)
 static int bow_batch_tail(sslpl_matcher* m, const uint8_t* d_desc, const sslpl_keypoint* d_kps, const int* d_n, int nframes, int cap, int nc,
                           float nnratio, int checkOri, int32_t* d_match, int32_t* d_nmatch) {
     cudaStream_t st = m->stream;
     const int npairs = nframes - 1, fc = m->p.max_features + 64, NN = m->p.max_nodes + 1;
-    SSLPL_REQUIRE((size_t)((nc + 1 + cap) * sizeof(int)) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "nodes + features exceed the shared memory of one CTA ((nc + 1 + cap) * 4 <= 200 KB)");
-    k_build_csr<<<nframes, 128, (nc + 1 + cap) * sizeof(int), st>>>(m->b_node, fc, d_n, cap, nc, m->b_off, NN + 1, m->b_idx, fc);
-    m->launches += 1;
+    launch(m, k_build_csr, nframes, 128, (nc + 1 + cap) * sizeof(int), m->b_node, fc, d_n, cap, nc, m->b_off, NN + 1, m->b_idx, fc);
     fill(m, d_match, (long long)npairs * cap, -1);
     SSLPL_CUDA(cudaMemsetAsync(m->b_rot, 255, (size_t)npairs * fc, st));
     SSLPL_CUDA(cudaMemsetAsync(m->b_taken, 0, (size_t)npairs * fc, st));
-    FrameSet S; memset(&S, 0, sizeof(S));
-    S.desc = d_desc; S.desc_fs = (long long)cap * 32;
-    S.n = d_n;
-    S.nodes = nullptr; S.off = m->b_off; S.idx = m->b_idx; S.off_fs = NN + 1; S.idx_fs = fc;
-    // dense vocabulary: node list is 0..nc-1 for every frame -> reuse one iota array
-    S.nodes = m->iota; S.nodes_fs = 0; S.nn = nullptr; S.nn_const = nc;
-    S.flag = nullptr;
-    const float* kf = reinterpret_cast<const float*>(d_kps);
-    S.angle = kf + 3; S.x = kf; S.y = kf + 1; S.oct = reinterpret_cast<const int*>(kf + 5); S.angle_es = 7; S.angle_fs = (long long)cap * 7;
-    k_bow_match<<<dim3((nc + 3) / 4, npairs), 128, 0, st>>>(S, 0, nnratio, cap, d_match, cap, m->b_rot, fc, m->b_taken, fc);
-    k_rot_filter<<<npairs, 256, 0, st>>>(d_match, cap, m->b_rot, fc, d_n, 1, 0, cap, checkOri, d_nmatch, nullptr, 0);
-    m->launches += 2;
+    launch(m, k_bow_match, dim3((nc + 3) / 4, npairs), 128, 0, dense_set(m, d_desc, d_kps, cap, nc, nullptr), 0, nnratio, cap, d_match, cap,
+           m->b_rot, fc, m->b_taken, fc);
+    launch(m, k_rot_filter, npairs, 256, 0, d_match, cap, m->b_rot, fc, d_n, 1, 0, cap, checkOri, d_nmatch, nullptr, 0);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
@@ -1910,11 +1984,11 @@ int sslpl_match_bow_batch_device(sslpl_matcher* m, const uint8_t* d_desc, const 
     SSLPL_REQUIRE(m && d_desc && d_kps && d_n && d_centroids && d_match && d_nmatch, SSLPL_ERR_ARG, "null argument");
     SSLPL_REQUIRE(nframes >= 2 && nframes <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nframes exceeds max_batch+1");
     SSLPL_REQUIRE(cap >= 1 && cap <= m->p.max_features + 64 && nc >= 1 && nc <= m->p.max_nodes, SSLPL_ERR_ARG, "cap or nc exceeds the matcher capacity");
+    SSLPL_REQUIRE((size_t)(nc * 32) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "too many centroids for one shared-memory tile (nc <= 6400)");
+    if (int rc = csr_fits(nc, cap)) return rc;
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     const int fc = m->p.max_features + 64;
-    SSLPL_REQUIRE((size_t)(nc * 32) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "too many centroids for one shared-memory tile (nc <= 6400)");
-    k_bow_assign<<<dim3((cap + 127) / 128, nframes), 128, nc * 32, m->stream>>>(d_desc, (long long)cap * 32, d_n, 0, cap, d_centroids, nc, m->b_node, fc);
-    m->launches += 1;
+    launch(m, k_bow_assign, dim3((cap + 127) / 128, nframes), 128, nc * 32, d_desc, (long long)cap * 32, d_n, 0, cap, d_centroids, nc, m->b_node, fc);
     return bow_batch_tail(m, d_desc, d_kps, d_n, nframes, cap, nc, nnratio, checkOri, d_match, d_nmatch);
 }
 
@@ -1925,8 +1999,8 @@ int sslpl_search_by_projection_frame(sslpl_matcher* m,
         const uint8_t* claimed2, const float* Tcw, const float* Tlw, const float* cam, const float* bounds,
         const float* scaleFactors, int nlevels, float th, int bMono, int checkOri, int32_t* assign2, int* nmatches) {
     SSLPL_REQUIRE(m && assign2 && nmatches && Tcw && cam && bounds && scaleFactors, SSLPL_ERR_ARG, "null argument");
-    SSLPL_REQUIRE(n1 >= 0 && n2 >= 0 && n1 <= m->cap && n2 <= m->cap && m->cap <= 8192 + 64, SSLPL_ERR_ARG, "n1 / n2 exceed the matcher capacity (<= 8192 features)");
-    SSLPL_REQUIRE(m->p.max_nodes >= GRID_COLS * GRID_ROWS, SSLPL_ERR_ARG, "the matcher needs max_nodes >= 3072 (64 x 48 grid cells)");
+    SSLPL_REQUIRE(n1 >= 0 && n2 >= 0 && n1 <= m->cap && n2 <= m->cap, SSLPL_ERR_ARG, "n1 / n2 exceed the matcher capacity");
+    if (int rc = grid_staging_ok(m)) return rc;
     SSLPL_REQUIRE(nlevels >= 1 && nlevels <= 32, SSLPL_ERR_ARG, "nlevels out of range");
     SSLPL_REQUIRE(n1 == 0 || (valid1 && obs1 && Xw && dmp && oct1 && angle1), SSLPL_ERR_ARG, "null last-frame array");
     SSLPL_REQUIRE(n2 == 0 || (d2 && x2 && y2 && oct2 && angle2), SSLPL_ERR_ARG, "null current-frame array");
@@ -1937,7 +2011,7 @@ int sslpl_search_by_projection_frame(sslpl_matcher* m,
     for (int i = 0; i < n1; i++) SSLPL_REQUIRE(oct1[i] >= 0 && oct1[i] < nlevels, SSLPL_ERR_ARG, "last-frame octave outside the scale-factor table");
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
-    const int cap = m->cap, NN = m->p.max_nodes + 1, nc = GRID_COLS * GRID_ROWS;
+    const int cap = m->cap;
     ProjArgs A; memset(&A, 0, sizeof(A));
     for (int k = 0; k < 12; k++) A.T[k] = Tcw[k];
     A.fx = cam[0]; A.fy = cam[1]; A.cx = cam[2]; A.cy = cam[3]; A.mbf = cam[4];
@@ -1971,13 +2045,9 @@ int sslpl_search_by_projection_frame(sslpl_matcher* m,
     SSLPL_CUDA(cudaMemcpyAsync(m->flag, fl.data(), n1, cudaMemcpyHostToDevice, st));
     if (claimed2) SSLPL_CUDA(cudaMemcpyAsync(m->flag + cap, claimed2, n2, cudaMemcpyHostToDevice, st));
     else SSLPL_CUDA(cudaMemsetAsync(m->flag + cap, 0, n2, st));
-    m->h_small[0] = n2;
-    SSLPL_CUDA(cudaMemcpyAsync(m->ncnt, m->h_small, sizeof(int), cudaMemcpyHostToDevice, st));
-    SSLPL_CUDA(cudaStreamSynchronize(st));                               // fl (pageable) and h_small are reused by the caller / next call
-    int* goff = m->off + (NN + 1); int* gidx = m->idx + cap;
-    k_grid_cells<<<(n2 + 127) / 128, 128, 0, st>>>(k1, k1 + cap, 1, 0, nullptr, n2, n2, A.minX, A.minY, A.invW, A.invH, m->node, 0);
-    SSLPL_REQUIRE((size_t)((nc + 1 + cap) * sizeof(int)) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "nodes + features exceed the shared memory of one CTA ((nc + 1 + cap) * 4 <= 200 KB)");
-    k_build_csr<<<1, 128, (nc + 1 + cap) * sizeof(int), st>>>(m->node, 0, m->ncnt, cap, nc, goff, 0, gidx, 0);
+    SSLPL_CUDA(cudaStreamSynchronize(st));                               // fl (pageable) is reused by the caller
+    int *goff, *gidx;
+    if (int rc = grid_staging_build(m, k1, k1 + cap, n2, A.minX, A.minY, A.invW, A.invH, goff, gidx)) return rc;
     ProjPair P; memset(&P, 0, sizeof(P));
     P.n1 = n1; P.n2 = n2; P.cap = cap;
     P.flag1 = m->flag; P.Xw = k0; P.dmp = m->desc; P.angle1 = k0 + 3 * (size_t)cap; P.oct1 = reinterpret_cast<const int*>(k0 + 4 * (size_t)cap); P.es1 = 1;
@@ -1985,32 +2055,12 @@ int sslpl_search_by_projection_frame(sslpl_matcher* m,
     P.uright2 = k1 + 3 * (size_t)cap; P.es2 = 1;
     P.claimed0 = m->flag + cap; P.goff = goff; P.gidx = gidx;
     P.claimed = m->taken; P.assign2 = m->out; P.sel = m->pairs; P.rbin = m->rot; P.nmatch = m->nmatch;
-    k_proj_match<<<1, 32, 0, st>>>(A, P);
-    m->launches += 3;
+    launch(m, k_proj_match, 1, 32, 0, A, P);
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(assign2, m->out, sizeof(int32_t) * n2, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaMemcpyAsync(m->h_small, m->nmatch, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaStreamSynchronize(st));
     *nmatches = m->h_small[0];
-    return SSLPL_OK;
-}
-
-// The per-frame grid workspace of the batched projection matchers ([max_batch + 1] frames), allocated by the first call that needs it
-// (a handle that never gets there never pays for it) and freed with the handle: per frame the grid cell of every feature and the grid
-// CSR, and the motion-model walker's claimed / sel / rbin tables.
-static int ensure_grid_ws(sslpl_matcher* m) {
-    if (m->pw) return SSLPL_OK;
-    const int B = m->p.max_batch + 1, fc = m->p.max_features + 64, nc = GRID_COLS * GRID_ROWS;
-    Arena W;
-    for (int k = 0; k < 2; k++) {
-        m->pw_cell = W.take<int32_t>((size_t)B * fc); m->pw_off = W.take<int>((size_t)B * (nc + 1)); m->pw_idx = W.take<int>((size_t)B * fc);
-        m->pw_sel = W.take<int32_t>((size_t)B * fc); m->pw_claimed = W.take<uint8_t>((size_t)B * fc); m->pw_rbin = W.take<uint8_t>((size_t)B * fc);
-        if (k == 0) {
-            cudaError_t e = cudaMalloc(&m->pw, W.used);
-            if (e != cudaSuccess) { m->pw = nullptr; set_error("cudaMalloc(%zu) failed: %s", W.used, cudaGetErrorString(e)); return SSLPL_ERR_CUDA; }
-            W.base = m->pw; W.size = W.used; W.used = 0;
-        }
-    }
     return SSLPL_OK;
 }
 
@@ -2029,11 +2079,9 @@ int sslpl_search_by_projection_frame_batch_device(sslpl_matcher* m, const sslpl_
     SSLPL_REQUIRE(th > 0.f, SSLPL_ERR_ARG, "th must be positive");
     SSLPL_REQUIRE(bounds[1] > bounds[0] && bounds[3] > bounds[2], SSLPL_ERR_ARG, "degenerate image bounds");
     const int nc = GRID_COLS * GRID_ROWS, npairs = nframes - 1;
-    SSLPL_REQUIRE((size_t)((nc + 1 + cap) * sizeof(int)) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "grid cells + features exceed the shared memory of one CTA ((3073 + cap) * 4 <= 200 KB)");
+    if (int rc = csr_fits(nc, cap)) return rc;
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     const int fc = m->p.max_features + 64;
-    if (int rc = ensure_grid_ws(m)) return rc;
-    cudaStream_t st = m->stream;
     ProjArgs A; memset(&A, 0, sizeof(A));
     A.fx = cam[0]; A.fy = cam[1]; A.cx = cam[2]; A.cy = cam[3];
     A.minX = bounds[0]; A.maxX = bounds[1]; A.minY = bounds[2]; A.maxY = bounds[3];
@@ -2042,6 +2090,7 @@ int sslpl_search_by_projection_frame_batch_device(sslpl_matcher* m, const sslpl_
     for (int k = 0; k < nlevels; k++) A.scale[k] = scaleFactors[k];
     const float* kf = reinterpret_cast<const float*>(d_kps);            // sslpl_keypoint = 7 x 4 B: x y size angle response octave class_id
     const long long kfs = 7LL * cap;
+    if (int rc = grid_batch_build(m, kf + kfs, d_n + 1, npairs, cap, A.minX, A.minY, A.invW, A.invH)) return rc;
     ProjPair P; memset(&P, 0, sizeof(P));
     P.n = d_n; P.cap = cap; P.Tcw = d_Tcw + 12;
     P.flag1 = d_mpflag; P.Xw = d_Xw; P.dmp = d_dmp ? d_dmp : d_desc; P.angle1 = kf + 3; P.oct1 = reinterpret_cast<const int*>(kf + 5);
@@ -2051,10 +2100,7 @@ int sslpl_search_by_projection_frame_batch_device(sslpl_matcher* m, const sslpl_
     P.goff = m->pw_off; P.gidx = m->pw_idx; P.goff_fs = nc + 1; P.gidx_fs = fc;
     P.claimed = m->pw_claimed; P.assign2 = d_assign; P.sel = m->pw_sel; P.rbin = m->pw_rbin; P.ws_fs = cap;
     P.nmatch = d_nmatch;
-    k_grid_cells<<<dim3((cap + 127) / 128, npairs), 128, 0, st>>>(P.x2, P.y2, 7, kfs, d_n + 1, 0, cap, A.minX, A.minY, A.invW, A.invH, m->pw_cell, fc);
-    k_build_csr<<<npairs, 128, (nc + 1 + cap) * sizeof(int), st>>>(m->pw_cell, fc, d_n + 1, cap, nc, m->pw_off, nc + 1, m->pw_idx, fc);
-    k_proj_match<<<npairs, 32, 0, st>>>(A, P);
-    m->launches += 3;
+    launch(m, k_proj_match, npairs, 32, 0, A, P);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
@@ -2072,8 +2118,8 @@ int sslpl_search_by_projection_mps(sslpl_matcher* m,
         int n2, const uint8_t* d2, const float* x2, const float* y2, const int32_t* oct2, const float* uright2, const uint8_t* held2,
         const float* bounds, const float* scaleFactors, int nlevels, float nnratio, float th, int32_t* assign2, int* nmatches) {
     SSLPL_REQUIRE(m && assign2 && nmatches && bounds && scaleFactors, SSLPL_ERR_ARG, "null argument");
-    SSLPL_REQUIRE(nmp >= 0 && n2 >= 0 && nmp <= m->cap && n2 <= m->cap && m->cap <= 8192 + 64, SSLPL_ERR_ARG, "nmp / n2 exceed the matcher capacity (<= 8192)");
-    SSLPL_REQUIRE(m->p.max_nodes >= GRID_COLS * GRID_ROWS, SSLPL_ERR_ARG, "the matcher needs max_nodes >= 3072 (64 x 48 grid cells)");
+    SSLPL_REQUIRE(nmp >= 0 && n2 >= 0 && nmp <= m->cap && n2 <= m->cap, SSLPL_ERR_ARG, "nmp / n2 exceed the matcher capacity");
+    if (int rc = grid_staging_ok(m)) return rc;
     SSLPL_REQUIRE(nlevels >= 1 && nlevels <= 32, SSLPL_ERR_ARG, "nlevels out of range");
     SSLPL_REQUIRE(nmp == 0 || (inview && projx && projy && level && viewcos && dmp), SSLPL_ERR_ARG, "null MapPoint array");
     SSLPL_REQUIRE(n2 == 0 || (d2 && x2 && y2 && oct2), SSLPL_ERR_ARG, "null frame array");
@@ -2084,7 +2130,7 @@ int sslpl_search_by_projection_mps(sslpl_matcher* m,
     for (int i = 0; i < nmp; i++) SSLPL_REQUIRE(level[i] >= 0 && level[i] < nlevels, SSLPL_ERR_ARG, "predicted level outside the scale-factor table");
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
-    const int cap = m->cap, NN = m->p.max_nodes + 1, nc = GRID_COLS * GRID_ROWS;
+    const int cap = m->cap;
     WinArgs A; fill_win(A, bounds, scaleFactors, nlevels);
     A.th = th; A.nnratio = nnratio; A.bFactor = th != 1.0f; A.use_right = uright2 ? 1 : 0;
     std::vector<uint8_t> fl(nmp), cl(n2, 0);
@@ -2104,17 +2150,12 @@ int sslpl_search_by_projection_mps(sslpl_matcher* m,
     SSLPL_CUDA(cudaMemcpyAsync(k1 + 4 * (size_t)cap, oct2, sizeof(int) * n2, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(m->flag, fl.data(), nmp, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(m->flag + cap, cl.data(), n2, cudaMemcpyHostToDevice, st));
-    m->h_small[0] = n2;
-    SSLPL_CUDA(cudaMemcpyAsync(m->ncnt, m->h_small, sizeof(int), cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaStreamSynchronize(st));                               // pageable staging vectors go out of scope
-    int* goff = m->off + (NN + 1); int* gidx = m->idx + cap;
-    k_grid_cells<<<(n2 + 127) / 128, 128, 0, st>>>(k1, k1 + cap, 1, 0, nullptr, n2, n2, A.minX, A.minY, A.invW, A.invH, m->node, 0);
-    SSLPL_REQUIRE((size_t)((nc + 1 + cap) * sizeof(int)) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "nodes + features exceed the shared memory of one CTA ((nc + 1 + cap) * 4 <= 200 KB)");
-    k_build_csr<<<1, 128, (nc + 1 + cap) * sizeof(int), st>>>(m->node, 0, m->ncnt, cap, nc, goff, 0, gidx, 0);
-    k_proj_match_mps<<<1, 32, 0, st>>>(A, nmp, m->flag, k0, k0 + cap, k0 + 2 * (size_t)cap, reinterpret_cast<const int*>(k0 + 4 * (size_t)cap), k0 + 3 * (size_t)cap, m->desc,
+    int *goff, *gidx;
+    if (int rc = grid_staging_build(m, k1, k1 + cap, n2, A.minX, A.minY, A.invW, A.invH, goff, gidx)) return rc;
+    launch(m, k_proj_match_mps, 1, 32, 0, A, nmp, m->flag, k0, k0 + cap, k0 + 2 * (size_t)cap, reinterpret_cast<const int*>(k0 + 4 * (size_t)cap), k0 + 3 * (size_t)cap, m->desc,
                                        n2, m->desc + (size_t)cap * 32, k1, k1 + cap, reinterpret_cast<const int*>(k1 + 4 * (size_t)cap), k1 + 3 * (size_t)cap,
                                        m->flag + cap, goff, gidx, m->out, m->nmatch);
-    m->launches += 3;
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(assign2, m->out, sizeof(int32_t) * n2, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaMemcpyAsync(m->h_small, m->nmatch, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -2128,8 +2169,8 @@ int sslpl_search_for_initialization(sslpl_matcher* m,
         int n2, const uint8_t* d2, const float* x2, const float* y2, const int32_t* oct2, const float* angle2,
         const float* bounds, float nnratio, int checkOri, int windowSize, int32_t* matches12, int* nmatches) {
     SSLPL_REQUIRE(m && matches12 && nmatches && bounds, SSLPL_ERR_ARG, "null argument");
-    SSLPL_REQUIRE(n1 >= 0 && n2 >= 0 && n1 <= m->cap && n2 <= m->cap && m->cap <= 8192 + 64, SSLPL_ERR_ARG, "n1 / n2 exceed the matcher capacity (<= 8192 features)");
-    SSLPL_REQUIRE(m->p.max_nodes >= GRID_COLS * GRID_ROWS, SSLPL_ERR_ARG, "the matcher needs max_nodes >= 3072 (64 x 48 grid cells)");
+    SSLPL_REQUIRE(n1 >= 0 && n2 >= 0 && n1 <= m->cap && n2 <= m->cap, SSLPL_ERR_ARG, "n1 / n2 exceed the matcher capacity");
+    if (int rc = grid_staging_ok(m)) return rc;
     SSLPL_REQUIRE(n1 == 0 || (d1 && oct1 && angle1 && prev_xy), SSLPL_ERR_ARG, "null first-frame array");
     SSLPL_REQUIRE(n2 == 0 || (d2 && x2 && y2 && oct2 && angle2), SSLPL_ERR_ARG, "null second-frame array");
     for (int i = 0; i < n1; i++) matches12[i] = -1;
@@ -2137,7 +2178,7 @@ int sslpl_search_for_initialization(sslpl_matcher* m,
     if (n1 == 0 || n2 == 0) return SSLPL_OK;
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
-    const int cap = m->cap, NN = m->p.max_nodes + 1, nc = GRID_COLS * GRID_ROWS;
+    const int cap = m->cap;
     WinArgs A; fill_win(A, bounds, nullptr, 0);
     A.nnratio = nnratio; A.checkOri = checkOri ? 1 : 0; A.window = windowSize;
     std::vector<float> px(n1), py(n1);
@@ -2153,17 +2194,12 @@ int sslpl_search_for_initialization(sslpl_matcher* m,
     SSLPL_CUDA(cudaMemcpyAsync(k1 + (size_t)cap, y2, sizeof(float) * n2, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(k1 + 2 * (size_t)cap, angle2, sizeof(float) * n2, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(k1 + 4 * (size_t)cap, oct2, sizeof(int) * n2, cudaMemcpyHostToDevice, st));
-    m->h_small[0] = n2;
-    SSLPL_CUDA(cudaMemcpyAsync(m->ncnt, m->h_small, sizeof(int), cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaStreamSynchronize(st));
-    int* goff = m->off + (NN + 1); int* gidx = m->idx + cap;
-    k_grid_cells<<<(n2 + 127) / 128, 128, 0, st>>>(k1, k1 + cap, 1, 0, nullptr, n2, n2, A.minX, A.minY, A.invW, A.invH, m->node, 0);
-    SSLPL_REQUIRE((size_t)((nc + 1 + cap) * sizeof(int)) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "nodes + features exceed the shared memory of one CTA ((nc + 1 + cap) * 4 <= 200 KB)");
-    k_build_csr<<<1, 128, (nc + 1 + cap) * sizeof(int), st>>>(m->node, 0, m->ncnt, cap, nc, goff, 0, gidx, 0);
-    k_init_match<<<1, 32, 0, st>>>(A, n1, m->desc, reinterpret_cast<const int*>(k0 + 4 * (size_t)cap), k0 + 3 * (size_t)cap, k0, k0 + cap,
+    int *goff, *gidx;
+    if (int rc = grid_staging_build(m, k1, k1 + cap, n2, A.minX, A.minY, A.invW, A.invH, goff, gidx)) return rc;
+    launch(m, k_init_match, 1, 32, 0, A, n1, m->desc, reinterpret_cast<const int*>(k0 + 4 * (size_t)cap), k0 + 3 * (size_t)cap, k0, k0 + cap,
                                    n2, m->desc + (size_t)cap * 32, k1, k1 + cap, reinterpret_cast<const int*>(k1 + 4 * (size_t)cap), k1 + 2 * (size_t)cap,
                                    goff, gidx, m->knn, m->knn + cap, m->out, m->rot, m->nmatch);
-    m->launches += 3;
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(matches12, m->out, sizeof(int32_t) * n1, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaMemcpyAsync(px.data(), k0, sizeof(float) * n1, cudaMemcpyDeviceToHost, st));
@@ -2215,9 +2251,8 @@ int sslpl_line_search_by_projection(sslpl_matcher* m, int nml, const uint8_t* ac
     uint8_t* d_cl = stage(A, cl.data(), nl2, st, e); int32_t* d_out = A.take<int32_t>(nl2 + 8);
     SSLPL_CUDA(e);
     SSLPL_CUDA(cudaStreamSynchronize(st));                               // the pageable staging vectors go out of scope
-    k_line_window_search<<<1, 32, 0, st>>>(nml, d_fl, reinterpret_cast<const float4*>(d_proj), d_rad, d_min, d_max, d_dml, nl2, d_ld2, d_kl2, d_oct, d_cl,
+    launch(m, k_line_window_search, 1, 32, 0, nml, d_fl, reinterpret_cast<const float4*>(d_proj), d_rad, d_min, d_max, d_dml, nl2, d_ld2, d_kl2, d_oct, d_cl,
                                            nnratio, d_out, m->nmatch);
-    m->launches++;
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(assign2, d_out, sizeof(int32_t) * nl2, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaMemcpyAsync(m->h_small, m->nmatch, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -2249,8 +2284,8 @@ int sslpl_fuse_lines_search(sslpl_matcher* m, int nml, const uint8_t* active, co
     SSLPL_CUDA(e);
     SSLPL_CUDA(cudaStreamSynchronize(st));
     FuseMap Z; memset(&Z, 0, sizeof(Z));
-    k_line_fuse_search<false><<<(nml + 3) / 4, 128, 0, st>>>(nml, d_act, reinterpret_cast<const float4*>(d_proj), d_lvl, d_dml, nl2, d_ld2, d_kl2, d_oct, d_sc, th, d_bi, d_bd, Z);
-    m->launches++;
+    launch(m, k_line_fuse_search<false>, (nml + 3) / 4, 128, 0, nml, d_act, reinterpret_cast<const float4*>(d_proj), d_lvl, d_dml, nl2, d_ld2, d_kl2,
+           d_oct, d_sc, th, d_bi, d_bd, Z);
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(best_idx, d_bi, sizeof(int32_t) * nml, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaMemcpyAsync(best_dist, d_bd, sizeof(int32_t) * nml, cudaMemcpyDeviceToHost, st));
@@ -2263,8 +2298,8 @@ int sslpl_fuse_points_search(sslpl_matcher* m, int nmp, const uint8_t* active, c
                              const float* bounds, const float* scaleFactors, const float* invLevelSigma2, int nlevels, float th,
                              int32_t* best_idx, int32_t* best_dist) {
     SSLPL_REQUIRE(m && nmp >= 0 && n2 >= 0 && bounds && scaleFactors && invLevelSigma2 && nlevels >= 1 && nlevels <= 32, SSLPL_ERR_ARG, "bad argument");
-    SSLPL_REQUIRE(n2 <= m->cap && m->cap <= 8192 + 64, SSLPL_ERR_ARG, "n2 exceeds the matcher capacity (<= 8192 features)");
-    SSLPL_REQUIRE(m->p.max_nodes >= GRID_COLS * GRID_ROWS, SSLPL_ERR_ARG, "the matcher needs max_nodes >= 3072 (64 x 48 grid cells)");
+    SSLPL_REQUIRE(n2 <= m->cap, SSLPL_ERR_ARG, "n2 exceeds the matcher capacity");
+    if (int rc = grid_staging_ok(m)) return rc;
     SSLPL_REQUIRE(nmp == 0 || (active && u && v && level && dmp && best_idx && best_dist), SSLPL_ERR_ARG, "null MapPoint array");
     SSLPL_REQUIRE(n2 == 0 || (d2 && x2 && y2 && oct2), SSLPL_ERR_ARG, "null KeyFrame array");
     for (int i = 0; i < nmp; i++) { best_idx[i] = -1; best_dist[i] = 256; }
@@ -2272,7 +2307,6 @@ int sslpl_fuse_points_search(sslpl_matcher* m, int nmp, const uint8_t* active, c
     for (int i = 0; i < nmp; i++) SSLPL_REQUIRE(!active[i] || (level[i] >= 0 && level[i] < nlevels), SSLPL_ERR_ARG, "predicted level outside the pyramid");
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
-    const int cap = m->cap, NN = m->p.max_nodes + 1, nc = GRID_COLS * GRID_ROWS;
     WinArgs A; fill_win(A, bounds, scaleFactors, nlevels);
     A.th = th; A.use_right = uright2 ? 1 : 0;
     const size_t need = (size_t)nmp * (1 + 12 + 4 + 32 + 8) + (size_t)n2 * (32 + 16) + 32 * 4 + 16 * 256 + 4096;
@@ -2286,17 +2320,13 @@ int sslpl_fuse_points_search(sslpl_matcher* m, int nmp, const uint8_t* active, c
     uint8_t* d_d2 = stage(S, d2, (size_t)32 * n2, st, e); float* d_x2 = stage(S, x2, n2, st, e); float* d_y2 = stage(S, y2, n2, st, e);
     int32_t* d_oct = stage(S, oct2, n2, st, e); float* d_ur2 = stage(S, uright2, uright2 ? n2 : 0, st, e); float* d_is2 = stage(S, invLevelSigma2, nlevels, st, e);
     int32_t* d_bi = S.take<int32_t>(nmp + 8); int32_t* d_bd = S.take<int32_t>(nmp + 8);
-    m->h_small[0] = n2;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(m->ncnt, m->h_small, sizeof(int), cudaMemcpyHostToDevice, st);
     SSLPL_CUDA(e);
     SSLPL_CUDA(cudaStreamSynchronize(st));
-    int* goff = m->off + (NN + 1); int* gidx = m->idx + cap;
-    k_grid_cells<<<(n2 + 127) / 128, 128, 0, st>>>(d_x2, d_y2, 1, 0, nullptr, n2, n2, A.minX, A.minY, A.invW, A.invH, m->node, 0);
-    SSLPL_REQUIRE((size_t)((nc + 1 + cap) * sizeof(int)) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "nodes + features exceed the shared memory of one CTA ((nc + 1 + cap) * 4 <= 200 KB)");
-    k_build_csr<<<1, 128, (nc + 1 + cap) * sizeof(int), st>>>(m->node, 0, m->ncnt, cap, nc, goff, 0, gidx, 0);
+    int *goff, *gidx;
+    if (int rc = grid_staging_build(m, d_x2, d_y2, n2, A.minX, A.minY, A.invW, A.invH, goff, gidx)) return rc;
     FuseMap Z; memset(&Z, 0, sizeof(Z));
-    k_point_fuse_search<false><<<(nmp + 3) / 4, 128, 0, st>>>(A, nmp, d_act, d_u, d_v, d_ur, d_lvl, d_dmp, d_d2, d_x2, d_y2, d_oct, d_ur2, d_is2, goff, gidx, d_bi, d_bd, Z);
-    m->launches += 3;
+    launch(m, k_point_fuse_search<false>, (nmp + 3) / 4, 128, 0, A, nmp, d_act, d_u, d_v, d_ur, d_lvl, d_dmp, d_d2, d_x2, d_y2, d_oct, d_ur2, d_is2,
+           goff, gidx, d_bi, d_bd, Z);
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(best_idx, d_bi, sizeof(int32_t) * nmp, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaMemcpyAsync(best_dist, d_bd, sizeof(int32_t) * nmp, cudaMemcpyDeviceToHost, st));
@@ -2320,8 +2350,7 @@ int sslpl_descriptor_medoid_batch(sslpl_matcher* m, const uint8_t* desc, const i
     int32_t* d_bi = A.take<int32_t>(ngroups); int32_t* d_bm = A.take<int32_t>(ngroups);
     if (total) SSLPL_CUDA(cudaMemcpyAsync(d_desc, desc, (size_t)total * 32, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(d_off, off, sizeof(int32_t) * (ngroups + 1), cudaMemcpyHostToDevice, st));
-    k_medoid<<<ngroups, 128, 0, st>>>(d_desc, d_off, d_bi, d_bm);
-    m->launches++;
+    launch(m, k_medoid, ngroups, 128, 0, d_desc, d_off, d_bi, d_bm);
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(best_idx, d_bi, sizeof(int32_t) * ngroups, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaMemcpyAsync(best_median, d_bm, sizeof(int32_t) * ngroups, cudaMemcpyDeviceToHost, st));
@@ -2443,8 +2472,8 @@ int sslpl_bow_transform(sslpl_matcher* m, const sslpl_vocab* v, const uint8_t* d
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
     SSLPL_CUDA(cudaMemcpyAsync(m->desc, desc, (size_t)n * 32, cudaMemcpyHostToDevice, st));
-    k_vocab_transform<<<dim3((n + 127) / 128, 1), 128, 0, st>>>(m->desc, 0, nullptr, n, n, v->view, v->L - levelsup, m->word, m->node, nullptr, m->wgt, 0);
-    m->launches++;
+    launch(m, k_vocab_transform, dim3((n + 127) / 128, 1), 128, 0, m->desc, 0, nullptr, n, n, v->view, v->L - levelsup, m->word, m->node, nullptr,
+           m->wgt, 0);
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(word, m->word, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaMemcpyAsync(node, m->node, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
@@ -2461,17 +2490,14 @@ int sslpl_match_bow_batch_device_vocab(sslpl_matcher* m, const uint8_t* d_desc, 
     const int nc = vocab_level_nodes(v, levelsup);
     SSLPL_REQUIRE(cap >= 1 && cap <= m->p.max_features + 64 && nc <= m->p.max_nodes, SSLPL_ERR_ARG, "cap or the vocabulary level exceeds the matcher capacity (max_nodes)");
     SSLPL_REQUIRE(v->device == m->p.device, SSLPL_ERR_ARG, "vocabulary and matcher live on different devices");
+    if (int rc = csr_fits(nc, cap)) return rc;
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     const int fc = m->p.max_features + 64;
+    const dim3 grid((cap + 127) / 128, nframes);
     // optional per-feature outputs use the caller's [nframes][cap] layout; the dense node index goes to the workspace ([..][fc])
-    if (d_word || d_node || d_weight) {
-        k_vocab_transform<<<dim3((cap + 127) / 128, nframes), 128, 0, m->stream>>>(d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup,
-                                                                                      d_word, d_node, nullptr, d_weight, cap);
-        m->launches += 1;
-    }
-    k_vocab_transform<<<dim3((cap + 127) / 128, nframes), 128, 0, m->stream>>>(d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup,
-                                                                                  nullptr, nullptr, m->b_node, nullptr, fc);
-    m->launches += 1;
+    if (d_word || d_node || d_weight)
+        launch(m, k_vocab_transform, grid, 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup, d_word, d_node, nullptr, d_weight, cap);
+    launch(m, k_vocab_transform, grid, 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup, nullptr, nullptr, m->b_node, nullptr, fc);
     return bow_batch_tail(m, d_desc, d_kps, d_n, nframes, cap, nc, nnratio, checkOri, d_match, d_nmatch);
 }
 
@@ -2482,13 +2508,11 @@ int sslpl_match_lines_batch_device(sslpl_matcher* m, const uint8_t* d_ldesc, con
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
     const int npairs = nframes - 1, lc = m->p.max_lines + 64;
-    k_knn2<false><<<dim3((capl + 7) / 8, npairs), 256, 0, st>>>(d_ldesc, (long long)capl * 32, d_nl, 0, d_ldesc + (size_t)capl * 32, (long long)capl * 32,
-                                                          d_nl, 0, m->b_knn, (long long)lc * 4, capl, nullptr, 0);
-    m->launches++;
+    launch(m, k_knn2<false>, dim3((capl + 7) / 8, npairs), 256, 0, d_ldesc, (long long)capl * 32, d_nl, 0, d_ldesc + (size_t)capl * 32, (long long)capl * 32,
+           d_nl, 0, m->b_knn, (long long)lc * 4, capl, nullptr, 0);
     fill(m, d_lmatch, (long long)npairs * capl, -1);
     SSLPL_CUDA(cudaMemsetAsync(d_nlmatch, 0, sizeof(int32_t) * npairs, st));
-    k_line_ratio<<<dim3((capl + 127) / 128, npairs), 128, 0, st>>>(m->b_knn, (long long)lc * 4, d_nl, 0, capl, nullptr, 0, d_lmatch, capl, d_nlmatch);
-    m->launches++;
+    launch(m, k_line_ratio, dim3((capl + 127) / 128, npairs), 128, 0, m->b_knn, (long long)lc * 4, d_nl, 0, capl, nullptr, 0, d_lmatch, capl, d_nlmatch);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
@@ -2501,42 +2525,26 @@ static int tri_match_stage(sslpl_matcher* m,
         const sslpl_vocab* v, int levelsup, int npairs, const int32_t* d_pair, const float* d_geom,
         const float* scale, const float* sigma2, int nlevels) {
     SSLPL_REQUIRE(d_kps && d_desc && d_n && d_has_mp && v && d_pair && d_geom && scale && sigma2, SSLPL_ERR_ARG, "null argument");
-    SSLPL_REQUIRE(nkf >= 1 && nkf <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nkf outside [1, max_batch + 1]");
-    SSLPL_REQUIRE(npairs >= 1 && npairs <= m->p.max_batch, SSLPL_ERR_ARG, "npairs outside [1, max_batch]");
-    SSLPL_REQUIRE(cap >= 1 && cap <= m->p.max_features + 64, SSLPL_ERR_ARG, "cap outside [1, max_features + 64]");
+    if (int rc = kf_pairs_ok(m, nkf, cap, m->p.max_features, npairs)) return rc;
     SSLPL_REQUIRE(nlevels >= 1 && nlevels <= SSLPL_MAX_LEVELS, SSLPL_ERR_ARG, "nlevels out of range");
     const int nc = vocab_level_nodes(v, levelsup);
     SSLPL_REQUIRE(nc <= m->p.max_nodes, SSLPL_ERR_ARG, "the vocabulary level exceeds the matcher capacity (max_nodes)");
     SSLPL_REQUIRE(v->device == m->p.device, SSLPL_ERR_ARG, "vocabulary and matcher live on different devices");
-    SSLPL_REQUIRE((size_t)((nc + 1 + cap) * sizeof(int)) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "nodes + features exceed the shared memory of one CTA ((nc + 1 + cap) * 4 <= 200 KB)");
+    if (int rc = csr_fits(nc, cap)) return rc;
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     const int fc = m->p.max_features + 64, NN = m->p.max_nodes + 1;
-    if (!m->tw) {                                                        // first call: a handle that never gets here never pays for it
-        const size_t bytes = sizeof(int32_t) * (size_t)m->p.max_batch * fc;
-        cudaError_t e = cudaMalloc(&m->tw, bytes);
-        if (e != cudaSuccess) { m->tw = nullptr; set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return SSLPL_ERR_CUDA; }
-    }
-    cudaStream_t st = m->stream;
-    const int2* pmap = reinterpret_cast<const int2*>(d_pair);
-    k_vocab_transform<<<dim3((cap + 127) / 128, nkf), 128, 0, st>>>(d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup,
-                                                                     nullptr, nullptr, m->b_node, nullptr, fc);
-    k_build_csr<<<nkf, 128, (nc + 1 + cap) * sizeof(int), st>>>(m->b_node, fc, d_n, cap, nc, m->b_off, NN + 1, m->b_idx, fc);
-    m->launches += 2;
+    if (int rc = first_use(m->tw, sizeof(int32_t) * (size_t)m->p.max_batch * fc)) return rc;
+    launch(m, k_vocab_transform, dim3((cap + 127) / 128, nkf), 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup,
+           nullptr, nullptr, m->b_node, nullptr, fc);
+    launch(m, k_build_csr, nkf, 128, (nc + 1 + cap) * sizeof(int), m->b_node, fc, d_n, cap, nc, m->b_off, NN + 1, m->b_idx, fc);
     fill(m, m->tw, (long long)npairs * cap, -1);
-    FrameSet S; memset(&S, 0, sizeof(S));
-    S.desc = d_desc; S.desc_fs = (long long)cap * 32;
-    S.nodes = m->iota; S.nodes_fs = 0; S.nn = nullptr; S.nn_const = nc;            // dense node ranks: every keyframe lists 0..nc-1
-    S.off = m->b_off; S.idx = m->b_idx; S.off_fs = NN + 1; S.idx_fs = fc;
-    S.flag = d_has_mp; S.flag_fs = cap;
-    const float* kf = reinterpret_cast<const float*>(d_kps);
-    S.angle = kf + 3; S.x = kf; S.y = kf + 1; S.oct = reinterpret_cast<const int*>(kf + 5); S.angle_es = 7; S.angle_fs = (long long)cap * 7;
-    S.pmap = pmap; S.nframes = nkf;
+    FrameSet S = dense_set(m, d_desc, d_kps, cap, nc, d_has_mp);
+    S.pmap = reinterpret_cast<const int2*>(d_pair); S.nframes = nkf;
     TriArgs T; memset(&T, 0, sizeof(T));
     T.nlevels = nlevels;
     for (int i = 0; i < nlevels; i++) { T.scale[i] = scale[i]; T.sigma2[i] = sigma2[i]; }
     // b_rot is only read where the table holds a match, and k_tri_match writes both together
-    k_tri_match<true><<<dim3((nc + 3) / 4, npairs), 128, 0, st>>>(S, T, d_geom, m->tw, cap, m->b_rot, fc);
-    m->launches++;
+    launch(m, k_tri_match<true>, dim3((nc + 3) / 4, npairs), 128, 0, S, T, d_geom, m->tw, cap, m->b_rot, fc);
     return SSLPL_OK;
 }
 
@@ -2546,12 +2554,10 @@ int sslpl_search_for_triangulation_batch_device(sslpl_matcher* m,
         const float* scale, const float* sigma2, int nlevels, int checkOrientation, int32_t* d_pairs, int32_t* d_nmatch) {
     SSLPL_REQUIRE(m && d_pairs && d_nmatch, SSLPL_ERR_ARG, "null argument");
     if (int rc = tri_match_stage(m, d_kps, d_desc, d_n, nkf, cap, d_has_mp, v, levelsup, npairs, d_pair, d_geom, scale, sigma2, nlevels)) return rc;
-    cudaStream_t st = m->stream;
     const int fc = m->p.max_features + 64;
     fill(m, d_pairs, 2LL * npairs * cap, -1);
-    k_rot_filter<<<npairs, 256, 0, st>>>(m->tw, cap, m->b_rot, fc, nullptr, 0, cap, cap, checkOrientation, d_nmatch, d_pairs, 2LL * cap);
-    k_bad_pairs<<<(npairs + 127) / 128, 128, 0, st>>>(reinterpret_cast<const int2*>(d_pair), npairs, nkf, d_nmatch);
-    m->launches += 2;
+    launch(m, k_rot_filter, npairs, 256, 0, m->tw, cap, m->b_rot, fc, nullptr, 0, cap, cap, checkOrientation, d_nmatch, d_pairs, 2LL * cap);
+    launch(m, k_bad_pairs, (npairs + 127) / 128, 128, 0, reinterpret_cast<const int2*>(d_pair), npairs, nkf, d_nmatch);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
@@ -2561,17 +2567,13 @@ int sslpl_search_for_triangulation_batch_device(sslpl_matcher* m,
 int sslpl_line_search_for_triangulation_batch_device(sslpl_matcher* m, const uint8_t* d_ldesc, const int* d_nl, int nkf, int capl,
         const uint8_t* d_has_ml, int npairs, const int32_t* d_pair, int32_t* d_lpairs, int32_t* d_nlmatch) {
     SSLPL_REQUIRE(m && d_ldesc && d_nl && d_has_ml && d_pair && d_lpairs && d_nlmatch, SSLPL_ERR_ARG, "null argument");
-    SSLPL_REQUIRE(nkf >= 1 && nkf <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nkf outside [1, max_batch + 1]");
-    SSLPL_REQUIRE(npairs >= 1 && npairs <= m->p.max_batch, SSLPL_ERR_ARG, "npairs outside [1, max_batch]");
-    SSLPL_REQUIRE(capl >= 1 && capl <= m->p.max_lines + 64, SSLPL_ERR_ARG, "capl outside [1, max_lines + 64]");
+    if (int rc = kf_pairs_ok(m, nkf, capl, m->p.max_lines, npairs)) return rc;
     SSLPL_CUDA(cudaSetDevice(m->p.device));
-    cudaStream_t st = m->stream;
     const int lc = m->p.max_lines + 64;
     const int2* pmap = reinterpret_cast<const int2*>(d_pair);
-    k_knn2<true><<<dim3((capl + 7) / 8, npairs), 256, 0, st>>>(d_ldesc, (long long)capl * 32, d_nl, 0, d_ldesc, (long long)capl * 32, d_nl, 0,
-                                                          m->b_knn, (long long)lc * 4, capl, pmap, nkf);
-    k_line_tri<<<npairs, 256, 0, st>>>(m->b_knn, (long long)lc * 4, d_nl, capl, pmap, nkf, d_has_ml, d_lpairs, d_nlmatch);
-    m->launches += 2;
+    launch(m, k_knn2<true>, dim3((capl + 7) / 8, npairs), 256, 0, d_ldesc, (long long)capl * 32, d_nl, 0, d_ldesc, (long long)capl * 32, d_nl, 0,
+           m->b_knn, (long long)lc * 4, capl, pmap, nkf);
+    launch(m, k_line_tri, npairs, 256, 0, m->b_knn, (long long)lc * 4, d_nl, capl, pmap, nkf, d_has_ml, d_lpairs, d_nlmatch);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
@@ -2592,10 +2594,8 @@ int sslpl_create_new_map_points_batch_device(sslpl_matcher* m,
     C.nlevels = nlevels;
     for (int i = 0; i < nlevels; i++) { C.scale[i] = scaleFactors[i]; C.sigma2[i] = levelSigma2[i]; }
     const size_t smem = sizeof(unsigned) * (size_t)((cap + 31) / 32);
-    k_create_points_chain<<<npairs, 256, smem, m->stream>>>(reinterpret_cast<const int2*>(d_pair), npairs, nkf, m->tw, cap,
-                                                            reinterpret_cast<const float*>(d_kps), d_n, d_has_mp, d_kfpose, C,
-                                                            d_pairs, d_nmatch, d_status, d_x3d, d_nnew);
-    m->launches++;
+    launch(m, k_create_points_chain, npairs, 256, smem, reinterpret_cast<const int2*>(d_pair), npairs, nkf, m->tw, cap,
+           reinterpret_cast<const float*>(d_kps), d_n, d_has_mp, d_kfpose, C, d_pairs, d_nmatch, d_status, d_x3d, d_nnew);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
@@ -2608,27 +2608,19 @@ int sslpl_create_new_map_lines_batch_device(sslpl_matcher* m,
         int32_t* d_lpairs, int32_t* d_nlmatch, int32_t* d_status, float* d_line3d, int32_t* d_nnew) {
     SSLPL_REQUIRE(m && d_kl && d_ldesc && d_lineeq && d_nl && d_has_ml && d_pair && d_kfpose && d_kfdepth && cam && d_lpairs && d_nlmatch &&
                   d_status && d_line3d && d_nnew, SSLPL_ERR_ARG, "null argument");
-    SSLPL_REQUIRE(nkf >= 1 && nkf <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nkf outside [1, max_batch + 1]");
-    SSLPL_REQUIRE(npairs >= 1 && npairs <= m->p.max_batch, SSLPL_ERR_ARG, "npairs outside [1, max_batch]");
-    SSLPL_REQUIRE(capl >= 1 && capl <= m->p.max_lines + 64, SSLPL_ERR_ARG, "capl outside [1, max_lines + 64]");
+    if (int rc = kf_pairs_ok(m, nkf, capl, m->p.max_lines, npairs)) return rc;
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     const int lc = m->p.max_lines + 64;
-    if (!m->ltw) {                                                       // first call: a handle that never gets here never pays for it
-        const size_t bytes = sizeof(int32_t) * (size_t)m->p.max_batch * lc;
-        cudaError_t e = cudaMalloc(&m->ltw, bytes);
-        if (e != cudaSuccess) { m->ltw = nullptr; set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return SSLPL_ERR_CUDA; }
-    }
+    if (int rc = first_use(m->ltw, sizeof(int32_t) * (size_t)m->p.max_batch * lc)) return rc;
     LineCam C;
     C.fx = cam[0]; C.fy = cam[1]; C.cx = cam[2]; C.cy = cam[3]; C.invfx = cam[4]; C.invfy = cam[5];
-    cudaStream_t st = m->stream;
     const int2* pmap = reinterpret_cast<const int2*>(d_pair);
-    k_knn2<true><<<dim3((capl + 7) / 8, npairs), 256, 0, st>>>(d_ldesc, (long long)capl * 32, d_nl, 0, d_ldesc, (long long)capl * 32, d_nl, 0,
-                                                          m->b_knn, (long long)lc * 4, capl, pmap, nkf);
-    k_line_tri_table<<<npairs, 256, 0, st>>>(m->b_knn, (long long)lc * 4, d_nl, capl, pmap, nkf, d_has_ml, m->ltw);
+    launch(m, k_knn2<true>, dim3((capl + 7) / 8, npairs), 256, 0, d_ldesc, (long long)capl * 32, d_nl, 0, d_ldesc, (long long)capl * 32, d_nl, 0,
+           m->b_knn, (long long)lc * 4, capl, pmap, nkf);
+    launch(m, k_line_tri_table, npairs, 256, 0, m->b_knn, (long long)lc * 4, d_nl, capl, pmap, nkf, d_has_ml, m->ltw);
     const size_t smem = sizeof(unsigned) * (size_t)((capl + 31) / 32);
-    k_create_lines_chain<<<npairs, 256, smem, st>>>(pmap, npairs, nkf, m->ltw, capl, reinterpret_cast<const float*>(d_kl), d_lineeq, d_nl,
-                                                    d_has_ml, d_kfpose, d_kfdepth, C, d_lpairs, d_nlmatch, d_status, d_line3d, d_nnew);
-    m->launches += 3;
+    launch(m, k_create_lines_chain, npairs, 256, smem, pmap, npairs, nkf, m->ltw, capl, reinterpret_cast<const float*>(d_kl), d_lineeq, d_nl,
+           d_has_ml, d_kfpose, d_kfdepth, C, d_lpairs, d_nlmatch, d_status, d_line3d, d_nnew);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
@@ -2645,8 +2637,7 @@ int sslpl_matcher_debug_svd4(sslpl_matcher* m, int n, const float* A, float* W, 
     const float* d_A = stage(Ar, A, (size_t)16 * n, st, e); float* d_W = Ar.take<float>((size_t)4 * n + 8); float* d_V = Ar.take<float>((size_t)16 * n + 8);
     const double* d_hx = stage(Ar, hx, nh, st, e); const double* d_hy = stage(Ar, hy, nh, st, e); double* d_h = Ar.take<double>((size_t)nh + 8);
     SSLPL_CUDA(e);
-    k_debug_svd4<<<(nt + 127) / 128, 128, 0, st>>>(n, d_A, d_W, d_V, nh, d_hx, d_hy, d_h);
-    m->launches++;
+    launch(m, k_debug_svd4, (nt + 127) / 128, 128, 0, n, d_A, d_W, d_V, nh, d_hx, d_hy, d_h);
     SSLPL_CUDA(cudaGetLastError());
     if (n) {
         SSLPL_CUDA(cudaMemcpyAsync(W, d_W, sizeof(float) * 4 * (size_t)n, cudaMemcpyDeviceToHost, st));
@@ -2695,19 +2686,18 @@ int sslpl_matcher_debug_predict_scale(sslpl_matcher* m, int n, const float* rati
     cudaError_t e = cudaSuccess;
     float* d_r = stage(A, ratio, n, st, e); int32_t* d_l = A.take<int32_t>(n + 8);
     SSLPL_CUDA(e);
-    k_predict_scale<<<(n + 255) / 256, 256, 0, st>>>(n, d_r, T, clamp, d_l);
-    m->launches++;
+    launch(m, k_predict_scale, (n + 255) / 256, 256, 0, n, d_r, T, clamp, d_l);
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(level, d_l, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaStreamSynchronize(st));
     return SSLPL_OK;
 }
 
-static int fuse_map_common(FuseMap& M, sslpl_matcher* m, int nkf, int nel, int nentries, const int32_t* d_entry, const uint8_t* d_skip,
-                           const float* d_kfpose, const float* d_el, const uint8_t* d_eldesc, const float* cam, const float* bounds,
-                           const float* scaleFactors, int nlevels, float logScaleFactor) {
+static int fuse_map_common(FuseMap& M, sslpl_matcher* m, int nkf, int cap, int rows, int nel, int nentries, const int32_t* d_entry,
+                           const uint8_t* d_skip, const float* d_kfpose, const float* d_el, const uint8_t* d_eldesc, const float* cam,
+                           const float* bounds, const float* scaleFactors, int nlevels, float logScaleFactor) {
     SSLPL_REQUIRE(d_entry && d_kfpose && d_el && d_eldesc && cam && bounds && scaleFactors, SSLPL_ERR_ARG, "null argument");
-    SSLPL_REQUIRE(nkf >= 1 && nkf <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nkf outside [1, max_batch + 1]");
+    if (int rc = kf_set_ok(m, nkf, cap, rows)) return rc;
     SSLPL_REQUIRE(nel >= 0 && nentries >= 0, SSLPL_ERR_ARG, "negative count");
     SSLPL_REQUIRE(nlevels >= 1 && nlevels <= SSLPL_MAX_LEVELS, SSLPL_ERR_ARG, "nlevels outside [1, SSLPL_MAX_LEVELS]");
     SSLPL_REQUIRE(bounds[1] > bounds[0] && bounds[3] > bounds[2], SSLPL_ERR_ARG, "degenerate image bounds");
@@ -2729,27 +2719,23 @@ int sslpl_fuse_points_batch_device(sslpl_matcher* m,
         const float* cam, const float* bounds, const float* scaleFactors, const float* invLevelSigma2, int nlevels, float logScaleFactor, float th,
         int32_t* d_best_idx, int32_t* d_best_dist) {
     SSLPL_REQUIRE(m && d_kps && d_desc && d_n && invLevelSigma2 && d_best_idx && d_best_dist, SSLPL_ERR_ARG, "null argument");
-    SSLPL_REQUIRE(cap >= 1 && cap <= m->p.max_features + 64, SSLPL_ERR_ARG, "cap outside [1, max_features + 64]");
-    const int nc = GRID_COLS * GRID_ROWS;
-    SSLPL_REQUIRE((size_t)((nc + 1 + cap) * sizeof(int)) <= (size_t)MAX_DYN_SMEM, SSLPL_ERR_CAPACITY, "grid cells + features exceed the shared memory of one CTA ((3073 + cap) * 4 <= 200 KB)");
     FuseMap M;
-    if (int rc = fuse_map_common(M, m, nkf, nmp, nentries, d_entry, d_skip, d_kfpose, d_mp, d_mpdesc, cam, bounds, scaleFactors, nlevels, logScaleFactor)) return rc;
+    if (int rc = fuse_map_common(M, m, nkf, cap, m->p.max_features, nmp, nentries, d_entry, d_skip, d_kfpose, d_mp, d_mpdesc, cam, bounds,
+                                 scaleFactors, nlevels, logScaleFactor)) return rc;
+    const int nc = GRID_COLS * GRID_ROWS;
+    if (int rc = csr_fits(nc, cap)) return rc;
     if (nentries == 0) return SSLPL_OK;
     SSLPL_CUDA(cudaSetDevice(m->p.device));
-    if (int rc = ensure_grid_ws(m)) return rc;
     const int fc = m->p.max_features + 64;
     for (int k = 0; k < nlevels; k++) M.invSigma2[k] = invLevelSigma2[k];
     const float* kf = reinterpret_cast<const float*>(d_kps);              // sslpl_keypoint = 7 x 4 B: x y size angle response octave class_id
     M.kp = kf; M.kp_fs = 7LL * cap; M.desc = d_desc; M.desc_fs = 32LL * cap; M.n = d_n; M.cap = cap;
-    M.goff = m->pw_off; M.gidx = m->pw_idx; M.goff_fs = nc + 1; M.gidx_fs = fc;
     WinArgs A; fill_win(A, bounds, scaleFactors, nlevels);
     A.th = th;
-    cudaStream_t st = m->stream;
-    k_grid_cells<<<dim3((cap + 127) / 128, nkf), 128, 0, st>>>(kf, kf + 1, 7, M.kp_fs, d_n, 0, cap, A.minX, A.minY, A.invW, A.invH, m->pw_cell, fc);
-    k_build_csr<<<nkf, 128, (nc + 1 + cap) * sizeof(int), st>>>(m->pw_cell, fc, d_n, cap, nc, m->pw_off, nc + 1, m->pw_idx, fc);
-    k_point_fuse_search<true><<<(nentries + 3) / 4, 128, 0, st>>>(A, nentries, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                                                  nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, d_best_idx, d_best_dist, M);
-    m->launches += 3;
+    if (int rc = grid_batch_build(m, kf, d_n, nkf, cap, A.minX, A.minY, A.invW, A.invH)) return rc;
+    M.goff = m->pw_off; M.gidx = m->pw_idx; M.goff_fs = nc + 1; M.gidx_fs = fc;
+    launch(m, k_point_fuse_search<true>, (nentries + 3) / 4, 128, 0, A, nentries, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+           nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, d_best_idx, d_best_dist, M);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
@@ -2762,15 +2748,14 @@ int sslpl_fuse_lines_batch_device(sslpl_matcher* m,
         const float* cam, const float* bounds, const float* scaleFactors, int nlevels, float logScaleFactor, float th,
         int32_t* d_best_idx, int32_t* d_best_dist) {
     SSLPL_REQUIRE(m && d_kl && d_ldesc && d_nl && d_best_idx && d_best_dist, SSLPL_ERR_ARG, "null argument");
-    SSLPL_REQUIRE(capl >= 1 && capl <= m->p.max_lines + 64, SSLPL_ERR_ARG, "capl outside [1, max_lines + 64]");
     FuseMap M;
-    if (int rc = fuse_map_common(M, m, nkf, nml, nentries, d_entry, d_skip, d_kfpose, d_ml, d_mldesc, cam, bounds, scaleFactors, nlevels, logScaleFactor)) return rc;
+    if (int rc = fuse_map_common(M, m, nkf, capl, m->p.max_lines, nml, nentries, d_entry, d_skip, d_kfpose, d_ml, d_mldesc, cam, bounds,
+                                 scaleFactors, nlevels, logScaleFactor)) return rc;
     if (nentries == 0) return SSLPL_OK;
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     M.kp = reinterpret_cast<const float*>(d_kl); M.kp_fs = 17LL * capl; M.desc = d_ldesc; M.desc_fs = 32LL * capl; M.n = d_nl; M.cap = capl;
-    k_line_fuse_search<true><<<(nentries + 3) / 4, 128, 0, m->stream>>>(nentries, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, th,
-                                                                        d_best_idx, d_best_dist, M);
-    m->launches++;
+    launch(m, k_line_fuse_search<true>, (nentries + 3) / 4, 128, 0, nentries, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr,
+           nullptr, th, d_best_idx, d_best_dist, M);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
