@@ -16,6 +16,7 @@ present, construction raises.  (The package directory name contains '-', so impo
 """
 import ctypes as C
 import os
+import re
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -56,26 +57,48 @@ class FeatVec(C.Structure):
     _fields_ = [("nodes", C.c_void_p), ("off", C.c_void_p), ("idx", C.c_void_p), ("nn", C.c_int)]
 
 
+_SCALARS = {"int": C.c_int, "float": C.c_float, "double": C.c_double, "size_t": C.c_size_t, "long long": C.c_longlong}
+
+
+def _prototypes(text):
+    """{name: (restype, argtypes)} of every sslpl_* function declared in `text`, the source of include/sslpl.h.  Every pointer is a
+    c_void_p, except that a const char* return comes back as bytes.  A scalar type outside _SCALARS raises, so no argument of a new
+    type reaches C without a conversion."""
+    def ctype(decl, name, named):
+        if "*" in decl:
+            return C.c_void_p
+        words = [w for w in decl.split() if w != "const"]
+        t = " ".join(words[:-1] if named else words)
+        if t not in _SCALARS:
+            raise SslplError(f"include/sslpl.h: {name} uses {t!r}, which has no ctypes type here")
+        return _SCALARS[t]
+
+    protos = {}
+    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
+    for ret, name, params in re.findall(r"^\s*([A-Za-z_][\w ]*\**)\s*(sslpl_\w+)\s*\(([^)]*)\)\s*;", text, flags=re.M):
+        ret = " ".join(ret.split())
+        restype = None if ret == "void" else C.c_char_p if ret == "const char*" else ctype(ret, name, False)
+        argtypes = [] if params.strip() == "void" else [ctype(p, name, True) for p in params.split(",")]
+        protos[name] = (restype, argtypes)
+    return protos
+
+
 _lib = None
 
 
 def lib():
-    """Load libsslpl_b200.so (fails loudly when it has not been built: run __graft_entry__.build())."""
+    """Load libsslpl_b200.so with the prototypes of include/sslpl.h on every function (fails loudly when it has not been built: run
+    __graft_entry__.build())."""
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise SslplError(f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'`"
                              " (there is no CPU fallback)")
         L = C.CDLL(LIB_PATH)
-        L.sslpl_last_error.restype = C.c_char_p
-        L.sslpl_orb_stream.restype = C.c_void_p
-        L.sslpl_orb_launch_count.restype = C.c_longlong
-        for name in ("sslpl_matcher_stream", "sslpl_line_stream"):
-            if hasattr(L, name):
-                getattr(L, name).restype = C.c_void_p
-        for name in ("sslpl_matcher_launch_count", "sslpl_line_launch_count"):
-            if hasattr(L, name):
-                getattr(L, name).restype = C.c_longlong
+        with open(os.path.join(_HERE, "..", "include", "sslpl.h")) as f:
+            for name, (restype, argtypes) in _prototypes(f.read()).items():
+                fn = getattr(L, name)
+                fn.restype, fn.argtypes = restype, argtypes
         _lib = L
     return _lib
 
@@ -86,15 +109,80 @@ def _check(rc):
 
 
 def _p(a):
-    if a is None:
-        return None
-    if isinstance(a, int):
-        return C.c_void_p(a)
-    return a.ctypes.data_as(C.c_void_p)
+    """An ndarray as a pointer argument (a c_void_p argtype rejects the array itself); the result keeps the array alive through the
+    call.  None stays NULL."""
+    return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _u8(a):
+    return None if a is None else np.ascontiguousarray(a, np.uint8)
+
+
+def _i32(a):
+    return None if a is None else np.ascontiguousarray(a, np.int32)
+
+
+def _f32(a):
+    return None if a is None else np.ascontiguousarray(a, np.float32)
+
+
+def _f64(a):
+    return None if a is None else np.ascontiguousarray(a, np.float64)
+
+
+class _Handle:
+    """A handle of include/sslpl.h.  A subclass names its kind, the <kind> of the sslpl_<kind>_* functions, and takes the lifecycle
+    methods the header declares for that kind: class Matcher(_Handle, kind="matcher", lifecycle=("sync", ...)).  A borrowed handle
+    belongs to another one (Frame's extractors): same methods, never destroyed from here."""
+    _h = None
+    _borrowed = False
+
+    def __init_subclass__(cls, kind, lifecycle=()):
+        cls._kind = kind
+        for name in lifecycle:
+            setattr(cls, name, getattr(_Handle, "_" + name))
+
+    def _fn(self, name):
+        return getattr(lib(), f"sslpl_{self._kind}_{name}")
+
+    def _create(self, params):
+        self._h = C.c_void_p()
+        _check(self._fn("create")(C.byref(params), C.byref(self._h)))
+
+    @classmethod
+    def _borrow(cls, ptr, **attrs):
+        self = cls.__new__(cls)
+        self.__dict__.update(attrs, _h=C.c_void_p(ptr), _borrowed=True)
+        return self
+
+    def close(self):
+        if self._h is not None and self._h.value and not self._borrowed:
+            self._fn("destroy")(self._h)
+            self._h = C.c_void_p()
+
+    __del__ = close
+
+    # the lifecycle methods, public under their names without the underscore in the classes that take them
+    def _sync(self):
+        _check(self._fn("sync")(self._h))
+
+    def _set_stream(self, cuda_stream):
+        _check(self._fn("set_stream")(self._h, cuda_stream))
+
+    _stream = property(lambda self: self._fn("stream")(self._h))
+    _launch_count = property(lambda self: self._fn("launch_count")(self._h))
+
+    def _set_profiling(self, on=True):
+        _check(self._fn("set_profiling")(self._h, int(on)))
+
+    def _stage_ms(self):
+        ms = (C.c_float * 16)(); names = (C.c_char_p * 16)(); n = C.c_int()
+        _check(self._fn("stage_ms")(self._h, ms, 16, names, C.byref(n)))
+        return {names[i].decode(): float(ms[i]) for i in range(n.value)}
 
 
 def device_count():
-    return int(lib().sslpl_device_count())
+    return lib().sslpl_device_count()
 
 
 def host_alloc(shape, dtype=np.uint8):
@@ -102,39 +190,21 @@ def host_alloc(shape, dtype=np.uint8):
     dtype = np.dtype(dtype)
     nbytes = int(np.prod(shape)) * dtype.itemsize
     ptr = C.c_void_p()
-    _check(lib().sslpl_host_alloc(C.byref(ptr), C.c_size_t(max(nbytes, 1))))
+    _check(lib().sslpl_host_alloc(C.byref(ptr), max(nbytes, 1)))
     buf = (C.c_uint8 * max(nbytes, 1)).from_address(ptr.value)
     arr = np.frombuffer(buf, dtype=dtype, count=int(np.prod(shape))).reshape(shape)
     return arr
 
 
-class ORBextractor:
+class ORBextractor(_Handle, kind="orb", lifecycle=("sync", "set_stream", "stream", "launch_count", "set_profiling", "stage_ms")):
     """Mirror of StructureSLAM::ORBextractor (include/ORBextractor.h:45-111)."""
 
     def __init__(self, nfeatures=1000, scaleFactor=1.2, nlevels=8, iniThFAST=20, minThFAST=7,
                  max_width=1280, max_height=960, max_batch=1, device=0):
         self.nfeatures, self.scaleFactor, self.nlevels = nfeatures, scaleFactor, nlevels
-        p = OrbParams(nfeatures, scaleFactor, nlevels, iniThFAST, minThFAST, max_width, max_height, max_batch, device)
-        self._h = C.c_void_p()
-        _check(lib().sslpl_orb_create(C.byref(p), C.byref(self._h)))
+        self._create(OrbParams(nfeatures, scaleFactor, nlevels, iniThFAST, minThFAST, max_width, max_height, max_batch, device))
         self.max_batch = max_batch
-        self.cap = int(lib().sslpl_orb_max_keypoints(self._h))
-
-    @classmethod
-    def _borrow(cls, ptr, nfeatures, scaleFactor, nlevels, max_batch):
-        """A view of an extractor owned by somebody else (Frame): same methods, never destroyed from here."""
-        self = cls.__new__(cls)
-        self.nfeatures, self.scaleFactor, self.nlevels, self.max_batch = nfeatures, scaleFactor, nlevels, max_batch
-        self._h = C.c_void_p(ptr); self._borrowed = True
-        self.cap = int(lib().sslpl_orb_max_keypoints(self._h))
-        return self
-
-    def close(self):
-        if getattr(self, "_h", None) is not None and self._h.value and not getattr(self, "_borrowed", False):
-            lib().sslpl_orb_destroy(self._h)
-            self._h = C.c_void_p()
-
-    __del__ = close
+        self.cap = lib().sslpl_orb_max_keypoints(self._h)
 
     # ORBextractor.h:60-77
     def GetLevels(self):
@@ -182,7 +252,7 @@ class ORBextractor:
         if out is None:
             out = (np.zeros((B, self.cap), KEYPOINT_DTYPE), np.zeros((B, self.cap, 32), np.uint8), np.zeros(B, np.int32))
         kps, desc, n = out
-        _check(lib().sslpl_orb_extract_batch(self._h, _p(frames), B, W, H, frames.strides[1], C.c_size_t(frames.strides[0]),
+        _check(lib().sslpl_orb_extract_batch(self._h, _p(frames), B, W, H, frames.strides[1], frames.strides[0],
                                              _p(kps), _p(desc), self.cap, _p(n)))
         return kps, desc, n
 
@@ -190,32 +260,17 @@ class ORBextractor:
         """Asynchronous host-buffer form: returns immediately; `out` (pinned) is valid after sync()."""
         B, H, W = frames.shape
         kps, desc, n = out
-        _check(lib().sslpl_orb_extract_batch_begin(self._h, _p(frames), B, W, H, frames.strides[1], C.c_size_t(frames.strides[0]),
+        _check(lib().sslpl_orb_extract_batch_begin(self._h, _p(frames), B, W, H, frames.strides[1], frames.strides[0],
                                                    _p(kps), _p(desc), self.cap, _p(n)))
 
     def extract_batch_device(self, d_ptr, nframes, width, height, pitch, frame_stride):
         """Frames already in HBM (raw device pointer, e.g. torch_tensor.data_ptr()); asynchronous."""
-        _check(lib().sslpl_orb_extract_batch_device(self._h, C.c_void_p(d_ptr), nframes, width, height, pitch,
-                                                    C.c_size_t(frame_stride)))
+        _check(lib().sslpl_orb_extract_batch_device(self._h, d_ptr, nframes, width, height, pitch, frame_stride))
 
     def device_results(self):
         kps = C.c_void_p(); desc = C.c_void_p(); n = C.c_void_p(); cap = C.c_int()
         _check(lib().sslpl_orb_device_results(self._h, C.byref(kps), C.byref(desc), C.byref(n), C.byref(cap)))
         return kps.value, desc.value, n.value, cap.value
-
-    def sync(self):
-        _check(lib().sslpl_orb_sync(self._h))
-
-    def set_stream(self, cuda_stream):
-        _check(lib().sslpl_orb_set_stream(self._h, C.c_void_p(cuda_stream)))
-
-    @property
-    def stream(self):
-        return lib().sslpl_orb_stream(self._h)
-
-    @property
-    def launch_count(self):
-        return int(lib().sslpl_orb_launch_count(self._h))
 
     # ---- stage intermediates (parity tests) ----
     def level_size(self, l):
@@ -248,21 +303,13 @@ class ORBextractor:
         _check(lib().sslpl_orb_download_level_keypoints(self._h, frame, l, _p(xs), _p(ys), _p(rs), cap, C.byref(n)))
         return xs[:n.value].copy(), ys[:n.value].copy(), rs[:n.value].copy()
 
-    def set_profiling(self, on=True):
-        _check(lib().sslpl_orb_set_profiling(self._h, int(on)))
-
-    def stage_ms(self):
-        ms = (C.c_float * 16)(); names = (C.c_char_p * 16)(); n = C.c_int()
-        _check(lib().sslpl_orb_stage_ms(self._h, ms, 16, names, C.byref(n)))
-        return {names[i].decode(): float(ms[i]) for i in range(n.value)}
-
 
 # =====================================================================================================
 # Matching
 # =====================================================================================================
 def _featvec(fv):
     """(nodes, off, idx) int32 arrays -> FeatVec struct (keeps references alive)."""
-    nodes, off, idx = (np.ascontiguousarray(a, np.int32) for a in fv)
+    nodes, off, idx = (_i32(a) for a in fv)
     s = FeatVec(_p(nodes) if len(nodes) else None, _p(off), _p(idx) if len(idx) else None, len(nodes))
     s._keep = (nodes, off, idx)
     return s
@@ -278,92 +325,63 @@ def feature_vector_csr(node):
     return ids.astype(np.int32), off, order
 
 
-class Matcher:
+class Matcher(_Handle, kind="matcher", lifecycle=("sync", "set_stream", "stream", "launch_count")):
     """Device context shared by ORBmatcher / LSDmatcher below (one stream + workspace; create one per thread)."""
 
     def __init__(self, max_features=4096, max_lines=512, max_nodes=1024, max_batch=1, device=0):
-        p = MatcherParams(max_features, max_lines, max_nodes, max_batch, device)
-        self._h = C.c_void_p()
-        _check(lib().sslpl_matcher_create(C.byref(p), C.byref(self._h)))
+        self._create(MatcherParams(max_features, max_lines, max_nodes, max_batch, device))
         self.max_features, self.max_lines = max_features, max_lines
 
-    def close(self):
-        if getattr(self, "_h", None) is not None and self._h.value:
-            lib().sslpl_matcher_destroy(self._h)
-            self._h = C.c_void_p()
-
-    __del__ = close
-
-    def sync(self):
-        _check(lib().sslpl_matcher_sync(self._h))
-
-    def set_stream(self, cuda_stream):
-        _check(lib().sslpl_matcher_set_stream(self._h, C.c_void_p(cuda_stream)))
-
-    @property
-    def stream(self):
-        return lib().sslpl_matcher_stream(self._h)
-
-    @property
-    def launch_count(self):
-        return int(lib().sslpl_matcher_launch_count(self._h))
-
     def descriptor_distance(self, a, b):
-        a = np.ascontiguousarray(a, np.uint8).reshape(-1, 32); b = np.ascontiguousarray(b, np.uint8).reshape(-1, 32)
+        a = _u8(a).reshape(-1, 32); b = _u8(b).reshape(-1, 32)
         out = np.empty(len(a), np.int32)
         _check(lib().sslpl_descriptor_distance(self._h, _p(a), _p(b), len(a), _p(out)))
         return out
 
     def knn2(self, q, t):
         """cv::BFMatcher(NORM_HAMMING).knnMatch(q, t, k=2) -> int32 [nq,4] = idx0, d0, idx1, d1."""
-        q = np.ascontiguousarray(q, np.uint8).reshape(-1, 32); t = np.ascontiguousarray(t, np.uint8).reshape(-1, 32)
+        q = _u8(q).reshape(-1, 32); t = _u8(t).reshape(-1, 32)
         out = np.empty((len(q), 4), np.int32)
         _check(lib().sslpl_hamming_knn2(self._h, _p(q), len(q), _p(t), len(t), _p(out)))
         return out
 
     def bow_assign(self, desc, centroids):
-        desc = np.ascontiguousarray(desc, np.uint8).reshape(-1, 32); centroids = np.ascontiguousarray(centroids, np.uint8).reshape(-1, 32)
+        desc = _u8(desc).reshape(-1, 32); centroids = _u8(centroids).reshape(-1, 32)
         node = np.empty(len(desc), np.int32)
         _check(lib().sslpl_bow_assign(self._h, _p(desc), len(desc), _p(centroids), len(centroids), _p(node)))
         return node
 
     def match_bow_batch_device(self, d_desc, d_kps, d_n, nframes, cap, d_centroids, nc, nnratio, check_ori, d_match, d_nmatch):
-        _check(lib().sslpl_match_bow_batch_device(self._h, C.c_void_p(d_desc), C.c_void_p(d_kps), C.c_void_p(d_n), nframes, cap,
-                                                  C.c_void_p(d_centroids), nc, C.c_float(nnratio), int(check_ori),
-                                                  C.c_void_p(d_match), C.c_void_p(d_nmatch)))
+        _check(lib().sslpl_match_bow_batch_device(self._h, d_desc, d_kps, d_n, nframes, cap, d_centroids, nc, nnratio, int(check_ori),
+                                                  d_match, d_nmatch))
 
     def match_bow_batch_device_vocab(self, d_desc, d_kps, d_n, nframes, cap, vocab, levelsup, nnratio, check_ori, d_match, d_nmatch,
                                      d_word=0, d_node=0, d_weight=0):
         """Batched SearchByBoW with the DBoW2 tree transform (optional per-feature word / node / weight outputs in HBM)."""
-        _check(lib().sslpl_match_bow_batch_device_vocab(self._h, C.c_void_p(d_desc), C.c_void_p(d_kps), C.c_void_p(d_n), nframes, cap,
-                                                        vocab._h, int(levelsup), C.c_float(nnratio), int(check_ori),
-                                                        C.c_void_p(d_match), C.c_void_p(d_nmatch),
-                                                        C.c_void_p(d_word or None), C.c_void_p(d_node or None), C.c_void_p(d_weight or None)))
+        _check(lib().sslpl_match_bow_batch_device_vocab(self._h, d_desc, d_kps, d_n, nframes, cap, vocab._h, levelsup, nnratio,
+                                                        int(check_ori), d_match, d_nmatch, d_word or None, d_node or None, d_weight or None))
 
     def bow_transform(self, vocab, desc, levelsup=4):
         """TemplatedVocabulary::transform per feature (TemplatedVocabulary.h:1218-1259): (word, node, weight) arrays."""
-        desc = np.ascontiguousarray(desc, np.uint8).reshape(-1, 32)
+        desc = _u8(desc).reshape(-1, 32)
         n = len(desc)
         word = np.empty(max(n, 1), np.int32); node = np.empty(max(n, 1), np.int32); w = np.empty(max(n, 1), np.float64)
-        _check(lib().sslpl_bow_transform(self._h, vocab._h, _p(desc), n, int(levelsup), _p(word), _p(node), _p(w)))
+        _check(lib().sslpl_bow_transform(self._h, vocab._h, _p(desc), n, levelsup, _p(word), _p(node), _p(w)))
         return word[:n], node[:n], w[:n]
 
     def search_by_projection_mps(self, mp, cur, bounds, scale_factors, nnratio=0.8, th=1.0):
         """ORBmatcher::SearchByProjection(Frame&, const vector<MapPoint*>&, th) (ORBmatcher.cc:45-129).
         mp = dict(inview, bad, obs, projx, projy, level, viewcos, desc[, projxr]); cur = dict(desc, x, y, oct[, uright, held])."""
-        f32 = lambda a: np.ascontiguousarray(a, np.float32); u8 = lambda a: np.ascontiguousarray(a, np.uint8)
         nmp = len(mp["inview"]); n2 = len(cur["x"])
-        iv, bad, obs = u8(mp["inview"]), u8(mp["bad"]), u8(mp["obs"])
-        px, py = f32(mp["projx"]), f32(mp["projy"]); pxr = f32(mp["projxr"]) if mp.get("projxr") is not None else None
-        lv = np.ascontiguousarray(mp["level"], np.int32); vc = f32(mp["viewcos"]); dmp = u8(mp["desc"]).reshape(-1, 32)
-        d2 = u8(cur["desc"]).reshape(-1, 32); x2, y2 = f32(cur["x"]), f32(cur["y"]); oc2 = np.ascontiguousarray(cur["oct"], np.int32)
-        ur = f32(cur["uright"]) if cur.get("uright") is not None else None
-        held = u8(cur["held"]) if cur.get("held") is not None else None
-        sf = f32(scale_factors); out = np.full(max(n2, 1), -1, np.int32); nm = C.c_int()
-        _check(lib().sslpl_search_by_projection_mps(self._h, nmp, _p(iv), _p(bad), _p(obs), _p(px), _p(py), _p(pxr) if pxr is not None else None,
-                                                    _p(lv), _p(vc), _p(dmp), n2, _p(d2), _p(x2), _p(y2), _p(oc2), _p(ur) if ur is not None else None,
-                                                    _p(held) if held is not None else None, _p(f32(bounds)), _p(sf), len(sf),
-                                                    C.c_float(nnratio), C.c_float(th), _p(out), C.byref(nm)))
+        iv, bad, obs = _u8(mp["inview"]), _u8(mp["bad"]), _u8(mp["obs"])
+        px, py, pxr = _f32(mp["projx"]), _f32(mp["projy"]), _f32(mp.get("projxr"))
+        lv = _i32(mp["level"]); vc = _f32(mp["viewcos"]); dmp = _u8(mp["desc"]).reshape(-1, 32)
+        d2 = _u8(cur["desc"]).reshape(-1, 32); x2, y2 = _f32(cur["x"]), _f32(cur["y"]); oc2 = _i32(cur["oct"])
+        ur, held = _f32(cur.get("uright")), _u8(cur.get("held"))
+        sf = _f32(scale_factors); out = np.full(max(n2, 1), -1, np.int32); nm = C.c_int()
+        _check(lib().sslpl_search_by_projection_mps(self._h, nmp, _p(iv), _p(bad), _p(obs), _p(px), _p(py), _p(pxr), _p(lv), _p(vc), _p(dmp),
+                                                    n2, _p(d2), _p(x2), _p(y2), _p(oc2), _p(ur), _p(held), _p(_f32(bounds)), _p(sf), len(sf),
+                                                    nnratio, th, _p(out), C.byref(nm)))
         return nm.value, out[:n2]
 
     def line_search_by_projection(self, q, obs, dml, ld2, kl2, oct2, held2=None, nnratio=0.8):
@@ -371,43 +389,38 @@ class Matcher:
         LSDmatcher::SearchByProjection(Frame&, const vector<MapLine*>&, th) (:210-251).  q = dict(active, proj[n,4], radius, min_level,
         max_level) per MapLine (the projection stage's outputs), obs = Observations() > 0, dml their descriptors; ld2 / kl2[n,3] (pt.x,
         pt.y, angle) / oct2 / held2 the frame's lines -> (nmatches, assign2)."""
-        f32 = lambda a: np.ascontiguousarray(a, np.float32); u8 = lambda a: np.ascontiguousarray(a, np.uint8); i32 = lambda a: np.ascontiguousarray(a, np.int32)
         nml = len(q["active"]); nl2 = len(oct2)
         out = np.full(max(nl2, 1), -1, np.int32); nm = C.c_int()
-        _check(lib().sslpl_line_search_by_projection(self._h, nml, _p(u8(q["active"])), _p(u8(obs)), _p(f32(q["proj"])), _p(f32(q["radius"])),
-                                                     _p(i32(q["min_level"])), _p(i32(q["max_level"])), _p(u8(dml)), nl2, _p(u8(ld2)), _p(f32(kl2)), _p(i32(oct2)),
-                                                     _p(u8(held2)) if held2 is not None else None, C.c_float(nnratio), _p(out), C.byref(nm)))
+        _check(lib().sslpl_line_search_by_projection(self._h, nml, _p(_u8(q["active"])), _p(_u8(obs)), _p(_f32(q["proj"])), _p(_f32(q["radius"])),
+                                                     _p(_i32(q["min_level"])), _p(_i32(q["max_level"])), _p(_u8(dml)), nl2, _p(_u8(ld2)), _p(_f32(kl2)), _p(_i32(oct2)),
+                                                     _p(_u8(held2)), nnratio, _p(out), C.byref(nm)))
         return nm.value, out[:nl2]
 
     def fuse_lines_search(self, q, dml, ld2, kl2, oct2, scale_factors, th=3.0):
         """Search stage of LSDmatcher::Fuse (LSDmatcher.cpp:495-523).  q = dict(active, proj[n,4], level) -> (best_idx, best_dist)."""
-        f32 = lambda a: np.ascontiguousarray(a, np.float32); u8 = lambda a: np.ascontiguousarray(a, np.uint8); i32 = lambda a: np.ascontiguousarray(a, np.int32)
-        n = len(q["active"]); sf = f32(scale_factors)
+        n = len(q["active"]); sf = _f32(scale_factors)
         bi = np.full(max(n, 1), -1, np.int32); bd = np.full(max(n, 1), 0x7fffffff, np.int32)
-        _check(lib().sslpl_fuse_lines_search(self._h, n, _p(u8(q["active"])), _p(f32(q["proj"])), _p(i32(q["level"])), _p(u8(dml)), len(oct2), _p(u8(ld2)),
-                                             _p(f32(kl2)), _p(i32(oct2)), _p(sf), len(sf), C.c_float(th), _p(bi), _p(bd)))
+        _check(lib().sslpl_fuse_lines_search(self._h, n, _p(_u8(q["active"])), _p(_f32(q["proj"])), _p(_i32(q["level"])), _p(_u8(dml)), len(oct2), _p(_u8(ld2)),
+                                             _p(_f32(kl2)), _p(_i32(oct2)), _p(sf), len(sf), th, _p(bi), _p(bd)))
         return bi[:n], bd[:n]
 
     def fuse_points_search(self, q, dmp, d2, x2, y2, oct2, uright2, bounds, scale_factors, inv_level_sigma2, th=3.0):
         """Search stage of ORBmatcher::Fuse (ORBmatcher.cc:889-950).  q = dict(active, u, v, ur, level) -> (best_idx, best_dist)."""
-        f32 = lambda a: np.ascontiguousarray(a, np.float32); u8 = lambda a: np.ascontiguousarray(a, np.uint8); i32 = lambda a: np.ascontiguousarray(a, np.int32)
-        n = len(q["active"]); sf = f32(scale_factors)
+        n = len(q["active"]); sf = _f32(scale_factors)
         bi = np.full(max(n, 1), -1, np.int32); bd = np.full(max(n, 1), 256, np.int32)
-        ur2 = f32(uright2) if uright2 is not None else None
-        _check(lib().sslpl_fuse_points_search(self._h, n, _p(u8(q["active"])), _p(f32(q["u"])), _p(f32(q["v"])), _p(f32(q["ur"])), _p(i32(q["level"])), _p(u8(dmp)),
-                                              len(x2), _p(u8(d2)), _p(f32(x2)), _p(f32(y2)), _p(i32(oct2)), _p(ur2) if ur2 is not None else None,
-                                              _p(f32(bounds)), _p(sf), _p(f32(inv_level_sigma2)), len(sf), C.c_float(th), _p(bi), _p(bd)))
+        _check(lib().sslpl_fuse_points_search(self._h, n, _p(_u8(q["active"])), _p(_f32(q["u"])), _p(_f32(q["v"])), _p(_f32(q["ur"])), _p(_i32(q["level"])), _p(_u8(dmp)),
+                                              len(x2), _p(_u8(d2)), _p(_f32(x2)), _p(_f32(y2)), _p(_i32(oct2)), _p(_f32(uright2)),
+                                              _p(_f32(bounds)), _p(sf), _p(_f32(inv_level_sigma2)), len(sf), th, _p(bi), _p(bd)))
         return bi[:n], bd[:n]
 
     def search_for_initialization(self, d1, k1, d2, k2, prev, bounds, nnratio=0.9, check_ori=True, window=100):
         """ORBmatcher::SearchForInitialization (ORBmatcher.cc:408-523) -> (nmatches, matches12, prev_out)."""
-        f32 = lambda a: np.ascontiguousarray(a, np.float32)
-        d1 = np.ascontiguousarray(d1, np.uint8).reshape(-1, 32); d2 = np.ascontiguousarray(d2, np.uint8).reshape(-1, 32)
-        prev = f32(prev).reshape(-1, 2).copy()
+        d1 = _u8(d1).reshape(-1, 32); d2 = _u8(d2).reshape(-1, 32)
+        prev = _f32(prev).reshape(-1, 2).copy()
         m12 = np.full(max(len(k1), 1), -1, np.int32); nm = C.c_int()
-        _check(lib().sslpl_search_for_initialization(self._h, len(k1), _p(d1), _p(np.ascontiguousarray(k1["octave"], np.int32)), _p(f32(k1["angle"])), _p(prev),
-                                                     len(k2), _p(d2), _p(f32(k2["x"])), _p(f32(k2["y"])), _p(np.ascontiguousarray(k2["octave"], np.int32)),
-                                                     _p(f32(k2["angle"])), _p(f32(bounds)), C.c_float(nnratio), int(check_ori), int(window), _p(m12), C.byref(nm)))
+        _check(lib().sslpl_search_for_initialization(self._h, len(k1), _p(d1), _p(_i32(k1["octave"])), _p(_f32(k1["angle"])), _p(prev),
+                                                     len(k2), _p(d2), _p(_f32(k2["x"])), _p(_f32(k2["y"])), _p(_i32(k2["octave"])),
+                                                     _p(_f32(k2["angle"])), _p(_f32(bounds)), nnratio, int(check_ori), window, _p(m12), C.byref(nm)))
         return nm.value, m12[:len(k1)], prev
 
     def search_by_projection_frame(self, last, cur, Tcw, Tlw, cam, bounds, scale_factors, th, mono=True, check_ori=True, raw=False):
@@ -415,21 +428,19 @@ class Matcher:
         last = dict(valid, obs, Xw[n,3], dmp[n,32], oct, angle); cur = dict(desc[n,32], x, y, oct, angle, uright|None, claimed|None);
         Tcw / Tlw 3x4 (or 4x4) row-major; cam = (fx, fy, cx, cy, mbf, mb); bounds = (minX, maxX, minY, maxY).
         Returns (nmatches, assign2) with assign2[j] = index of the last-frame MapPoint given to current feature j or -1."""
-        f32 = lambda a: np.ascontiguousarray(a, np.float32)
         n1, n2 = len(last["valid"]), len(cur["x"])
-        v1 = np.ascontiguousarray(last["valid"], np.uint8); o1 = np.ascontiguousarray(last["obs"], np.uint8)
-        Xw = f32(last["Xw"]).reshape(-1, 3); dmp = np.ascontiguousarray(last["dmp"], np.uint8).reshape(-1, 32)
-        oc1 = np.ascontiguousarray(last["oct"], np.int32); a1 = f32(last["angle"])
-        d2 = np.ascontiguousarray(cur["desc"], np.uint8).reshape(-1, 32); x2 = f32(cur["x"]); y2 = f32(cur["y"])
-        oc2 = np.ascontiguousarray(cur["oct"], np.int32); a2 = f32(cur["angle"])
-        ur = f32(cur["uright"]) if cur.get("uright") is not None else None
-        cl = np.ascontiguousarray(cur["claimed"], np.uint8) if cur.get("claimed") is not None else None
-        Tc = f32(Tcw).reshape(-1)[:12].copy(); Tl = f32(Tlw).reshape(-1)[:12].copy() if Tlw is not None else None
-        camv = f32(cam); bnd = f32(bounds); sf = f32(scale_factors)
+        v1 = _u8(last["valid"]); o1 = _u8(last["obs"])
+        Xw = _f32(last["Xw"]).reshape(-1, 3); dmp = _u8(last["dmp"]).reshape(-1, 32)
+        oc1 = _i32(last["oct"]); a1 = _f32(last["angle"])
+        d2 = _u8(cur["desc"]).reshape(-1, 32); x2 = _f32(cur["x"]); y2 = _f32(cur["y"])
+        oc2 = _i32(cur["oct"]); a2 = _f32(cur["angle"])
+        ur, cl = _f32(cur.get("uright")), _u8(cur.get("claimed"))
+        Tc = _f32(Tcw).reshape(-1)[:12].copy(); Tl = _f32(Tlw).reshape(-1)[:12].copy() if Tlw is not None else None
+        camv = _f32(cam); bnd = _f32(bounds); sf = _f32(scale_factors)
         out = np.full(max(n2, 1), -1, np.int32); nm = C.c_int()
         _check(lib().sslpl_search_by_projection_frame(self._h, n1, _p(v1), _p(o1), _p(Xw), _p(dmp), _p(oc1), _p(a1),
                                                       n2, _p(d2), _p(x2), _p(y2), _p(oc2), _p(a2), _p(ur), _p(cl), _p(Tc), _p(Tl),
-                                                      _p(camv), _p(bnd), _p(sf), len(sf), C.c_float(th), int(mono), int(check_ori),
+                                                      _p(camv), _p(bnd), _p(sf), len(sf), th, int(mono), int(check_ori),
                                                       _p(out), C.byref(nm)))
         # -2 = assigned, then removed by the rotation check (the reference writes NULL there, ORBmatcher.cc:1461); -1 = never assigned
         return nm.value, (out[:n2] if raw else np.where(out[:n2] == -2, -1, out[:n2]).astype(np.int32))
@@ -442,24 +453,21 @@ class Matcher:
         MapPoint and not outlier, bit1 Observations() > 0), d_dmp [nframes, cap, 32] or 0 (= d_desc), d_Tcw [nframes, 12] f32 ->
         d_assign [nframes - 1, cap] i32 (-1 never assigned, -2 removed by the rotation check), d_nmatch [nframes - 1] i32.
         Asynchronous on the matcher's stream."""
-        f32 = lambda a: np.ascontiguousarray(a, np.float32)
-        sf = f32(scale_factors)
+        sf = _f32(scale_factors)
         _check(lib().sslpl_search_by_projection_frame_batch_device(
-            self._h, C.c_void_p(d_kps), C.c_void_p(d_desc), C.c_void_p(d_n), int(nframes), int(cap), C.c_void_p(d_Xw), C.c_void_p(d_mpflag),
-            C.c_void_p(d_dmp or None), C.c_void_p(d_Tcw), _p(f32(cam)[:4].copy()), _p(f32(bounds)), _p(sf), len(sf), C.c_float(th),
-            int(check_ori), int(retry_below), C.c_void_p(d_assign), C.c_void_p(d_nmatch)))
+            self._h, d_kps, d_desc, d_n, nframes, cap, d_Xw, d_mpflag, d_dmp or None, d_Tcw, _p(_f32(cam)[:4].copy()), _p(_f32(bounds)),
+            _p(sf), len(sf), th, int(check_ori), retry_below, d_assign, d_nmatch))
 
     def descriptor_medoid(self, desc, off):
         """ComputeDistinctiveDescriptors (MapPoint.cc:247-312 / MapLine.cpp:246-317) for CSR groups of descriptors."""
-        desc = np.ascontiguousarray(desc, np.uint8).reshape(-1, 32); off = np.ascontiguousarray(off, np.int32)
+        desc = _u8(desc).reshape(-1, 32); off = _i32(off)
         ng = len(off) - 1
         bi = np.empty(max(ng, 1), np.int32); bm = np.empty(max(ng, 1), np.int32)
         _check(lib().sslpl_descriptor_medoid_batch(self._h, _p(desc), _p(off), ng, _p(bi), _p(bm)))
         return bi[:ng], bm[:ng]
 
     def match_lines_batch_device(self, d_ldesc, d_nl, nframes, capl, d_lmatch, d_nlmatch):
-        _check(lib().sslpl_match_lines_batch_device(self._h, C.c_void_p(d_ldesc), C.c_void_p(d_nl), nframes, capl,
-                                                    C.c_void_p(d_lmatch), C.c_void_p(d_nlmatch)))
+        _check(lib().sslpl_match_lines_batch_device(self._h, d_ldesc, d_nl, nframes, capl, d_lmatch, d_nlmatch))
 
     def search_for_triangulation_batch_device(self, d_kps, d_desc, d_n, nkf, cap, d_has_mp, vocab, levelsup, npairs, d_pair, d_geom,
                                               scale, sigma2, check_ori, d_pairs, d_nmatch):
@@ -468,21 +476,19 @@ class Matcher:
         i32 (kf1, kf2), d_geom [npairs, 11] f32 (F12 row-major, ex, ey); scale / sigma2 host arrays (nlevels = len(scale)) ->
         d_pairs [npairs, cap, 2] i32 ((idx1, idx2) ascending idx1, -1 after the count), d_nmatch [npairs] i32 (-1: pair index out of
         range).  Asynchronous on the matcher's stream."""
-        sc = np.ascontiguousarray(scale, np.float32); s2 = np.ascontiguousarray(sigma2, np.float32)
+        sc = _f32(scale); s2 = _f32(sigma2)
         assert len(s2) >= len(sc)
         _check(lib().sslpl_search_for_triangulation_batch_device(
-            self._h, C.c_void_p(d_kps), C.c_void_p(d_desc), C.c_void_p(d_n), int(nkf), int(cap), C.c_void_p(d_has_mp), vocab._h,
-            int(levelsup), int(npairs), C.c_void_p(d_pair), C.c_void_p(d_geom), _p(sc), _p(s2), len(sc), int(check_ori),
-            C.c_void_p(d_pairs), C.c_void_p(d_nmatch)))
+            self._h, d_kps, d_desc, d_n, nkf, cap, d_has_mp, vocab._h, levelsup, npairs, d_pair, d_geom, _p(sc), _p(s2), len(sc),
+            int(check_ori), d_pairs, d_nmatch))
 
     def line_search_for_triangulation_batch_device(self, d_ldesc, d_nl, nkf, capl, d_has_ml, npairs, d_pair, d_lpairs, d_nlmatch):
         """LSDmatcher::SearchForTriangulation(pKF1, pKF2, pairs) (LSDmatcher.cpp:382-415) for npairs keyframe pairs in HBM, with
         KeyFrame::lineDescriptorMAD on the device.  d_ldesc [nkf, capl, 32], d_nl [nkf], d_has_ml [nkf, capl] u8, d_pair [npairs, 2] ->
         d_lpairs [npairs, capl, 2] ((qdx, tdx) ascending qdx, -1 after the count), d_nlmatch [npairs] (-1: pair index out of range, or
         KF1 has lines and KF2 fewer than 2).  Asynchronous on the matcher's stream."""
-        _check(lib().sslpl_line_search_for_triangulation_batch_device(
-            self._h, C.c_void_p(d_ldesc), C.c_void_p(d_nl), int(nkf), int(capl), C.c_void_p(d_has_ml), int(npairs), C.c_void_p(d_pair),
-            C.c_void_p(d_lpairs), C.c_void_p(d_nlmatch)))
+        _check(lib().sslpl_line_search_for_triangulation_batch_device(self._h, d_ldesc, d_nl, nkf, capl, d_has_ml, npairs, d_pair,
+                                                                      d_lpairs, d_nlmatch))
 
     def create_new_map_points_batch_device(self, d_kps, d_desc, d_n, nkf, cap, d_has_mp, vocab, levelsup, npairs, d_pair, d_geom, d_kfpose,
                                            cam, scale_factors, level_sigma2, scale_factor, d_pairs, d_nmatch, d_status, d_x3d, d_nnew):
@@ -491,13 +497,11 @@ class Matcher:
         (see sslpl_create_new_map_points_batch_device).  Inputs as search_for_triangulation_batch_device, plus d_kfpose [nkf, 15] f32 (Tcw
         3x4, Ow) and host cam = fx fy cx cy invfx invfy, scale_factors / level_sigma2 (nlevels = len) and scale_factor -> d_pairs [npairs,
         cap, 2], d_nmatch [npairs], d_status [npairs, cap] i32, d_x3d [npairs, cap, 3] f32, d_nnew [npairs].  Asynchronous."""
-        f32 = lambda a: np.ascontiguousarray(a, np.float32)
-        sc = f32(scale_factors); s2 = f32(level_sigma2); cm = f32(cam)
+        sc = _f32(scale_factors); s2 = _f32(level_sigma2); cm = _f32(cam)
         assert len(s2) >= len(sc) and len(cm) == 6
         _check(lib().sslpl_create_new_map_points_batch_device(
-            self._h, C.c_void_p(d_kps), C.c_void_p(d_desc), C.c_void_p(d_n), int(nkf), int(cap), C.c_void_p(d_has_mp), vocab._h,
-            int(levelsup), int(npairs), C.c_void_p(d_pair), C.c_void_p(d_geom), C.c_void_p(d_kfpose), _p(cm), _p(sc), _p(s2), len(sc),
-            C.c_float(scale_factor), C.c_void_p(d_pairs), C.c_void_p(d_nmatch), C.c_void_p(d_status), C.c_void_p(d_x3d), C.c_void_p(d_nnew)))
+            self._h, d_kps, d_desc, d_n, nkf, cap, d_has_mp, vocab._h, levelsup, npairs, d_pair, d_geom, d_kfpose, _p(cm), _p(sc), _p(s2),
+            len(sc), scale_factor, d_pairs, d_nmatch, d_status, d_x3d, d_nnew))
 
     def create_new_map_lines_batch_device(self, d_kl, d_ldesc, d_lineeq, d_nl, nkf, capl, d_has_ml, npairs, d_pair, d_kfpose, d_kfdepth,
                                           cam, d_lpairs, d_nlmatch, d_status, d_line3d, d_nnew):
@@ -508,19 +512,18 @@ class Matcher:
         (the caller's pair list: baseline gate 0.1, nn = 10), d_kfpose [nkf, 15] f32 (Tcw 3x4, Ow), d_kfdepth [nkf] f32
         (ComputeSceneMedianDepth(2)) and host cam = fx fy cx cy invfx invfy -> d_lpairs [npairs, capl, 2], d_nlmatch [npairs],
         d_status [npairs, capl] i32, d_line3d [npairs, capl, 6] f32 (s3D, e3D), d_nnew [npairs].  Asynchronous."""
-        cm = np.ascontiguousarray(cam, np.float32)
+        cm = _f32(cam)
         assert len(cm) == 6
         _check(lib().sslpl_create_new_map_lines_batch_device(
-            self._h, C.c_void_p(d_kl), C.c_void_p(d_ldesc), C.c_void_p(d_lineeq), C.c_void_p(d_nl), int(nkf), int(capl), C.c_void_p(d_has_ml),
-            int(npairs), C.c_void_p(d_pair), C.c_void_p(d_kfpose), C.c_void_p(d_kfdepth), _p(cm), C.c_void_p(d_lpairs), C.c_void_p(d_nlmatch),
-            C.c_void_p(d_status), C.c_void_p(d_line3d), C.c_void_p(d_nnew)))
+            self._h, d_kl, d_ldesc, d_lineeq, d_nl, nkf, capl, d_has_ml, npairs, d_pair, d_kfpose, d_kfdepth, _p(cm), d_lpairs, d_nlmatch,
+            d_status, d_line3d, d_nnew))
 
     def debug_svd4(self, A, hx=None, hy=None):
         """The device's 4x4 SVD (cv::SVD::compute on CV_32F) of host matrices A [n, 4, 4] -> (W [n, 4], Vt [n, 4, 4]), and its glibc
         hypot of hx, hy (float64) -> h.  Synchronous."""
-        A = np.ascontiguousarray(A, np.float32).reshape(-1, 16)
-        hx = np.ascontiguousarray(hx if hx is not None else [], np.float64).reshape(-1)
-        hy = np.ascontiguousarray(hy if hy is not None else [], np.float64).reshape(-1)
+        A = _f32(A).reshape(-1, 16)
+        hx = _f64(hx if hx is not None else []).reshape(-1)
+        hy = _f64(hy if hy is not None else []).reshape(-1)
         assert hx.shape == hy.shape
         n, nh = len(A), len(hx)
         W = np.empty((max(n, 1), 4), np.float32); Vt = np.empty((max(n, 1), 4, 4), np.float32); h = np.empty(max(nh, 1), np.float64)
@@ -535,13 +538,11 @@ class Matcher:
         d_entry [nentries, 2] i32 (kf, mp; mp = -1 NULL), d_skip [nentries] u8 or 0; cam = fx fy cx cy, bounds, scale_factors (nlevels =
         len), inv_level_sigma2 host arrays -> d_best_idx / d_best_dist [nentries] i32 ((-1, 256) no candidate, (-1, -1) index out of
         range).  Asynchronous on the matcher's stream."""
-        f32 = lambda a: np.ascontiguousarray(a, np.float32)
-        sf = f32(scale_factors); isg = f32(inv_level_sigma2)
+        sf = _f32(scale_factors); isg = _f32(inv_level_sigma2)
         assert len(isg) >= len(sf)
         _check(lib().sslpl_fuse_points_batch_device(
-            self._h, C.c_void_p(d_kps), C.c_void_p(d_desc), C.c_void_p(d_n), int(nkf), int(cap), C.c_void_p(d_kfpose), int(nmp),
-            C.c_void_p(d_mp), C.c_void_p(d_mpdesc), int(nentries), C.c_void_p(d_entry), C.c_void_p(d_skip or None), _p(f32(cam)[:4].copy()),
-            _p(f32(bounds)), _p(sf), _p(isg), len(sf), C.c_float(log_scale_factor), C.c_float(th), C.c_void_p(d_best_idx), C.c_void_p(d_best_dist)))
+            self._h, d_kps, d_desc, d_n, nkf, cap, d_kfpose, nmp, d_mp, d_mpdesc, nentries, d_entry, d_skip or None, _p(_f32(cam)[:4].copy()),
+            _p(_f32(bounds)), _p(sf), _p(isg), len(sf), log_scale_factor, th, d_best_idx, d_best_dist))
 
     def fuse_lines_batch_device(self, d_kl, d_ldesc, d_nl, nkf, capl, d_kfpose, nml, d_ml, d_mldesc, nentries, d_entry, d_skip,
                                 cam, bounds, scale_factors, log_scale_factor, th, d_best_idx, d_best_dist):
@@ -549,18 +550,16 @@ class Matcher:
         d_ldesc / d_nl as sslpl_line_device_results gives them, d_ml [nml, 12] f32 (SP, EP, normal, minInv, maxInv, maxRaw), d_mldesc
         [nml, 32]; the rest as fuse_points_batch_device -> (-1, INT_MAX) no candidate (a level outside the pyramid included), (-1, -1)
         index out of range.  Asynchronous on the matcher's stream."""
-        f32 = lambda a: np.ascontiguousarray(a, np.float32)
-        sf = f32(scale_factors)
+        sf = _f32(scale_factors)
         _check(lib().sslpl_fuse_lines_batch_device(
-            self._h, C.c_void_p(d_kl), C.c_void_p(d_ldesc), C.c_void_p(d_nl), int(nkf), int(capl), C.c_void_p(d_kfpose), int(nml),
-            C.c_void_p(d_ml), C.c_void_p(d_mldesc), int(nentries), C.c_void_p(d_entry), C.c_void_p(d_skip or None), _p(f32(cam)[:4].copy()),
-            _p(f32(bounds)), _p(sf), len(sf), C.c_float(log_scale_factor), C.c_float(th), C.c_void_p(d_best_idx), C.c_void_p(d_best_dist)))
+            self._h, d_kl, d_ldesc, d_nl, nkf, capl, d_kfpose, nml, d_ml, d_mldesc, nentries, d_entry, d_skip or None, _p(_f32(cam)[:4].copy()),
+            _p(_f32(bounds)), _p(sf), len(sf), log_scale_factor, th, d_best_idx, d_best_dist))
 
     def debug_predict_scale(self, ratio, log_scale_factor, nlevels, clamp=True):
         """MapPoint / MapLine::PredictScale on the device for host ratios (see sslpl_matcher_debug_predict_scale) -> int32 levels."""
-        r = np.ascontiguousarray(ratio, np.float32).reshape(-1)
+        r = _f32(ratio).reshape(-1)
         out = np.empty(max(len(r), 1), np.int32)
-        _check(lib().sslpl_matcher_debug_predict_scale(self._h, len(r), _p(r), C.c_float(log_scale_factor), int(nlevels), int(clamp), _p(out)))
+        _check(lib().sslpl_matcher_debug_predict_scale(self._h, len(r), _p(r), log_scale_factor, nlevels, int(clamp), _p(out)))
         return out[:len(r)]
 
 
@@ -568,11 +567,11 @@ def predict_scale_table(log_scale_factor, nlevels):
     """The nlevels + 1 PredictScale thresholds of sslpl_predict_scale_table (host only, no device): thr[k] = the smallest positive float
     ratio whose level (int)ceil(logf(ratio) / log_scale_factor) is >= k."""
     thr = np.empty(int(nlevels) + 1, np.float32)
-    _check(lib().sslpl_predict_scale_table(C.c_float(log_scale_factor), int(nlevels), _p(thr)))
+    _check(lib().sslpl_predict_scale_table(log_scale_factor, nlevels, _p(thr)))
     return thr
 
 
-class Vocabulary:
+class Vocabulary(_Handle, kind="vocab"):
     """DBoW2 ORB vocabulary tree on the device (the reference's ORBVocabulary = TemplatedVocabulary<FORB::TDescriptor, FORB>,
     include/ORBVocabulary.h; used by Frame::ComputeBoW Frame.cc:474-481 with levelsup = 4).
 
@@ -583,8 +582,8 @@ class Vocabulary:
     TF_IDF, TF, IDF, BINARY = 0, 1, 2, 3
 
     def __init__(self, k, L, parent, desc, weight, is_leaf, device=0, scoring=0, weighting=0):
-        self.parent = np.ascontiguousarray(parent, np.int32); self.desc = np.ascontiguousarray(desc, np.uint8).reshape(-1, 32)
-        self.weight = np.ascontiguousarray(weight, np.float64); self.is_leaf = np.ascontiguousarray(is_leaf, np.uint8)
+        self.parent = _i32(parent); self.desc = _u8(desc).reshape(-1, 32)
+        self.weight = _f64(weight); self.is_leaf = _u8(is_leaf)
         self.k, self.L, self.scoring, self.weighting = int(k), int(L), int(scoring), int(weighting)
         self._h = C.c_void_p()
         _check(lib().sslpl_vocab_create(device, self.k, self.L, len(self.parent), _p(self.parent), _p(self.desc), _p(self.weight),
@@ -636,7 +635,7 @@ class Vocabulary:
 
     def level_nodes(self, levelsup=4):
         c = C.c_int()
-        _check(lib().sslpl_vocab_level_nodes(self._h, int(levelsup), C.byref(c)))
+        _check(lib().sslpl_vocab_level_nodes(self._h, levelsup, C.byref(c)))
         return c.value
 
     def bow_vector(self, word, weight):
@@ -677,13 +676,6 @@ class Vocabulary:
         off = np.zeros(len(ids) + 1, np.int32); off[1:] = np.cumsum(counts)
         return ids.astype(np.int32), off, order.astype(np.int32)
 
-    def close(self):
-        if getattr(self, "_h", None) is not None and self._h.value:
-            lib().sslpl_vocab_destroy(self._h)
-            self._h = C.c_void_p()
-
-    __del__ = close
-
 
 class ORBmatcher:
     """Mirror of StructureSLAM::ORBmatcher (include/ORBmatcher.h:36-101) on indices + masks instead of
@@ -700,38 +692,36 @@ class ORBmatcher:
     def SearchByBoW(self, d1, fv1, valid1, angle1, d2, fv2, angle2, valid2=None):
         """KeyFrame-vs-Frame (valid2 is None; ORBmatcher.cc:159) -> (nmatches, match2[n2] = KF index or -1);
         KeyFrame-vs-KeyFrame (valid2 given; ORBmatcher.cc:525) -> (nmatches, match12[n1] = KF2 index or -1)."""
-        d1 = np.ascontiguousarray(d1, np.uint8).reshape(-1, 32); d2 = np.ascontiguousarray(d2, np.uint8).reshape(-1, 32)
+        d1 = _u8(d1).reshape(-1, 32); d2 = _u8(d2).reshape(-1, 32)
         f1, f2 = _featvec(fv1), _featvec(fv2)
-        valid1 = np.ascontiguousarray(valid1, np.uint8)
-        angle1 = np.ascontiguousarray(angle1, np.float32); angle2 = np.ascontiguousarray(angle2, np.float32)
+        valid1 = _u8(valid1)
+        angle1 = _f32(angle1); angle2 = _f32(angle2)
         nm = C.c_int()
         if valid2 is None:
             out = np.empty(len(d2), np.int32)
             _check(lib().sslpl_search_by_bow(self.ctx._h, _p(d1), len(d1), _p(d2), len(d2), C.byref(f1), C.byref(f2),
-                                             _p(valid1), _p(angle1), _p(angle2), C.c_float(self.mfNNratio),
-                                             int(self.mbCheckOrientation), _p(out), C.byref(nm)))
+                                             _p(valid1), _p(angle1), _p(angle2), self.mfNNratio, self.mbCheckOrientation, _p(out), C.byref(nm)))
         else:
-            valid2 = np.ascontiguousarray(valid2, np.uint8)
+            valid2 = _u8(valid2)
             out = np.empty(len(d1), np.int32)
             _check(lib().sslpl_search_by_bow_kf(self.ctx._h, _p(d1), len(d1), _p(d2), len(d2), C.byref(f1), C.byref(f2),
-                                                _p(valid1), _p(valid2), _p(angle1), _p(angle2), C.c_float(self.mfNNratio),
-                                                int(self.mbCheckOrientation), _p(out), C.byref(nm)))
+                                                _p(valid1), _p(valid2), _p(angle1), _p(angle2), self.mfNNratio, self.mbCheckOrientation,
+                                                _p(out), C.byref(nm)))
         return nm.value, out
 
     def SearchForTriangulation(self, d1, fv1, has_mp1, kp1, d2, fv2, has_mp2, kp2, F12, ex, ey, scale, sigma2):
         """ORBmatcher.cc:660 (monocular) -> (nmatches, pairs[nmatches,2])."""
-        d1 = np.ascontiguousarray(d1, np.uint8).reshape(-1, 32); d2 = np.ascontiguousarray(d2, np.uint8).reshape(-1, 32)
+        d1 = _u8(d1).reshape(-1, 32); d2 = _u8(d2).reshape(-1, 32)
         f1, f2 = _featvec(fv1), _featvec(fv2)
-        has_mp1 = np.ascontiguousarray(has_mp1, np.uint8); has_mp2 = np.ascontiguousarray(has_mp2, np.uint8)
+        has_mp1 = _u8(has_mp1); has_mp2 = _u8(has_mp2)
         kp1 = np.ascontiguousarray(kp1, KEYPOINT_DTYPE); kp2 = np.ascontiguousarray(kp2, KEYPOINT_DTYPE)
-        F12 = np.ascontiguousarray(F12, np.float32).reshape(9)
-        scale = np.ascontiguousarray(scale, np.float32); sigma2 = np.ascontiguousarray(sigma2, np.float32)
+        F12 = _f32(F12).reshape(9)
+        scale = _f32(scale); sigma2 = _f32(sigma2)
         pairs = np.empty((max(len(d1), 1), 2), np.int32)
         nm = C.c_int()
         _check(lib().sslpl_search_for_triangulation(self.ctx._h, _p(d1), len(d1), _p(d2), len(d2), C.byref(f1), C.byref(f2),
-                                                    _p(has_mp1), _p(has_mp2), _p(kp1), _p(kp2), _p(F12), C.c_float(ex), C.c_float(ey),
-                                                    _p(scale), _p(sigma2), len(scale), int(self.mbCheckOrientation),
-                                                    _p(pairs), C.byref(nm)))
+                                                    _p(has_mp1), _p(has_mp2), _p(kp1), _p(kp2), _p(F12), ex, ey, _p(scale), _p(sigma2), len(scale),
+                                                    self.mbCheckOrientation, _p(pairs), C.byref(nm)))
         return nm.value, pairs[:nm.value].copy()
 
 
@@ -742,9 +732,9 @@ class LSDmatcher:
         self.ctx = ctx or Matcher()
 
     def _run(self, mode, d1, d2, has_ml1, has_ml2):
-        d1 = np.ascontiguousarray(d1, np.uint8).reshape(-1, 32); d2 = np.ascontiguousarray(d2, np.uint8).reshape(-1, 32)
-        h1 = np.ascontiguousarray(has_ml1 if has_ml1 is not None else np.zeros(len(d1)), np.uint8)
-        h2 = np.ascontiguousarray(has_ml2 if has_ml2 is not None else np.zeros(len(d2)), np.uint8)
+        d1 = _u8(d1).reshape(-1, 32); d2 = _u8(d2).reshape(-1, 32)
+        h1 = _u8(has_ml1 if has_ml1 is not None else np.zeros(len(d1)))
+        h2 = _u8(has_ml2 if has_ml2 is not None else np.zeros(len(d2)))
         out = np.full(2 * max(len(d1), len(d2), 1), -1, np.int32)
         k = C.c_int(); nm = C.c_int(); mad = (C.c_double * 2)()
         _check(lib().sslpl_line_match(self.ctx._h, mode, _p(d1), len(d1), _p(d2), len(d2), _p(h1), _p(h2), _p(out),
@@ -767,10 +757,7 @@ class LSDmatcher:
     def SearchByDescriptorKF(self, ldesc1, ldesc2, has_mapline_KF2):    # LSDmatcher.cpp:329
         return self._run(2, ldesc1, ldesc2, None, has_mapline_KF2)
 
-    def SearchForTriangulation(self, ldesc1, has_mapline_KF1, ldesc2, has_mapline_KF2):    # LSDmatcher.cpp:382 -> (n, pairs[n, 2])
-        return self._run(3, ldesc1, ldesc2, has_mapline_KF1, has_mapline_KF2)
-
-    def SearchForTriangulation(self, ldesc1, has_ml1, ldesc2, has_ml2):  # LSDmatcher.cpp:382
+    def SearchForTriangulation(self, ldesc1, has_ml1, ldesc2, has_ml2):  # LSDmatcher.cpp:382 -> (n, pairs[n, 2])
         return self._run(3, ldesc1, ldesc2, has_ml1, has_ml2)
 
     def DescriptorDistance(self, a, b):                                 # LSDmatcher.cpp:364
@@ -784,30 +771,25 @@ class FrameParams(C.Structure):
     _fields_ = [("orb", OrbParams), ("line", LineParams)]
 
 
-class Frame:
+class Frame(_Handle, kind="frame", lifecycle=("sync", "launch_count")):
     """What StructureSLAM::Frame::Frame(imGray, ...) does with the two extractors (src/Frame.cc:69-131): ONE upload of the frame,
     ORB and LSD+LBD on two streams, optional colour conversion in front (Tracking.cc:148-161) and keypoint undistortion behind
     (Frame.cc:483-513).  `extract(image)` -> dict(keys, keysUn, desc, keylines, ldesc, lineeq)."""
 
     def __init__(self, nfeatures=1000, scaleFactor=1.2, nlevels=8, iniThFAST=20, minThFAST=7, lsdNFeatures=40,
                  max_width=1280, max_height=960, max_batch=1, device=0):
-        p = FrameParams(OrbParams(nfeatures, scaleFactor, nlevels, iniThFAST, minThFAST, max_width, max_height, max_batch, device),
-                        LineParams(lsdNFeatures, max_width, max_height, max_batch, device))
-        self._h = C.c_void_p()
-        lib().sslpl_frame_create.argtypes = [C.c_void_p, C.c_void_p]
-        _check(lib().sslpl_frame_create(C.byref(p), C.byref(self._h)))
-        lib().sslpl_frame_orb.restype = C.c_void_p; lib().sslpl_frame_orb.argtypes = [C.c_void_p]
-        lib().sslpl_frame_line.restype = C.c_void_p; lib().sslpl_frame_line.argtypes = [C.c_void_p]
-        lib().sslpl_frame_stream.restype = C.c_void_p; lib().sslpl_frame_stream.argtypes = [C.c_void_p, C.c_int]
-        self.orb = ORBextractor._borrow(lib().sslpl_frame_orb(self._h), nfeatures, scaleFactor, nlevels, max_batch)
-        self.line = LineSegment._borrow(lib().sslpl_frame_line(self._h), lsdNFeatures, max_batch)
-        self.cap = self.orb.cap
+        self._create(FrameParams(OrbParams(nfeatures, scaleFactor, nlevels, iniThFAST, minThFAST, max_width, max_height, max_batch, device),
+                                 LineParams(lsdNFeatures, max_width, max_height, max_batch, device)))
+        orb = lib().sslpl_frame_orb(self._h)
+        self.cap = lib().sslpl_orb_max_keypoints(orb)
+        self.orb = ORBextractor._borrow(orb, nfeatures=nfeatures, scaleFactor=scaleFactor, nlevels=nlevels, max_batch=max_batch, cap=self.cap)
+        self.line = LineSegment._borrow(lib().sslpl_frame_line(self._h), cap=lsdNFeatures, max_batch=max_batch)
         self.lcap = lsdNFeatures
         self.max_batch = max_batch
 
     def stream(self, which):
         """CUDA stream handle of the ORB (0) or line (1) side."""
-        return int(lib().sslpl_frame_stream(self._h, int(which)))
+        return lib().sslpl_frame_stream(self._h, which)
 
     def extract_batch_begin(self, frames, out):
         """Asynchronous: frames [B, H, W] uint8 in pinned memory (host_alloc); out = dict(keys, desc, n, keylines, ldesc, lineeq, nl) of
@@ -815,12 +797,9 @@ class Frame:
         B, h, w = frames.shape[:3]
         cn = 1 if frames.ndim == 3 else frames.shape[3]
         assert out["keys"].shape[1] == self.cap and out["keylines"].shape[1] == self.lcap
-        _check(lib().sslpl_frame_extract_batch_begin(self._h, _p(frames), B, w, h, frames.strides[1], C.c_size_t(frames.strides[0]), cn, 0,
+        _check(lib().sslpl_frame_extract_batch_begin(self._h, _p(frames), B, w, h, frames.strides[1], frames.strides[0], cn, 0,
                                                      _p(out["keys"]), None, _p(out["desc"]), self.cap, _p(out["n"]),
                                                      _p(out["keylines"]), _p(out["ldesc"]), _p(out["lineeq"]), self.lcap, _p(out["nl"])))
-
-    def sync(self):
-        _check(lib().sslpl_frame_sync(self._h))
 
     def device_keypoints_un(self):
         """(device pointer, cap) of the last call's mvKeysUn: undistorted keypoints when k1 != 0, else the ORB keypoints (Frame.cc:485).
@@ -829,27 +808,14 @@ class Frame:
         _check(lib().sslpl_frame_device_keypoints_un(self._h, C.byref(p), C.byref(cap)))
         return p.value, cap.value
 
-    def close(self):
-        if getattr(self, "_h", None) is not None and self._h.value:
-            lib().sslpl_frame_destroy.argtypes = [C.c_void_p]
-            lib().sslpl_frame_destroy(self._h)
-            self._h = C.c_void_p()
-
-    __del__ = close
-
     def set_camera(self, fx, fy, cx, cy, dist=()):
-        d = np.ascontiguousarray(dist, np.float32)
-        _check(lib().sslpl_frame_set_camera(self._h, C.c_float(fx), C.c_float(fy), C.c_float(cx), C.c_float(cy), _p(d) if len(d) else None, len(d)))
+        d = _f32(dist)
+        _check(lib().sslpl_frame_set_camera(self._h, fx, fy, cx, cy, _p(d) if len(d) else None, len(d)))
 
     def image_bounds(self, cols, rows):
         b = np.zeros(4, np.float32)
-        _check(lib().sslpl_frame_image_bounds(self._h, int(cols), int(rows), _p(b)))
+        _check(lib().sslpl_frame_image_bounds(self._h, cols, rows, _p(b)))
         return b
-
-    @property
-    def launch_count(self):
-        lib().sslpl_frame_launch_count.restype = C.c_longlong
-        return int(lib().sslpl_frame_launch_count(self._h))
 
     def extract(self, image, rgb_order=False):
         """image: HxW (grey) or HxWx3 / HxWx4 uint8 (BGR[A] unless rgb_order)."""
@@ -873,7 +839,7 @@ class Frame:
         kps = np.zeros((B, self.cap), KEYPOINT_DTYPE); un = np.zeros((B, self.cap), KEYPOINT_DTYPE); desc = np.zeros((B, self.cap, 32), np.uint8)
         kl = np.zeros((B, self.lcap), KEYLINE_DTYPE); ld = np.zeros((B, self.lcap, 32), np.uint8); eq = np.zeros((B, self.lcap, 3), np.float64)
         n = np.zeros(B, np.int32); nl = np.zeros(B, np.int32)
-        _check(lib().sslpl_frame_extract_batch(self._h, _p(frames), B, w, h, frames.strides[1], C.c_size_t(frames.strides[0]), cn, int(rgb_order),
+        _check(lib().sslpl_frame_extract_batch(self._h, _p(frames), B, w, h, frames.strides[1], frames.strides[0], cn, int(rgb_order),
                                                _p(kps), _p(un), _p(desc), self.cap, _p(n), _p(kl), _p(ld), _p(eq), self.lcap, _p(nl)))
         return dict(keys=kps, keysUn=un, desc=desc, n=n, keylines=kl, ldesc=ld, lineeq=eq, nl=nl)
 
@@ -881,29 +847,14 @@ class Frame:
 # =====================================================================================================
 # Lines
 # =====================================================================================================
-class LineSegment:
+class LineSegment(_Handle, kind="line", lifecycle=("sync", "set_stream", "stream", "launch_count", "set_profiling", "stage_ms")):
     """Mirror of StructureSLAM::LineSegment (include/ExtractLineSegment.h:53-76).  lsdNFeatures is hard-coded to 40
     in the reference (ExtractLineSegment.cpp:42); it is a constructor parameter here (BASELINE.json config 4: 500)."""
 
     def __init__(self, lsdNFeatures=40, max_width=1280, max_height=960, max_batch=1, device=0):
-        p = LineParams(lsdNFeatures, max_width, max_height, max_batch, device)
-        self._h = C.c_void_p()
-        _check(lib().sslpl_line_create(C.byref(p), C.byref(self._h)))
+        self._create(LineParams(lsdNFeatures, max_width, max_height, max_batch, device))
         self.cap = lsdNFeatures
         self.max_batch = max_batch
-
-    @classmethod
-    def _borrow(cls, ptr, lsdNFeatures, max_batch):
-        self = cls.__new__(cls)
-        self._h = C.c_void_p(ptr); self._borrowed = True; self.cap = lsdNFeatures; self.max_batch = max_batch
-        return self
-
-    def close(self):
-        if getattr(self, "_h", None) is not None and self._h.value and not getattr(self, "_borrowed", False):
-            lib().sslpl_line_destroy(self._h)
-            self._h = C.c_void_p()
-
-    __del__ = close
 
     def ExtractLineSegment(self, img, scale=1, numOctaves=1):
         """-> (keylines, ldesc, keylineFunctions): ExtractLineSegment.cpp:18-69 (scale / numOctaves as the reference
@@ -925,18 +876,18 @@ class LineSegment:
             out = (np.zeros((B, self.cap), KEYLINE_DTYPE), np.zeros((B, self.cap, 32), np.uint8),
                    np.zeros((B, self.cap, 3), np.float64), np.zeros(B, np.int32))
         kl, ld, eq, n = out
-        _check(lib().sslpl_line_extract_batch(self._h, _p(frames), B, W, H, frames.strides[1], C.c_size_t(frames.strides[0]),
+        _check(lib().sslpl_line_extract_batch(self._h, _p(frames), B, W, H, frames.strides[1], frames.strides[0],
                                               _p(kl), _p(ld), _p(eq), self.cap, _p(n)))
         return kl, ld, eq, n
 
     def extract_batch_begin(self, frames, out):
         B, H, W = frames.shape
         kl, ld, eq, n = out
-        _check(lib().sslpl_line_extract_batch_begin(self._h, _p(frames), B, W, H, frames.strides[1], C.c_size_t(frames.strides[0]),
+        _check(lib().sslpl_line_extract_batch_begin(self._h, _p(frames), B, W, H, frames.strides[1], frames.strides[0],
                                                     _p(kl), _p(ld), _p(eq), self.cap, _p(n)))
 
     def extract_batch_device(self, d_ptr, nframes, width, height, pitch, frame_stride):
-        _check(lib().sslpl_line_extract_batch_device(self._h, C.c_void_p(d_ptr), nframes, width, height, pitch, C.c_size_t(frame_stride)))
+        _check(lib().sslpl_line_extract_batch_device(self._h, d_ptr, nframes, width, height, pitch, frame_stride))
 
     def device_results(self):
         kl = C.c_void_p(); ld = C.c_void_p(); eq = C.c_void_p(); n = C.c_void_p(); cap = C.c_int()
@@ -974,37 +925,29 @@ class LineSegment:
         """The NFA kernels' nfa() on arrays (n, k, p) with the log_nt and log-gamma table of a width x height frame -> (log_nfa float64,
         stop int32: loop index of the early stop, n + 1 when the tail loop ran out, -1 for the early returns).  plain=True turns the
         pow skip and the log10 bracket off."""
-        n = np.ascontiguousarray(n, np.int32); k = np.ascontiguousarray(k, np.int32); p = np.ascontiguousarray(p, np.float64)
+        n = _i32(n); k = _i32(k); p = _f64(p)
         assert n.shape == k.shape == p.shape and n.ndim == 1
         out = np.empty(len(n), np.float64); stop = np.empty(len(n), np.int32)
-        _check(lib().sslpl_line_debug_nfa(self._h, int(width), int(height), len(n), _p(n), _p(k), _p(p), int(bool(plain)), _p(out), _p(stop)))
+        _check(lib().sslpl_line_debug_nfa(self._h, width, height, len(n), _p(n), _p(k), _p(p), int(bool(plain)), _p(out), _p(stop)))
         return out, stop
 
     def debug_sincos(self, x, full=False):
         """ddtrig::sincos_cr (full=False, region2rect's form) or sincos_cr_full of a float64 array on the device -> (sin, cos)."""
-        x = np.ascontiguousarray(x, np.float64).reshape(-1)
+        x = _f64(x).reshape(-1)
         s = np.empty_like(x); c = np.empty_like(x)
         _check(lib().sslpl_line_debug_sincos(self._h, len(x), _p(x), int(bool(full)), _p(s), _p(c)))
         return s, c
 
     def debug_atan2(self, y, x):
         """The line path's fast_atan2_deg (cv::fastAtan2) of float32 arrays on the device."""
-        y = np.ascontiguousarray(y, np.float32).reshape(-1); x = np.ascontiguousarray(x, np.float32).reshape(-1)
+        y = _f32(y).reshape(-1); x = _f32(x).reshape(-1)
         assert y.shape == x.shape
         out = np.empty_like(x)
         _check(lib().sslpl_line_debug_atan2(self._h, len(x), _p(y), _p(x), _p(out)))
         return out
 
     def set_max_walkers(self, n):
-        _check(lib().sslpl_line_set_max_walkers(self._h, int(n)))
-
-    def set_profiling(self, on=True):
-        _check(lib().sslpl_line_set_profiling(self._h, int(on)))
-
-    def stage_ms(self):
-        ms = (C.c_float * 16)(); names = (C.c_char_p * 16)(); n = C.c_int()
-        _check(lib().sslpl_line_stage_ms(self._h, ms, 16, names, C.byref(n)))
-        return {names[i].decode(): float(ms[i]) for i in range(n.value)}
+        _check(lib().sslpl_line_set_max_walkers(self._h, n))
 
     def walker_stats(self):
         out = (C.c_ulonglong * 16)()
@@ -1017,13 +960,3 @@ class LineSegment:
         out = np.empty((cap, 10), np.float64); n = C.c_int()
         _check(lib().sslpl_line_debug_trace(self._h, frame, _p(out), cap, C.byref(n)))
         return out[:min(n.value, cap)].copy()
-
-    def sync(self):
-        _check(lib().sslpl_line_sync(self._h))
-
-    def set_stream(self, cuda_stream):
-        _check(lib().sslpl_line_set_stream(self._h, C.c_void_p(cuda_stream)))
-
-    @property
-    def launch_count(self):
-        return int(lib().sslpl_line_launch_count(self._h))
