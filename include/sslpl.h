@@ -540,6 +540,7 @@ int  sslpl_line_debug_trace(sslpl_line* h, int frame, double* out, int cap_rows,
    entries), *nseeds.  Any output pointer may be NULL.  Region growing changes none of these, so they stay valid after a full call. */
 int  sslpl_line_download_prep(sslpl_line* h, int frame, int* w, int* hgt, int* sw, int* sh, int16_t* dx, int16_t* dy, float* angdeg,
                               float* pix_cs, float* cs0, double* modgrad, double* maxgrad, uint32_t* seeds, int* nseeds);
+/* The four debug calls below each launch one kernel on the handle's stream, counted by sslpl_line_launch_count, and wait for it. */
 /* debug: the pre-pass's per-pixel ll_angle arithmetic on every 2x2 difference pair (DA = D - A, BC = B - C, each in [-255, 255]),
    entry (DA + 255) * 511 + (BC + 255): 261121 angles, cs / cs0 pairs and norms, as in sslpl_line_download_prep.  NULL = skip. */
 int  sslpl_line_debug_ll_table(sslpl_line* h, float* angdeg, float* cs, float* cs0, double* modgrad);

@@ -57,19 +57,38 @@ __global__ void __launch_bounds__(256) k_undistort(const sslpl_keypoint* __restr
 
 using namespace sslpl;
 
-struct sslpl_frame {
+// The core's stream is the ORB side's (the upload, colour conversion and undistortion run on it); its scratch stages multi-channel input.
+struct sslpl_frame : sslpl::StreamHandle {
     sslpl_frame_params p;
     sslpl_orb* orb = nullptr; sslpl_line* line = nullptr;
-    cudaStream_t s_orb = nullptr, s_line = nullptr;
+    cudaStream_t s_line = nullptr;
     cudaEvent_t ev_in = nullptr, ev_line = nullptr;
-    uint8_t* d_raw = nullptr; size_t raw_bytes = 0;       // multi-channel input staging
     uint8_t* d_gray = nullptr; int gpitch = 0; size_t gstride = 0;
     sslpl_keypoint* d_un = nullptr;                        // undistorted keypoints [max_batch][cap]
     Camera cam;
     int cap = 0, last_pitch = 0; size_t last_stride = 0;
     bool last_undistorted = false;                         // the last call wrote mvKeysUn to d_un (k1 != 0)
-    long long launches = 0;
 };
+
+namespace {
+
+int frame_init(sslpl_frame* h) {
+    const sslpl_frame_params* p = &h->p;
+    if (int rc = h->open(p->orb.device)) return rc;
+    if (int rc = sslpl_orb_create(&p->orb, &h->orb)) return rc;
+    if (int rc = sslpl_line_create(&p->line, &h->line)) return rc;
+    SSLPL_CUDA(cudaStreamCreateWithFlags(&h->s_line, cudaStreamNonBlocking));
+    SSLPL_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
+    SSLPL_CUDA(cudaEventCreateWithFlags(&h->ev_line, cudaEventDisableTiming));
+    h->gpitch = (int)align_up((size_t)p->orb.max_width, 64); h->gstride = (size_t)h->gpitch * p->orb.max_height;
+    h->cap = sslpl_orb_max_keypoints(h->orb);
+    SSLPL_CUDA(cudaMalloc(&h->d_gray, h->gstride * p->orb.max_batch + 256));
+    SSLPL_CUDA(cudaMalloc(&h->d_un, sizeof(sslpl_keypoint) * (size_t)h->cap * p->orb.max_batch));
+    if (int rc = sslpl_orb_set_stream(h->orb, h->stream)) return rc;
+    return sslpl_line_set_stream(h->line, h->s_line);
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -80,40 +99,27 @@ int sslpl_frame_create(const sslpl_frame_params* p, sslpl_frame** out) {
     sslpl_frame* h = new (std::nothrow) sslpl_frame();
     SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "out of host memory");
     h->p = *p;
-    int rc = sslpl_orb_create(&p->orb, &h->orb);
-    if (rc == SSLPL_OK) rc = sslpl_line_create(&p->line, &h->line);
-    if (rc != SSLPL_OK) { sslpl_frame_destroy(h); return rc; }
-    cudaError_t e = cudaSetDevice(p->orb.device);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->s_orb, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->s_line, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&h->ev_line, cudaEventDisableTiming);
-    h->gpitch = (int)align_up((size_t)p->orb.max_width, 64); h->gstride = (size_t)h->gpitch * p->orb.max_height;
-    h->cap = sslpl_orb_max_keypoints(h->orb);
-    if (e == cudaSuccess) e = cudaMalloc(&h->d_gray, h->gstride * p->orb.max_batch + 256);
-    if (e == cudaSuccess) e = cudaMalloc(&h->d_un, sizeof(sslpl_keypoint) * (size_t)h->cap * p->orb.max_batch);
-    if (e != cudaSuccess) { set_error("sslpl_frame_create: %s", cudaGetErrorString(e)); sslpl_frame_destroy(h); return SSLPL_ERR_CUDA; }
-    sslpl_orb_set_stream(h->orb, h->s_orb); sslpl_line_set_stream(h->line, h->s_line);
     memset(&h->cam, 0, sizeof(h->cam)); h->cam.fx = h->cam.fy = 1.0;
+    const int rc = frame_init(h);
+    if (rc != SSLPL_OK) { sslpl_frame_destroy(h); return rc; }
     *out = h;
     return SSLPL_OK;
 }
 
 void sslpl_frame_destroy(sslpl_frame* h) {
     if (!h) return;
-    if (h->orb) sslpl_orb_destroy(h->orb);
+    if (h->orb) sslpl_orb_destroy(h->orb);                 // before the streams they were given
     if (h->line) sslpl_line_destroy(h->line);
-    if (h->d_raw) cudaFree(h->d_raw);
+    h->close();
     if (h->d_gray) cudaFree(h->d_gray);
     if (h->d_un) cudaFree(h->d_un);
     if (h->ev_in) cudaEventDestroy(h->ev_in);
     if (h->ev_line) cudaEventDestroy(h->ev_line);
-    if (h->s_orb) cudaStreamDestroy(h->s_orb);
     if (h->s_line) cudaStreamDestroy(h->s_line);
     delete h;
 }
 
-void* sslpl_frame_stream(sslpl_frame* h, int which) { return h ? (which ? (void*)h->s_line : (void*)h->s_orb) : nullptr; }
+void* sslpl_frame_stream(sslpl_frame* h, int which) { return h ? (which ? (void*)h->s_line : (void*)h->stream) : nullptr; }
 sslpl_orb* sslpl_frame_orb(sslpl_frame* h) { return h ? h->orb : nullptr; }
 sslpl_line* sslpl_frame_line(sslpl_frame* h) { return h ? h->line : nullptr; }
 long long sslpl_frame_launch_count(const sslpl_frame* h) { return h ? h->launches + sslpl_orb_launch_count(h->orb) + sslpl_line_launch_count(h->line) : 0; }
@@ -131,20 +137,18 @@ int sslpl_frame_image_bounds(sslpl_frame* h, int cols, int rows, float* bounds4)
     SSLPL_REQUIRE(h && bounds4, SSLPL_ERR_ARG, "null argument");
     if (!h->cam.distorted) { bounds4[0] = 0.f; bounds4[1] = (float)cols; bounds4[2] = 0.f; bounds4[3] = (float)rows; return SSLPL_OK; }
     SSLPL_CUDA(cudaSetDevice(h->p.orb.device));
-    sslpl_keypoint c[4]; int n4 = 4;
+    sslpl_keypoint c[4]; const int n4 = 4;
     memset(c, 0, sizeof(c));
     c[1].x = (float)cols; c[2].y = (float)rows; c[3].x = (float)cols; c[3].y = (float)rows;
-    sslpl_keypoint* d = nullptr; int* dn = nullptr;
-    SSLPL_CUDA(cudaMalloc(&d, sizeof(c) * 2)); 
-    cudaError_t e = cudaMalloc(&dn, sizeof(int));
-    if (e != cudaSuccess) { cudaFree(d); set_error("cudaMalloc: %s", cudaGetErrorString(e)); return SSLPL_ERR_CUDA; }
-    cudaMemcpyAsync(d, c, sizeof(c), cudaMemcpyHostToDevice, h->s_orb); cudaMemcpyAsync(dn, &n4, sizeof(int), cudaMemcpyHostToDevice, h->s_orb);
-    k_undistort<<<dim3(1, 1), 256, 0, h->s_orb>>>(d, dn, 4, h->cam, d + 4);
-    h->launches++;
-    cudaMemcpyAsync(c, d + 4, sizeof(c), cudaMemcpyDeviceToHost, h->s_orb);
-    e = cudaStreamSynchronize(h->s_orb);
-    cudaFree(d); cudaFree(dn);
-    if (e != cudaSuccess) { set_error("sslpl_frame_image_bounds: %s", cudaGetErrorString(e)); return SSLPL_ERR_CUDA; }
+    if (int rc = ensure_scratch(h, 2 * sizeof(c) + 1024)) return rc;
+    Arena A; A.base = h->scratch;
+    cudaError_t e = cudaSuccess;
+    const sslpl_keypoint* d_in = stage(A, c, 4, h->stream, e); const int* d_n = stage(A, &n4, 1, h->stream, e); sslpl_keypoint* d_out = A.take<sslpl_keypoint>(4);
+    SSLPL_CUDA(e);
+    launch(h, k_undistort, dim3(1, 1), 256, 0, d_in, d_n, 4, h->cam, d_out);
+    SSLPL_CUDA(cudaGetLastError());
+    SSLPL_CUDA(cudaMemcpyAsync(c, d_out, sizeof(c), cudaMemcpyDeviceToHost, h->stream));
+    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
     bounds4[0] = fminf(c[0].x, c[2].x); bounds4[1] = fmaxf(c[1].x, c[3].x); bounds4[2] = fminf(c[0].y, c[1].y); bounds4[3] = fmaxf(c[2].y, c[3].y);
     return SSLPL_OK;
 }
@@ -166,29 +170,20 @@ int sslpl_frame_extract_batch_begin(sslpl_frame* h, const uint8_t* imgs, int nfr
     const int gp = (int)align_up((size_t)width, 64); const size_t gs = (size_t)gp * height;
     h->last_pitch = gp; h->last_stride = gs;
     // ---- one upload
-    if (channels == 1) {
-        if (nframes == 1 || frame_stride == (size_t)pitch * height)      // contiguous frames: one 2-D copy over all rows
-            SSLPL_CUDA(cudaMemcpy2DAsync(h->d_gray, gp, imgs, pitch, width, (size_t)height * nframes, cudaMemcpyHostToDevice, h->s_orb));
-        else for (int f = 0; f < nframes; f++)
-            SSLPL_CUDA(cudaMemcpy2DAsync(h->d_gray + f * gs, gp, imgs + f * frame_stride, pitch, width, height, cudaMemcpyHostToDevice, h->s_orb));
-    } else {
-        const size_t rowb = (size_t)width * channels, need = rowb * height * nframes;
-        if (need > h->raw_bytes) {
-            SSLPL_CUDA(cudaStreamSynchronize(h->s_orb));
-            if (h->d_raw) cudaFree(h->d_raw);
-            h->d_raw = nullptr; h->raw_bytes = 0;
-            SSLPL_CUDA(cudaMalloc(&h->d_raw, need)); h->raw_bytes = need;
-        }
-        for (int f = 0; f < nframes; f++)
-            SSLPL_CUDA(cudaMemcpy2DAsync(h->d_raw + f * rowb * height, rowb, imgs + f * frame_stride, pitch, rowb, height, cudaMemcpyHostToDevice, h->s_orb));
-        k_cvt_gray<<<dim3((width + 255) / 256, height, nframes), 256, 0, h->s_orb>>>(h->d_raw, width, height, (int)rowb, channels, rgb_order ? 1 : 0,
-                                                                                 h->d_gray, gp, (long long)(rowb * height), (long long)gs);
-        h->launches++;
+    int rc;
+    if (channels == 1) rc = h->upload_frames(h->d_gray, gp, gs, imgs, pitch, frame_stride, width, height, nframes);
+    else {                                                               // the colour frames into the scratch, the grey frames from it
+        const size_t rowb = (size_t)width * channels;
+        rc = ensure_scratch(h, rowb * height * nframes);
+        if (rc == SSLPL_OK) rc = h->upload_frames(h->scratch, rowb, rowb * height, imgs, pitch, frame_stride, rowb, height, nframes);
+        if (rc == SSLPL_OK) launch(h, k_cvt_gray, dim3((width + 255) / 256, height, nframes), 256, 0, h->scratch, width, height, (int)rowb, channels,
+                                   rgb_order ? 1 : 0, h->d_gray, gp, (long long)(rowb * height), (long long)gs);
     }
-    SSLPL_CUDA(cudaEventRecord(h->ev_in, h->s_orb));
+    if (rc != SSLPL_OK) return rc;
+    SSLPL_CUDA(cudaEventRecord(h->ev_in, h->stream));
     SSLPL_CUDA(cudaStreamWaitEvent(h->s_line, h->ev_in, 0));
     // ---- ORB and LSD+LBD on two streams, from the same device frame
-    int rc = sslpl_orb_extract_batch_device(h->orb, h->d_gray, nframes, width, height, gp, gs);
+    rc = sslpl_orb_extract_batch_device(h->orb, h->d_gray, nframes, width, height, gp, gs);
     if (rc != SSLPL_OK) return rc;
     rc = sslpl_line_extract_batch_device(h->line, h->d_gray, nframes, width, height, gp, gs);
     if (rc != SSLPL_OK) return rc;
@@ -198,20 +193,17 @@ int sslpl_frame_extract_batch_begin(sslpl_frame* h, const uint8_t* imgs, int nfr
     // mvKeysUn: always computed with k1 != 0 (the device consumers read it through sslpl_frame_device_keypoints_un); with k1 == 0 it
     // equals the ORB keypoints and is only copied for the host output
     h->last_undistorted = h->cam.distorted != 0;
-    if (kps_un || h->last_undistorted) {
-        k_undistort<<<dim3((c2 + 255) / 256, nframes), 256, 0, h->s_orb>>>(d_kps, d_n, c2, h->cam, h->d_un);
-        h->launches++;
-    }
+    if (kps_un || h->last_undistorted) launch(h, k_undistort, dim3((c2 + 255) / 256, nframes), 256, 0, d_kps, d_n, c2, h->cam, h->d_un);
     // ---- results
-    SSLPL_CUDA(cudaMemcpyAsync(nkp, d_n, sizeof(int) * nframes, cudaMemcpyDeviceToHost, h->s_orb));
+    SSLPL_CUDA(cudaMemcpyAsync(nkp, d_n, sizeof(int) * nframes, cudaMemcpyDeviceToHost, h->stream));
     if (cap == c2) {                                                     // same stride on both sides: one copy per array
-        if (kps) SSLPL_CUDA(cudaMemcpyAsync(kps, d_kps, sizeof(sslpl_keypoint) * (size_t)c2 * nframes, cudaMemcpyDeviceToHost, h->s_orb));
-        if (kps_un) SSLPL_CUDA(cudaMemcpyAsync(kps_un, h->d_un, sizeof(sslpl_keypoint) * (size_t)c2 * nframes, cudaMemcpyDeviceToHost, h->s_orb));
-        if (desc) SSLPL_CUDA(cudaMemcpyAsync(desc, d_desc, (size_t)c2 * 32 * nframes, cudaMemcpyDeviceToHost, h->s_orb));
+        if (kps) SSLPL_CUDA(cudaMemcpyAsync(kps, d_kps, sizeof(sslpl_keypoint) * (size_t)c2 * nframes, cudaMemcpyDeviceToHost, h->stream));
+        if (kps_un) SSLPL_CUDA(cudaMemcpyAsync(kps_un, h->d_un, sizeof(sslpl_keypoint) * (size_t)c2 * nframes, cudaMemcpyDeviceToHost, h->stream));
+        if (desc) SSLPL_CUDA(cudaMemcpyAsync(desc, d_desc, (size_t)c2 * 32 * nframes, cudaMemcpyDeviceToHost, h->stream));
     } else for (int f = 0; f < nframes; f++) {
-        if (kps) SSLPL_CUDA(cudaMemcpyAsync(kps + (size_t)f * cap, d_kps + (size_t)f * c2, sizeof(sslpl_keypoint) * c2, cudaMemcpyDeviceToHost, h->s_orb));
-        if (kps_un) SSLPL_CUDA(cudaMemcpyAsync(kps_un + (size_t)f * cap, h->d_un + (size_t)f * c2, sizeof(sslpl_keypoint) * c2, cudaMemcpyDeviceToHost, h->s_orb));
-        if (desc) SSLPL_CUDA(cudaMemcpyAsync(desc + (size_t)f * cap * 32, d_desc + (size_t)f * c2 * 32, (size_t)c2 * 32, cudaMemcpyDeviceToHost, h->s_orb));
+        if (kps) SSLPL_CUDA(cudaMemcpyAsync(kps + (size_t)f * cap, d_kps + (size_t)f * c2, sizeof(sslpl_keypoint) * c2, cudaMemcpyDeviceToHost, h->stream));
+        if (kps_un) SSLPL_CUDA(cudaMemcpyAsync(kps_un + (size_t)f * cap, h->d_un + (size_t)f * c2, sizeof(sslpl_keypoint) * c2, cudaMemcpyDeviceToHost, h->stream));
+        if (desc) SSLPL_CUDA(cudaMemcpyAsync(desc + (size_t)f * cap * 32, d_desc + (size_t)f * c2 * 32, (size_t)c2 * 32, cudaMemcpyDeviceToHost, h->stream));
     }
     const sslpl_keyline* d_kl; const uint8_t* d_ld; const double* d_eq; const int* d_nl; int cl;
     rc = sslpl_line_device_results(h->line, &d_kl, &d_ld, &d_eq, &d_nl, &cl);

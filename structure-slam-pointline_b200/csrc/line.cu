@@ -1760,10 +1760,8 @@ __global__ void __launch_bounds__(64) k_lbd(const __grid_constant__ LineGeom g, 
 // =================================================================================================
 using namespace sslpl;
 
-struct sslpl_line {
+struct sslpl_line : sslpl::StreamHandle {
     sslpl_line_params p;
-    cudaStream_t stream = nullptr, own_stream = nullptr;
-    uint8_t* arena = nullptr; size_t arena_size = 0;
     LineGeom g; LineWs ws; LView view;
     uint8_t* d_input = nullptr;
     LbdCoef coef;
@@ -1774,20 +1772,9 @@ struct sslpl_line {
     int max_walkers = 0;        // 0 = one walker CTA per frame
     int walker_warps = 0;       // 0 = automatic (one warp or 16 warps per frame), -1 = one warp, 2..16 = a multi-warp CTA per frame
     int cur_w = 0, cur_h = 0, cur_frames = 0;
-    long long launches = 0;
-    int* h_err = nullptr;
-    bool profiling = false;
-    std::vector<cudaEvent_t> ev; std::vector<const char*> ev_name; int ev_n = 0;
 };
 
 namespace {
-
-void lmark(sslpl_line* h, const char* name) {
-    if (!h->profiling) return;
-    if ((int)h->ev.size() <= h->ev_n) { cudaEvent_t e; cudaEventCreate(&e); h->ev.push_back(e); h->ev_name.push_back(name); }
-    h->ev_name[h->ev_n] = name;
-    cudaEventRecord(h->ev[h->ev_n++], h->stream);
-}
 
 // gradient threshold of lsd.cpp: quant / sin(ang_th) with quant 2, ang_th 22.5 degrees
 double lsd_rho() { return 2.0 / std::sin(L_PI * 22.5 / 180); }
@@ -1887,13 +1874,13 @@ int run_pipeline(sslpl_line* h, int B) {
     const LineGeom& g = h->g;
     cudaStream_t st = h->stream;
     h->ev_n = 0;
-    lmark(h, "start");
+    h->mark("start");
     SSLPL_CUDA(cudaMemsetAsync(h->ws.maxgrad, 0, sizeof(unsigned long long) * B, st));
     SSLPL_CUDA(cudaMemsetAsync(h->ws.prep_next, 0, sizeof(int), st));
-    k_lsd_prep<<<std::min(h->prep_ctas, g.tiles_x * g.tiles_y * B), PT_NT, 0, st>>>(g, h->view, h->ws, B);      // blurs, resize, ll_angle, Sobel
-    lmark(h, "lsd_prep");
-    k_lsd_seeds<<<B, SEED_WARPS * 32, 0, st>>>(g, h->ws);
-    lmark(h, "lsd_seeds");
+    launch(h, k_lsd_prep, std::min(h->prep_ctas, g.tiles_x * g.tiles_y * B), PT_NT, 0, g, h->view, h->ws, B);      // blurs, resize, ll_angle, Sobel
+    h->mark("lsd_prep");
+    launch(h, k_lsd_seeds, B, SEED_WARPS * 32, 0, g, h->ws);
+    h->mark("lsd_seeds");
     SSLPL_CUDA(cudaMemsetAsync(h->ws.rejctl, 0, 4 * sizeof(int), st));
     SSLPL_CUDA(cudaMemsetAsync(h->ws.wstat, 0, 16 * sizeof(unsigned long long), st));
     {   // one CTA per frame; few frames -> more warps per frame (latency), many frames -> more CTAs per SM (throughput)
@@ -1903,52 +1890,32 @@ int run_pipeline(sslpl_line* h, int B) {
         const int grid = h->max_walkers > 0 ? std::min(B, h->max_walkers) : B;
         const size_t smem = (size_t)((g.pix_stride + 31) / 32) * sizeof(unsigned);
         if ((int)smem > h->used_smem) { SSLPL_CUDA(cudaFuncSetAttribute(k_lsd_regions, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); h->used_smem = (int)smem; }
-        if (ww == 0) k_lsd_regions_solo<<<grid, 32, 0, st>>>(g, h->ws, B);       // one warp per frame
-        else k_lsd_regions<<<grid, ww * 32, smem, st>>>(g, h->ws, B);
+        if (ww == 0) launch(h, k_lsd_regions_solo, grid, 32, 0, g, h->ws, B);       // one warp per frame
+        else launch(h, k_lsd_regions, grid, ww * 32, smem, g, h->ws, B);
     }
-    lmark(h, "lsd_regions");
-    k_lsd_nfa_count<<<dim3(NFA_COUNT_CTAS, B), 128, 0, st>>>(g, h->ws);
-    k_lsd_nfa_first<<<dim3(NFA_FIRST_CTAS, B), 128, 0, st>>>(g, h->ws);
-    k_lsd_nfa_improve<<<std::min(h->sm_count * 8, (B * 64 + 3) / 4), 128, 0, st>>>(g, h->ws);
-    lmark(h, "lsd_nfa");
-    k_keylines<<<B, 256, 0, st>>>(g, h->ws);
-    k_lbd<<<dim3(g.kl_cap, B), 64, 0, st>>>(g, h->ws, h->coef);
-    lmark(h, "keylines_lbd");
-    h->launches += 8;      // kernels only (the three small memsets are not counted)
+    h->mark("lsd_regions");
+    launch(h, k_lsd_nfa_count, dim3(NFA_COUNT_CTAS, B), 128, 0, g, h->ws);
+    launch(h, k_lsd_nfa_first, dim3(NFA_FIRST_CTAS, B), 128, 0, g, h->ws);
+    launch(h, k_lsd_nfa_improve, std::min(h->sm_count * 8, (B * 64 + 3) / 4), 128, 0, g, h->ws);
+    h->mark("lsd_nfa");
+    launch(h, k_keylines, B, 256, 0, g, h->ws);
+    launch(h, k_lbd, dim3(g.kl_cap, B), 64, 0, g, h->ws, h->coef);
+    h->mark("keylines_lbd");
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
 
-int check_device_err(sslpl_line* h) {
-    if (h->cur_w == 0) { SSLPL_CUDA(cudaStreamSynchronize(h->stream)); return SSLPL_OK; }     // never used yet: no workspace, nothing to report
-    SSLPL_CUDA(cudaMemcpyAsync(h->h_err, h->ws.err, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
-    if (*h->h_err) {
-        set_error("device-side capacity overflow in the line path, flags=0x%x", *h->h_err);
-        cudaMemsetAsync(h->ws.err, 0, sizeof(int), h->stream);
-        return SSLPL_ERR_CAPACITY;
-    }
-    return SSLPL_OK;
-}
+// ws.err is null until the first configure: a handle that has not run has nothing to report
+int line_sync(sslpl_line* h) { return h->sync(h->ws.err, "the line path"); }
 
-}  // namespace
-
-extern "C" {
-
-int sslpl_line_create(const sslpl_line_params* p, sslpl_line** out) {
-    SSLPL_REQUIRE(p && out, SSLPL_ERR_ARG, "null argument");
-    SSLPL_REQUIRE(p->lsdNFeatures >= 1 && p->lsdNFeatures <= 65536, SSLPL_ERR_ARG, "lsdNFeatures out of range");
-    SSLPL_REQUIRE(p->max_batch >= 1 && p->max_width >= 16 && p->max_height >= 16, SSLPL_ERR_ARG, "bad max_batch / max size");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { set_error("no CUDA device available: libsslpl_b200 has no CPU fallback"); return SSLPL_ERR_CUDA; }
-    SSLPL_CUDA(cudaSetDevice(p->device));
-    sslpl_line* h = new sslpl_line();
-    h->p = *p;
+int line_init(sslpl_line* h) {
+    const sslpl_line_params* p = &h->p;
+    if (int rc = h->open(p->device)) return rc;
     { int v = 0; if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, p->device) == cudaSuccess && v > 0) h->sm_count = v; }
     {   // the persistent pre-pass fills the device once; tiles beyond that are taken from its counter
         int occ = 0;
         const cudaError_t oe = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_lsd_prep, PT_NT, 0);
-        if (oe != cudaSuccess || occ < 1) { set_error("k_lsd_prep occupancy query failed: %s", cudaGetErrorString(oe)); delete h; return SSLPL_ERR_CUDA; }
+        if (oe != cudaSuccess || occ < 1) { set_error("k_lsd_prep occupancy query failed: %s", cudaGetErrorString(oe)); return SSLPL_ERR_CUDA; }
         h->prep_ctas = occ * h->sm_count;
     }
     h->trace = getenv("SSLPL_LINE_TRACE") != nullptr;
@@ -1962,38 +1929,34 @@ int sslpl_line_create(const sslpl_line_params* p, sslpl_line** out) {
     LineGeom g;
     make_geometry(h, p->max_width, p->max_height, g, nullptr);
     Arena A; carve(h, A, g, p->max_batch);
-    h->arena_size = A.used + (1 << 20);
-    cudaError_t e = cudaMalloc(&h->arena, h->arena_size);
-    if (e != cudaSuccess) { set_error("cudaMalloc(%zu) failed: %s", h->arena_size, cudaGetErrorString(e)); delete h; return SSLPL_ERR_CUDA; }
-    SSLPL_CUDA(cudaMemset(h->arena, 0, h->arena_size));
-    SSLPL_CUDA(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
-    h->stream = h->own_stream;
-    SSLPL_CUDA(cudaHostAlloc((void**)&h->h_err, sizeof(int), cudaHostAllocDefault));
+    return h->alloc_arena(A.used + (1 << 20));
+}
+
+}  // namespace
+
+extern "C" {
+
+int sslpl_line_create(const sslpl_line_params* p, sslpl_line** out) {
+    SSLPL_REQUIRE(p && out, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(p->lsdNFeatures >= 1 && p->lsdNFeatures <= 65536, SSLPL_ERR_ARG, "lsdNFeatures out of range");
+    SSLPL_REQUIRE(p->max_batch >= 1 && p->max_width >= 16 && p->max_height >= 16, SSLPL_ERR_ARG, "bad max_batch / max size");
+    sslpl_line* h = new sslpl_line();
+    h->p = *p;
+    const int rc = line_init(h);
+    if (rc != SSLPL_OK) { sslpl_line_destroy(h); return rc; }
     *out = h;
     return SSLPL_OK;
 }
 
 void sslpl_line_destroy(sslpl_line* h) {
     if (!h) return;
-    cudaSetDevice(h->p.device);
-    // an external stream may already be gone (its owner was destroyed first): never touch it here
-    if (h->stream && h->stream == h->own_stream) cudaStreamSynchronize(h->own_stream); else cudaDeviceSynchronize();
-    if (h->own_stream) cudaStreamDestroy(h->own_stream);
-    for (auto e : h->ev) cudaEventDestroy(e);
-    if (h->arena) cudaFree(h->arena);
-    if (h->h_err) cudaFreeHost(h->h_err);
+    h->close();
     delete h;
 }
 
-int sslpl_line_sync(sslpl_line* h) { SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle"); SSLPL_CUDA(cudaSetDevice(h->p.device)); return check_device_err(h); }
+int sslpl_line_sync(sslpl_line* h) { SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle"); return line_sync(h); }
 void* sslpl_line_stream(sslpl_line* h) { return h ? (void*)h->stream : nullptr; }
-int sslpl_line_set_stream(sslpl_line* h, void* s) {
-    SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle");
-    SSLPL_CUDA(cudaSetDevice(h->p.device));
-    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
-    h->stream = s ? (cudaStream_t)s : h->own_stream;
-    return SSLPL_OK;
-}
+int sslpl_line_set_stream(sslpl_line* h, void* s) { SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle"); return h->set_stream(s); }
 long long sslpl_line_launch_count(const sslpl_line* h) { return h ? h->launches : 0; }
 int sslpl_line_set_max_walkers(sslpl_line* h, int max_concurrent) {
     SSLPL_REQUIRE(h && max_concurrent >= 0, SSLPL_ERR_ARG, "bad argument");
@@ -2001,15 +1964,7 @@ int sslpl_line_set_max_walkers(sslpl_line* h, int max_concurrent) {
     return SSLPL_OK;
 }
 int sslpl_line_set_profiling(sslpl_line* h, int on) { SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle"); h->profiling = on != 0; return SSLPL_OK; }
-int sslpl_line_stage_ms(sslpl_line* h, float* ms, int cap, const char** names, int* nstages) {
-    SSLPL_REQUIRE(h && nstages, SSLPL_ERR_ARG, "null argument");
-    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
-    int k = 0;
-    for (int i = 1; i < h->ev_n; i++, k++)
-        if (k < cap) { float t = 0; cudaEventElapsedTime(&t, h->ev[i - 1], h->ev[i]); if (ms) ms[k] = t; if (names) names[k] = h->ev_name[i]; }
-    *nstages = k;
-    return SSLPL_OK;
-}
+int sslpl_line_stage_ms(sslpl_line* h, float* ms, int cap, const char** names, int* nstages) { SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle"); return h->stage_ms(ms, cap, names, nstages); }
 
 int sslpl_line_extract_batch_device(sslpl_line* h, const uint8_t* d_imgs, int nframes, int width, int height, int pitch, size_t frame_stride) {
     SSLPL_REQUIRE(h && d_imgs, SSLPL_ERR_ARG, "null argument");
@@ -2041,11 +1996,8 @@ int sslpl_line_extract_batch_begin(sslpl_line* h, const uint8_t* imgs, int nfram
     int rc = configure(h, width, height);
     if (rc) return rc;
     const LineGeom& g = h->g;
-    if (frame_stride == (size_t)pitch * height)
-        SSLPL_CUDA(cudaMemcpy2DAsync(h->d_input, g.pitch, imgs, pitch, width, (size_t)height * nframes, cudaMemcpyHostToDevice, h->stream));
-    else
-        for (int f = 0; f < nframes; f++)
-            SSLPL_CUDA(cudaMemcpy2DAsync(h->d_input + f * g.in_stride, g.pitch, imgs + f * frame_stride, pitch, width, height, cudaMemcpyHostToDevice, h->stream));
+    rc = h->upload_frames(h->d_input, g.pitch, g.in_stride, imgs, pitch, frame_stride, width, height, nframes);
+    if (rc) return rc;
     h->view.base = h->d_input; h->view.pitch = g.pitch; h->view.frame_stride = g.in_stride;
     h->cur_frames = nframes;
     rc = run_pipeline(h, nframes);
@@ -2062,7 +2014,7 @@ int sslpl_line_extract_batch(sslpl_line* h, const uint8_t* imgs, int nframes, in
                              sslpl_keyline* kl, uint8_t* ldesc, double* lineeq, int cap, int* n) {
     int rc = sslpl_line_extract_batch_begin(h, imgs, nframes, width, height, pitch, frame_stride, kl, ldesc, lineeq, cap, n);
     if (rc) return rc;
-    return check_device_err(h);
+    return line_sync(h);
 }
 
 int sslpl_line_extract(sslpl_line* h, const uint8_t* img, int width, int height, int pitch, sslpl_keyline* kl, uint8_t* ldesc, double* lineeq, int cap, int* n) {
@@ -2116,23 +2068,17 @@ int sslpl_line_download_prep(sslpl_line* h, int frame, int* w, int* hgt, int* sw
 int sslpl_line_debug_ll_table(sslpl_line* h, float* angdeg, float* cs, float* cs0, double* modgrad) {
     SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle");
     SSLPL_CUDA(cudaSetDevice(h->p.device));
-    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
     constexpr size_t N = (size_t)LL_SPAN * LL_SPAN;
-    uint8_t* buf = nullptr;
-    SSLPL_CUDA(cudaMalloc(&buf, N * (sizeof(float) + 2 * sizeof(float2) + sizeof(double))));
-    double* d_norm = reinterpret_cast<double*>(buf);
-    float2* d_cs = reinterpret_cast<float2*>(d_norm + N);
-    float2* d_cs0 = d_cs + N;
-    float* d_ang = reinterpret_cast<float*>(d_cs0 + N);
-    k_ll_table<<<(unsigned)((N + 255) / 256), 256, 0, h->stream>>>(lsd_rho(), d_ang, d_cs, d_cs0, d_norm);
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    if (e == cudaSuccess && angdeg) e = cudaMemcpy(angdeg, d_ang, N * sizeof(float), cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && cs) e = cudaMemcpy(cs, d_cs, N * sizeof(float2), cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && cs0) e = cudaMemcpy(cs0, d_cs0, N * sizeof(float2), cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && modgrad) e = cudaMemcpy(modgrad, d_norm, N * sizeof(double), cudaMemcpyDeviceToHost);
-    cudaFree(buf);
-    SSLPL_CUDA(e);
+    if (int rc = ensure_scratch(h, N * (sizeof(float) + 2 * sizeof(float2) + sizeof(double)) + 1024)) return rc;
+    Arena A; A.base = h->scratch;
+    double* d_norm = A.take<double>(N); float2* d_cs = A.take<float2>(N); float2* d_cs0 = A.take<float2>(N); float* d_ang = A.take<float>(N);
+    launch(h, k_ll_table, (unsigned)((N + 255) / 256), 256, 0, lsd_rho(), d_ang, d_cs, d_cs0, d_norm);
+    SSLPL_CUDA(cudaGetLastError());
+    if (angdeg) SSLPL_CUDA(cudaMemcpyAsync(angdeg, d_ang, N * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    if (cs) SSLPL_CUDA(cudaMemcpyAsync(cs, d_cs, N * sizeof(float2), cudaMemcpyDeviceToHost, h->stream));
+    if (cs0) SSLPL_CUDA(cudaMemcpyAsync(cs0, d_cs0, N * sizeof(float2), cudaMemcpyDeviceToHost, h->stream));
+    if (modgrad) SSLPL_CUDA(cudaMemcpyAsync(modgrad, d_norm, N * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
     return SSLPL_OK;
 }
 
@@ -2144,25 +2090,18 @@ int sslpl_line_debug_nfa(sslpl_line* h, int width, int height, int n, const int*
     const long long lg_size = h->g.pix_stride + 2;
     for (int i = 0; i < n; i++) SSLPL_REQUIRE(K[i] >= 0 && K[i] <= N[i] && N[i] < lg_size, SSLPL_ERR_ARG, "(n, k) outside 0 <= k <= n < lgam size");
     if (n == 0) return SSLPL_OK;
-    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
-    uint8_t* buf = nullptr;
-    SSLPL_CUDA(cudaMalloc(&buf, (size_t)n * (2 * sizeof(double) + 3 * sizeof(int))));
-    double* d_p = reinterpret_cast<double*>(buf); double* d_out = d_p + n;
-    int* d_n = reinterpret_cast<int*>(d_out + n); int* d_k = d_n + n; int* d_stop = d_k + n;
-    cudaError_t e = cudaMemcpy(d_p, P, (size_t)n * sizeof(double), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(d_n, N, (size_t)n * sizeof(int), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(d_k, K, (size_t)n * sizeof(int), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) {
-        const unsigned blocks = (unsigned)((n + 127) / 128);
-        if (plain) k_dbg_nfa<true><<<blocks, 128, 0, h->stream>>>(n, d_n, d_k, d_p, h->g.log_nt, h->ws.lgam, d_out, stop ? d_stop : nullptr);
-        else k_dbg_nfa<false><<<blocks, 128, 0, h->stream>>>(n, d_n, d_k, d_p, h->g.log_nt, h->ws.lgam, d_out, stop ? d_stop : nullptr);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    if (e == cudaSuccess) e = cudaMemcpy(out, d_out, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && stop) e = cudaMemcpy(stop, d_stop, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost);
-    cudaFree(buf);
+    if (int rc2 = ensure_scratch(h, (size_t)n * (2 * sizeof(double) + 3 * sizeof(int)) + 2048)) return rc2;
+    Arena A; A.base = h->scratch;
+    cudaError_t e = cudaSuccess;
+    const double* d_p = stage(A, P, n, h->stream, e); const int* d_n = stage(A, N, n, h->stream, e); const int* d_k = stage(A, K, n, h->stream, e);
+    double* d_out = A.take<double>(n); int* d_stop = A.take<int>(n);
     SSLPL_CUDA(e);
+    launch(h, plain ? k_dbg_nfa<true> : k_dbg_nfa<false>, (unsigned)((n + 127) / 128), 128, 0, n, d_n, d_k, d_p, h->g.log_nt, h->ws.lgam, d_out,
+           stop ? d_stop : nullptr);
+    SSLPL_CUDA(cudaGetLastError());
+    SSLPL_CUDA(cudaMemcpyAsync(out, d_out, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    if (stop) SSLPL_CUDA(cudaMemcpyAsync(stop, d_stop, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
     return SSLPL_OK;
 }
 
@@ -2170,19 +2109,16 @@ int sslpl_line_debug_sincos(sslpl_line* h, int n, const double* x, int full, dou
     SSLPL_REQUIRE(h && n >= 0 && (n == 0 || (x && s && c)), SSLPL_ERR_ARG, "bad argument");
     if (n == 0) return SSLPL_OK;
     SSLPL_CUDA(cudaSetDevice(h->p.device));
-    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
-    double* buf = nullptr;
-    SSLPL_CUDA(cudaMalloc(&buf, (size_t)n * 3 * sizeof(double)));
-    cudaError_t e = cudaMemcpy(buf, x, (size_t)n * sizeof(double), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) {
-        k_dbg_sincos<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(n, buf, full, buf + n, buf + 2 * (size_t)n);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    if (e == cudaSuccess) e = cudaMemcpy(s, buf + n, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) e = cudaMemcpy(c, buf + 2 * (size_t)n, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost);
-    cudaFree(buf);
+    if (int rc = ensure_scratch(h, (size_t)n * 3 * sizeof(double) + 1024)) return rc;
+    Arena A; A.base = h->scratch;
+    cudaError_t e = cudaSuccess;
+    const double* d_x = stage(A, x, n, h->stream, e); double* d_s = A.take<double>(n); double* d_c = A.take<double>(n);
     SSLPL_CUDA(e);
+    launch(h, k_dbg_sincos, (unsigned)((n + 127) / 128), 128, 0, n, d_x, full, d_s, d_c);
+    SSLPL_CUDA(cudaGetLastError());
+    SSLPL_CUDA(cudaMemcpyAsync(s, d_s, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    SSLPL_CUDA(cudaMemcpyAsync(c, d_c, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
     return SSLPL_OK;
 }
 
@@ -2190,19 +2126,15 @@ int sslpl_line_debug_atan2(sslpl_line* h, int n, const float* y, const float* x,
     SSLPL_REQUIRE(h && n >= 0 && (n == 0 || (x && y && out)), SSLPL_ERR_ARG, "bad argument");
     if (n == 0) return SSLPL_OK;
     SSLPL_CUDA(cudaSetDevice(h->p.device));
-    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
-    float* buf = nullptr;
-    SSLPL_CUDA(cudaMalloc(&buf, (size_t)n * 3 * sizeof(float)));
-    cudaError_t e = cudaMemcpy(buf, y, (size_t)n * sizeof(float), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(buf + n, x, (size_t)n * sizeof(float), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) {
-        k_dbg_atan2<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(n, buf, buf + n, buf + 2 * (size_t)n);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    if (e == cudaSuccess) e = cudaMemcpy(out, buf + 2 * (size_t)n, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost);
-    cudaFree(buf);
+    if (int rc = ensure_scratch(h, (size_t)n * 3 * sizeof(float) + 1024)) return rc;
+    Arena A; A.base = h->scratch;
+    cudaError_t e = cudaSuccess;
+    const float* d_y = stage(A, y, n, h->stream, e); const float* d_x = stage(A, x, n, h->stream, e); float* d_out = A.take<float>(n);
     SSLPL_CUDA(e);
+    launch(h, k_dbg_atan2, (unsigned)((n + 127) / 128), 128, 0, n, d_y, d_x, d_out);
+    SSLPL_CUDA(cudaGetLastError());
+    SSLPL_CUDA(cudaMemcpyAsync(out, d_out, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
     return SSLPL_OK;
 }
 

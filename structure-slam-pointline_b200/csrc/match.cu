@@ -1495,16 +1495,13 @@ struct sslpl_vocab {
     std::vector<int> level_count;        // nodes per depth
 };
 
-struct sslpl_matcher {
+struct sslpl_matcher : sslpl::StreamHandle {
     sslpl_matcher_params p;
-    cudaStream_t stream = nullptr, own_stream = nullptr;
-    uint8_t* arena = nullptr; size_t arena_size = 0;
     int cap = 0;                     // rows per frame slot of the single-call staging (max(features, lines))
     // single-call staging: 2 frame slots
     uint8_t* desc; int* nodes; int* off; int* idx; uint8_t* flag; float* kpf; int* nn2; int* ncnt;
     int32_t* out; uint8_t* rot; uint8_t* taken; int32_t* pairs; int32_t* nmatch; int32_t* knn; uint8_t* cent; int32_t* node;
     int32_t* word; double* wgt;      // per-feature outputs of the vocabulary transform (single-call staging)
-    uint8_t* scratch = nullptr; size_t scratch_size = 0;   // grow-only scratch of sslpl_descriptor_medoid_batch
     // batch workspace
     int32_t* b_node; int* b_off; int* b_idx; uint8_t* b_rot; uint8_t* b_taken; int32_t* b_knn; int* iota;
     // workspace of sslpl_search_by_projection_frame_batch_device, allocated by its first call: per frame the grid cell of every
@@ -1515,8 +1512,6 @@ struct sslpl_matcher {
     int32_t* tw = nullptr;
     // per-pair row table of sslpl_create_new_map_lines_batch_device ([max_batch][max_lines + 64]), allocated by its first call
     int32_t* ltw = nullptr;
-    int32_t* h_small = nullptr;      // pinned scratch
-    long long launches = 0;
 };
 
 namespace {
@@ -1539,29 +1534,6 @@ int carve(sslpl_matcher* m, Arena& A) {
     m->b_knn = A.take<int32_t>((size_t)B * lc * 4);
     m->iota = A.take<int>(NN);
     return 0;
-}
-
-// carve `count` elements out of a scratch arena and start their upload
-template <class T> T* stage(Arena& A, const T* host, size_t count, cudaStream_t st, cudaError_t& err) {
-    T* d = A.take<T>(count + 8);
-    if (host && count && err == cudaSuccess) err = cudaMemcpyAsync(d, host, sizeof(T) * count, cudaMemcpyHostToDevice, st);
-    return d;
-}
-
-// every kernel launch of the matcher: on its stream, counted by sslpl_matcher_launch_count
-template <class T> struct same_type { using type = T; };
-template <class... KArgs>
-void launch(sslpl_matcher* m, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, typename same_type<KArgs>::type... args) {
-    kernel<<<grid, block, smem, m->stream>>>(args...);
-    m->launches++;
-}
-
-// a workspace of the handle allocated by the first call that needs it (a handle that never gets there never pays for it), freed with it
-template <class T> int first_use(T*& p, size_t bytes) {
-    if (p) return SSLPL_OK;
-    cudaError_t e = cudaMalloc(&p, bytes);
-    if (e != cudaSuccess) { p = nullptr; set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return SSLPL_ERR_CUDA; }
-    return SSLPL_OK;
 }
 
 int featvec_ok(const sslpl_matcher* m, const sslpl_featvec* fv, int n) {
@@ -1760,6 +1732,20 @@ void line_mad(const int32_t* knn, int nq, double* nn_mad, double* nn12_mad) {
     *nn12_mad = 1.4826 * a[nq / 2];
 }
 
+int matcher_init(sslpl_matcher* m) {
+    if (int rc = m->open(m->p.device)) return rc;
+    Arena A; carve(m, A);
+    if (int rc = m->alloc_arena(A.used + (1 << 16))) return rc;
+    Arena B; B.base = m->arena; B.size = m->arena_size; carve(m, B);
+    std::vector<int> iota(m->p.max_nodes + 1);
+    for (int i = 0; i <= m->p.max_nodes; i++) iota[i] = i;
+    SSLPL_CUDA(cudaMemcpy(m->iota, iota.data(), sizeof(int) * iota.size(), cudaMemcpyHostToDevice));
+    // the two kernels with data-dependent dynamic shared memory may use the whole 227 KB of an sm_90 CTA
+    SSLPL_CUDA(cudaFuncSetAttribute(k_bow_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
+    SSLPL_CUDA(cudaFuncSetAttribute(k_build_csr, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
+    return SSLPL_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1770,63 +1756,27 @@ int sslpl_matcher_create(const sslpl_matcher_params* p, sslpl_matcher** out) {
     SSLPL_REQUIRE(p && out, SSLPL_ERR_ARG, "null argument");
     SSLPL_REQUIRE(p->max_features >= 1 && p->max_lines >= 0 && p->max_nodes >= 1 && p->max_batch >= 1, SSLPL_ERR_ARG, "bad matcher capacity");
     SSLPL_REQUIRE(p->max_features < (1 << 20) && p->max_lines < (1 << 20), SSLPL_ERR_ARG, "capacity too large");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { set_error("no CUDA device available: libsslpl_b200 has no CPU fallback"); return SSLPL_ERR_CUDA; }
-    SSLPL_CUDA(cudaSetDevice(p->device));
     sslpl_matcher* m = new sslpl_matcher();
     m->p = *p;
     m->cap = std::max(p->max_features, p->max_lines) + 64;
-    Arena A; carve(m, A);
-    m->arena_size = A.used + (1 << 16);
-    cudaError_t e = cudaMalloc(&m->arena, m->arena_size);
-    if (e != cudaSuccess) { set_error("cudaMalloc(%zu) failed: %s", m->arena_size, cudaGetErrorString(e)); delete m; return SSLPL_ERR_CUDA; }
-    cudaError_t e2 = cudaMemset(m->arena, 0, m->arena_size);
-    Arena B; B.base = m->arena; B.size = m->arena_size; carve(m, B);
-    if (e2 == cudaSuccess) e2 = cudaStreamCreateWithFlags(&m->own_stream, cudaStreamNonBlocking);
-    m->stream = m->own_stream;
-    if (e2 == cudaSuccess) e2 = cudaHostAlloc((void**)&m->h_small, 64 * sizeof(int32_t), cudaHostAllocDefault);
-    if (e2 == cudaSuccess) {
-        std::vector<int> iota(p->max_nodes + 1);
-        for (int i = 0; i <= p->max_nodes; i++) iota[i] = i;
-        e2 = cudaMemcpy(m->iota, iota.data(), sizeof(int) * iota.size(), cudaMemcpyHostToDevice);
-    }
-    // the two kernels with data-dependent dynamic shared memory may use the whole 227 KB of an sm_90 CTA
-    if (e2 == cudaSuccess) e2 = cudaFuncSetAttribute(k_bow_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM);
-    if (e2 == cudaSuccess) e2 = cudaFuncSetAttribute(k_build_csr, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM);
-    if (e2 != cudaSuccess) { set_error("sslpl_matcher_create: %s", cudaGetErrorString(e2)); sslpl_matcher_destroy(m); return SSLPL_ERR_CUDA; }
+    const int rc = matcher_init(m);
+    if (rc != SSLPL_OK) { sslpl_matcher_destroy(m); return rc; }
     *out = m;
     return SSLPL_OK;
 }
 
 void sslpl_matcher_destroy(sslpl_matcher* m) {
     if (!m) return;
-    cudaSetDevice(m->p.device);
-    // an external stream may already be gone (its owner was destroyed first): never touch it here
-    if (m->stream && m->stream == m->own_stream) cudaStreamSynchronize(m->own_stream); else cudaDeviceSynchronize();
-    if (m->own_stream) cudaStreamDestroy(m->own_stream);
-    if (m->arena) cudaFree(m->arena);
-    if (m->scratch) cudaFree(m->scratch);
+    m->close();
     if (m->pw) cudaFree(m->pw);
     if (m->tw) cudaFree(m->tw);
     if (m->ltw) cudaFree(m->ltw);
-    if (m->h_small) cudaFreeHost(m->h_small);
     delete m;
 }
 
-int sslpl_matcher_sync(sslpl_matcher* m) {
-    SSLPL_REQUIRE(m, SSLPL_ERR_ARG, "null handle");
-    SSLPL_CUDA(cudaSetDevice(m->p.device));
-    SSLPL_CUDA(cudaStreamSynchronize(m->stream));
-    return SSLPL_OK;
-}
+int sslpl_matcher_sync(sslpl_matcher* m) { SSLPL_REQUIRE(m, SSLPL_ERR_ARG, "null handle"); return m->sync(nullptr, nullptr); }
 void* sslpl_matcher_stream(sslpl_matcher* m) { return m ? (void*)m->stream : nullptr; }
-int sslpl_matcher_set_stream(sslpl_matcher* m, void* cuda_stream) {
-    SSLPL_REQUIRE(m, SSLPL_ERR_ARG, "null handle");
-    SSLPL_CUDA(cudaSetDevice(m->p.device));
-    SSLPL_CUDA(cudaStreamSynchronize(m->stream));
-    m->stream = cuda_stream ? (cudaStream_t)cuda_stream : m->own_stream;
-    return SSLPL_OK;
-}
+int sslpl_matcher_set_stream(sslpl_matcher* m, void* cuda_stream) { SSLPL_REQUIRE(m, SSLPL_ERR_ARG, "null handle"); return m->set_stream(cuda_stream); }
 long long sslpl_matcher_launch_count(const sslpl_matcher* m) { return m ? m->launches : 0; }
 
 int sslpl_descriptor_distance(sslpl_matcher* m, const uint8_t* a, const uint8_t* b, int n, int32_t* dist) {
@@ -2215,16 +2165,6 @@ int sslpl_search_for_initialization(sslpl_matcher* m,
 // device consumer.  (The per-frame grid build is k_grid_cells + k_build_csr.)
 
 // ---------------- line projection search and Fuse search (SURVEY.md 8(f) row 3) ----------------
-static int ensure_scratch(sslpl_matcher* m, size_t need) {           // grow-only scratch shared by the entry points below
-    if (need <= m->scratch_size) return SSLPL_OK;
-    SSLPL_CUDA(cudaStreamSynchronize(m->stream));
-    if (m->scratch) cudaFree(m->scratch);
-    m->scratch = nullptr; m->scratch_size = 0;
-    cudaError_t e = cudaMalloc(&m->scratch, need);
-    if (e != cudaSuccess) { set_error("cudaMalloc(%zu) failed: %s", need, cudaGetErrorString(e)); return SSLPL_ERR_CUDA; }
-    m->scratch_size = need;
-    return SSLPL_OK;
-}
 
 int sslpl_line_search_by_projection(sslpl_matcher* m, int nml, const uint8_t* active, const uint8_t* obs, const float* proj, const float* radius,
                                     const int32_t* minLevel, const int32_t* maxLevel, const uint8_t* dml,

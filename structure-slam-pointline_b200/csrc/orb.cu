@@ -801,19 +801,13 @@ __global__ void __launch_bounds__(256) k_orient_desc(const __grid_constant__ Orb
 // =================================================================================================
 using namespace sslpl;
 
-struct sslpl_orb {
+struct sslpl_orb : sslpl::StreamHandle {
     sslpl_orb_params p;
     std::vector<float> scale, invscale, sigma2, invsigma2;
     std::vector<int> nfeat, umax;
-    cudaStream_t stream = nullptr, own_stream = nullptr;
-    uint8_t* arena = nullptr; size_t arena_size = 0;
     OrbGeom g; OrbWs ws; View view;
     uint8_t* d_input = nullptr;         // staging for host frames
     int cur_w = 0, cur_h = 0, cur_frames = 0;
-    long long launches = 0;
-    bool profiling = false;
-    std::vector<cudaEvent_t> ev; std::vector<const char*> ev_name; int ev_n = 0;
-    int* h_err = nullptr;               // pinned
     int octree_smem = 0;
     TMaps tm;                           // per-level tensor maps (level 0 re-encoded per call: the input view moves)
     PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
@@ -975,19 +969,12 @@ int configure(sslpl_orb* h, int W, int H) {
     return SSLPL_OK;
 }
 
-void mark(sslpl_orb* h, const char* name) {
-    if (!h->profiling) return;
-    if ((int)h->ev.size() <= h->ev_n) { cudaEvent_t e; cudaEventCreate(&e); h->ev.push_back(e); h->ev_name.push_back(name); }
-    h->ev_name[h->ev_n] = name;
-    cudaEventRecord(h->ev[h->ev_n++], h->stream);
-}
-
 // Enqueue the whole extraction for B frames described by `view`.
 int run_pipeline(sslpl_orb* h, int B) {
     const OrbGeom& g = h->g;
     cudaStream_t st = h->stream;
     h->ev_n = 0;
-    mark(h, "start");
+    h->mark("start");
     bool tma = h->use_tma && h->tma_levels_ok;
     if (tma && !(h->tm0_base == h->view.base && h->tm0_pitch == h->view.pitch && h->tm0_fs == h->view.frame_stride && h->tm0_frames >= B)) {
         // level 0 is the caller's buffer: (re-)encode its maps when the view moves
@@ -997,37 +984,41 @@ int run_pipeline(sslpl_orb* h, int B) {
             h->tm0_base = h->view.base; h->tm0_pitch = h->view.pitch; h->tm0_fs = h->view.frame_stride; h->tm0_frames = B;
         } else h->tm0_base = nullptr;
     }
-    for (int l = 1; l < g.nlevels; l++) {
-        dim3 grid((g.lv[l].w + 127) / 128, (g.lv[l].h + 7) / 8, B), block(32, 8);
-        k_resize<<<grid, block, 0, st>>>(g, h->ws, h->view, l);
-        h->launches++;
-    }
-    mark(h, "pyramid");
-    if (g.total_cells > 0) {
-        if (tma) k_fast<true><<<dim3(g.total_cells, B), 128, 0, st>>>(g, h->ws, h->view, h->ws.tmaps);
-        else k_fast<false><<<dim3(g.total_cells, B), 128, 0, st>>>(g, h->ws, h->view, h->ws.tmaps);
-        h->launches++;
-    }
-    mark(h, "fast");
-    k_octree<<<dim3(g.nlevels, B), 256, h->octree_smem, st>>>(g, h->ws); h->launches++;
-    mark(h, "octree");
-    if (tma) k_blur<true><<<dim3(g.total_tiles, B), 256, 0, st>>>(g, h->ws, h->view, h->ws.tmaps);
-    else k_blur<false><<<dim3(g.total_tiles, B), 256, 0, st>>>(g, h->ws, h->view, h->ws.tmaps);
-    h->launches++;
-    mark(h, "blur");
-    k_orient_desc<<<dim3((g.kp_total_cap + 7) / 8, B), 256, 0, st>>>(g, h->ws, h->view); h->launches++;
-    mark(h, "orient_desc");
+    for (int l = 1; l < g.nlevels; l++)
+        launch(h, k_resize, dim3((g.lv[l].w + 127) / 128, (g.lv[l].h + 7) / 8, B), dim3(32, 8), 0, g, h->ws, h->view, l);
+    h->mark("pyramid");
+    if (g.total_cells > 0) launch(h, tma ? k_fast<true> : k_fast<false>, dim3(g.total_cells, B), 128, 0, g, h->ws, h->view, h->ws.tmaps);
+    h->mark("fast");
+    launch(h, k_octree, dim3(g.nlevels, B), 256, h->octree_smem, g, h->ws);
+    h->mark("octree");
+    launch(h, tma ? k_blur<true> : k_blur<false>, dim3(g.total_tiles, B), 256, 0, g, h->ws, h->view, h->ws.tmaps);
+    h->mark("blur");
+    launch(h, k_orient_desc, dim3((g.kp_total_cap + 7) / 8, B), 256, 0, g, h->ws, h->view);
+    h->mark("orient_desc");
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
 
-int check_device_err(sslpl_orb* h) {
-    SSLPL_CUDA(cudaMemcpyAsync(h->h_err, h->ws.err, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
-    if (*h->h_err) {
-        set_error("device-side capacity overflow, flags=0x%x (1 pool, 2 keys, 4 sort, 8 keypoints)", *h->h_err);
-        cudaMemsetAsync(h->ws.err, 0, sizeof(int), h->stream);
-        return SSLPL_ERR_CAPACITY;
+// ws.err is null until the first configure: a handle that has not run has nothing to report
+int orb_sync(sslpl_orb* h) { return h->sync(h->ws.err, "the ORB path (1 pool, 2 keys, 4 sort, 8 keypoints)"); }
+
+int orb_init(sslpl_orb* h) {
+    const sslpl_orb_params* p = &h->p;
+    if (int rc = h->open(p->device)) return rc;
+    make_tables(h);
+    OrbGeom g;
+    make_geometry(h, p->max_width, p->max_height, g, nullptr);
+    SSLPL_REQUIRE(g.sort_cap * 8 <= 200 * 1024, SSLPL_ERR_UNSUPPORTED, "nfeatures too large for the octree sort buffer");
+    Arena A;                                   // dry run for the size
+    carve(h, A, g, p->max_batch, p->max_width, p->max_height);
+    if (int rc = h->alloc_arena(A.used + (1 << 20))) return rc;
+    {   // TMA descriptors are encoded by the driver; resolve the entry point through the runtime (no libcuda link)
+        void* fn = nullptr; cudaDriverEntryPointQueryResult qres;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
+            h->encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
+        else cudaGetLastError();
+        const char* e = getenv("SSLPL_NO_TMA");
+        h->use_tma = !(e && e[0] == '1');
     }
     return SSLPL_OK;
 }
@@ -1043,48 +1034,17 @@ int sslpl_orb_create(const sslpl_orb_params* p, sslpl_orb** out) {
     SSLPL_REQUIRE(p->scaleFactor > 1.0f, SSLPL_ERR_ARG, "scaleFactor must be > 1");
     SSLPL_REQUIRE(p->minThFAST >= 1 && p->iniThFAST >= p->minThFAST && p->iniThFAST < 255, SSLPL_ERR_ARG, "need 1 <= minThFAST <= iniThFAST < 255");
     SSLPL_REQUIRE(p->max_batch >= 1 && p->max_width >= 2 * EDGE && p->max_height >= 2 * EDGE, SSLPL_ERR_ARG, "bad max_batch / max size");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
-        set_error("no CUDA device available: libsslpl_b200 has no CPU fallback");
-        return SSLPL_ERR_CUDA;
-    }
-    SSLPL_CUDA(cudaSetDevice(p->device));
     sslpl_orb* h = new sslpl_orb();
     h->p = *p;
-    make_tables(h);
-    OrbGeom g;
-    make_geometry(h, p->max_width, p->max_height, g, nullptr);
-    SSLPL_REQUIRE(g.sort_cap * 8 <= 200 * 1024, SSLPL_ERR_UNSUPPORTED, "nfeatures too large for the octree sort buffer");
-    Arena A;                                   // dry run for the size
-    carve(h, A, g, p->max_batch, p->max_width, p->max_height);
-    h->arena_size = A.used + (1 << 20);
-    cudaError_t e = cudaMalloc(&h->arena, h->arena_size);
-    if (e != cudaSuccess) { set_error("cudaMalloc(%zu) failed: %s", h->arena_size, cudaGetErrorString(e)); delete h; return SSLPL_ERR_CUDA; }
-    SSLPL_CUDA(cudaMemset(h->arena, 0, h->arena_size));
-    SSLPL_CUDA(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
-    h->stream = h->own_stream;
-    SSLPL_CUDA(cudaHostAlloc((void**)&h->h_err, sizeof(int), cudaHostAllocDefault));
-    {   // TMA descriptors are encoded by the driver; resolve the entry point through the runtime (no libcuda link)
-        void* fn = nullptr; cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-            h->encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
-        else cudaGetLastError();
-        const char* e = getenv("SSLPL_NO_TMA");
-        h->use_tma = !(e && e[0] == '1');
-    }
+    const int rc = orb_init(h);
+    if (rc != SSLPL_OK) { sslpl_orb_destroy(h); return rc; }
     *out = h;
     return SSLPL_OK;
 }
 
 void sslpl_orb_destroy(sslpl_orb* h) {
     if (!h) return;
-    cudaSetDevice(h->p.device);
-    // an external stream may already be gone (its owner was destroyed first): never touch it here
-    if (h->stream && h->stream == h->own_stream) cudaStreamSynchronize(h->own_stream); else cudaDeviceSynchronize();
-    if (h->own_stream) cudaStreamDestroy(h->own_stream);
-    for (auto e : h->ev) cudaEventDestroy(e);
-    if (h->arena) cudaFree(h->arena);
-    if (h->h_err) cudaFreeHost(h->h_err);
+    h->close();
     delete h;
 }
 
@@ -1136,21 +1096,9 @@ int sslpl_orb_device_results(sslpl_orb* h, const sslpl_keypoint** d_kps, const u
     return SSLPL_OK;
 }
 
-int sslpl_orb_sync(sslpl_orb* h) {
-    SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle");
-    SSLPL_CUDA(cudaSetDevice(h->p.device));
-    return check_device_err(h);
-}
-
+int sslpl_orb_sync(sslpl_orb* h) { SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle"); return orb_sync(h); }
 void* sslpl_orb_stream(sslpl_orb* h) { return h ? (void*)h->stream : nullptr; }
-
-int sslpl_orb_set_stream(sslpl_orb* h, void* cuda_stream) {
-    SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle");
-    SSLPL_CUDA(cudaSetDevice(h->p.device));
-    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
-    h->stream = cuda_stream ? (cudaStream_t)cuda_stream : h->own_stream;
-    return SSLPL_OK;
-}
+int sslpl_orb_set_stream(sslpl_orb* h, void* cuda_stream) { SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle"); return h->set_stream(cuda_stream); }
 
 // Enqueue H2D of the frames, the whole extraction and the D2H of the results on the handle's stream; no host sync.
 static int orb_enqueue_host_batch(sslpl_orb* h, const uint8_t* imgs, int nframes, int width, int height, int pitch, size_t frame_stride,
@@ -1162,11 +1110,8 @@ static int orb_enqueue_host_batch(sslpl_orb* h, const uint8_t* imgs, int nframes
     if (rc) return rc;
     const int ip = (int)align_up(width, 16);
     const size_t fs = (size_t)ip * height;
-    if (frame_stride == (size_t)pitch * height)
-        SSLPL_CUDA(cudaMemcpy2DAsync(h->d_input, ip, imgs, pitch, width, (size_t)height * nframes, cudaMemcpyHostToDevice, h->stream));
-    else
-        for (int f = 0; f < nframes; f++)
-            SSLPL_CUDA(cudaMemcpy2DAsync(h->d_input + f * fs, ip, imgs + f * frame_stride, pitch, width, height, cudaMemcpyHostToDevice, h->stream));
+    rc = h->upload_frames(h->d_input, ip, fs, imgs, pitch, frame_stride, width, height, nframes);
+    if (rc) return rc;
     h->view.base = h->d_input; h->view.pitch = ip; h->view.frame_stride = (long long)fs;
     h->cur_frames = nframes;
     rc = run_pipeline(h, nframes);
@@ -1195,7 +1140,7 @@ int sslpl_orb_extract_batch(sslpl_orb* h, const uint8_t* imgs, int nframes, int 
     const bool fits = cap >= sslpl_orb_max_keypoints(h);
     int rc = orb_enqueue_host_batch(h, imgs, nframes, width, height, pitch, frame_stride, kps, desc, cap, n, fits);
     if (rc) return rc;
-    rc = check_device_err(h);
+    rc = orb_sync(h);
     if (rc || fits) return rc;
     // caller capacity smaller than the worst case: counts are on the host now, download only what fits
     const int kc = h->g.kp_total_cap;
@@ -1288,15 +1233,6 @@ int sslpl_orb_download_level_keypoints(sslpl_orb* h, int frame, int level, int* 
 long long sslpl_orb_launch_count(const sslpl_orb* h) { return h ? h->launches : 0; }
 
 int sslpl_orb_set_profiling(sslpl_orb* h, int on) { SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle"); h->profiling = on != 0; return SSLPL_OK; }
-
-int sslpl_orb_stage_ms(sslpl_orb* h, float* ms, int cap, const char** names, int* nstages) {
-    SSLPL_REQUIRE(h && nstages, SSLPL_ERR_ARG, "null argument");
-    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
-    int k = 0;
-    for (int i = 1; i < h->ev_n; i++, k++)
-        if (k < cap) { float t = 0; cudaEventElapsedTime(&t, h->ev[i - 1], h->ev[i]); if (ms) ms[k] = t; if (names) names[k] = h->ev_name[i]; }
-    *nstages = k;
-    return SSLPL_OK;
-}
+int sslpl_orb_stage_ms(sslpl_orb* h, float* ms, int cap, const char** names, int* nstages) { SSLPL_REQUIRE(h, SSLPL_ERR_ARG, "null handle"); return h->stage_ms(ms, cap, names, nstages); }
 
 }  // extern "C"
