@@ -87,18 +87,19 @@ _lib = None
 
 
 def lib():
-    """Load libsslpl_b200.so with the prototypes of include/sslpl.h on every function (fails loudly when it has not been built: run
-    __graft_entry__.build())."""
+    """Load libsslpl_b200.so with the prototypes of include/sslpl.h and include/sslpl_map.h on every function (fails loudly when it has
+    not been built: run __graft_entry__.build())."""
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise SslplError(f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'`"
                              " (there is no CPU fallback)")
         L = C.CDLL(LIB_PATH)
-        with open(os.path.join(_HERE, "..", "include", "sslpl.h")) as f:
-            for name, (restype, argtypes) in _prototypes(f.read()).items():
-                fn = getattr(L, name)
-                fn.restype, fn.argtypes = restype, argtypes
+        for header in ("sslpl.h", "sslpl_map.h"):
+            with open(os.path.join(_HERE, "..", "include", header)) as f:
+                for name, (restype, argtypes) in _prototypes(f.read()).items():
+                    fn = getattr(L, name)
+                    fn.restype, fn.argtypes = restype, argtypes
         _lib = L
     return _lib
 

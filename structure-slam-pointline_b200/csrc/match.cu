@@ -6,6 +6,7 @@
 // 2 x uint4 per row.  The batched layout is "a set of frames": frame f owns desc[f*cap..], a CSR feature
 // vector and optional masks; pair p matches frame p (KeyFrame role) against frame p+1 (Frame role).
 #include "common.cuh"
+#include "../../include/sslpl_map.h"
 #include "svd4.cuh"
 #include <algorithm>
 #include <climits>
@@ -976,6 +977,27 @@ __global__ void __launch_bounds__(32) k_init_match(const __grid_constant__ WinAr
 // One CTA per group, one thread per row; the median of a row (rank r = int(0.5 (N-1)) of N distances in 0..256) is found by
 // bisection on the value with count(d <= v) (8 passes over the row, descriptors stay in L1) — no sort, no per-thread arrays.
 // -------------------------------------------------------------------------------------------------
+// The median of row i: the smallest v with count(d <= v) >= r + 1 over the rows j in [0, n) with use(j) (the self-distance 0 counted),
+// returned as the key (median, i) whose minimum is the first least median.  row(j) is the address of row j's descriptor.
+template <class Row, class Use>
+__device__ __forceinline__ unsigned medoid_key(Row row, Use use, int n, int r, int i) {
+    uint4 a0, a1;
+    load_desc(row(i), a0, a1);
+    int lo = 0, hi = 256;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        int cnt = 0;
+        for (int j = 0; j < n; j++) {
+            if (!use(j)) continue;
+            uint4 b0, b1;
+            load_desc(row(j), b0, b1);
+            cnt += (j == i ? 0 : popc256(a0, a1, b0, b1)) <= mid;
+        }
+        if (cnt >= r + 1) hi = mid; else lo = mid + 1;
+    }
+    return ((unsigned)lo << 20) | (unsigned)i;
+}
+
 __global__ void __launch_bounds__(128) k_medoid(const uint8_t* desc, const int32_t* off, int32_t* best_idx, int32_t* best_median) {
     __shared__ unsigned s_best;
     const int gI = blockIdx.x, b = off[gI], N = off[gI + 1] - b;
@@ -984,23 +1006,9 @@ __global__ void __launch_bounds__(128) k_medoid(const uint8_t* desc, const int32
     if (N > 0) {
         const int r = (int)(0.5 * (double)(N - 1));
         unsigned mine = 0xffffffffu;
-        for (int i = threadIdx.x; i < N; i += blockDim.x) {
-            uint4 a0, a1;
-            load_desc(desc + (long long)(b + i) * 32, a0, a1);
-            int lo = 0, hi = 256;                                        // smallest v with count(d <= v) >= r + 1
-            while (lo < hi) {
-                const int mid = (lo + hi) >> 1;
-                int cnt = 0;
-                for (int j = 0; j < N; j++) {
-                    uint4 b0, b1;
-                    load_desc(desc + (long long)(b + j) * 32, b0, b1);
-                    cnt += (j == i ? 0 : popc256(a0, a1, b0, b1)) <= mid;
-                }
-                if (cnt >= r + 1) hi = mid; else lo = mid + 1;
-            }
-            const unsigned key = ((unsigned)lo << 20) | (unsigned)i;     // (median, row): the minimum is the first least median
-            mine = min(mine, key);
-        }
+        const auto row = [&](int j) { return desc + (long long)(b + j) * 32; };
+        for (int i = threadIdx.x; i < N; i += blockDim.x)
+            mine = min(mine, medoid_key(row, [](int) { return true; }, N, r, i));
         atomicMin(&s_best, mine);
     }
     __syncthreads();
@@ -1480,6 +1488,149 @@ __global__ void k_debug_svd4(int n, const float* A, float* W, float* Vt, int nh,
         for (int k = 0; k < 16; k++) Vt[16LL * i + k] = v[k];
     }
     if (i < nh) h[i] = glibc_hypot(hx[i], hy[i]);
+}
+
+// ---------------- MapPoint / MapLine ComputeDistinctiveDescriptors and UpdateNormalAndDepth / UpdateAverageDir (include/sslpl_map.h) ----------------
+struct MapUpd {
+    const float* kp; long long kp_fs; const uint8_t* desc; long long desc_fs; const int* n; int cap, nkf;   // the keyframe set
+    const float* pose; const uint8_t* kfbad;
+    int nel; float* el; uint8_t* eldesc; const double* pos; double* nrm64;    // element rows (lines: pos = mWorldPos in double)
+    int nupd; const int32_t* elem; const int32_t* refkf; const int32_t* off; const int2* obs; const int32_t* first;
+    int what, nlevels; float scale[SSLPL_MAX_LEVELS];
+    int32_t* status;
+};
+
+// first[e] = the first entry of this call that names element e
+__global__ void k_first_entry(const int32_t* elem, int nupd, int nel, int32_t* first) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nupd) return;
+    const int e = elem[i];
+    if ((unsigned)e < (unsigned)nel) atomicMin(first + e, i);
+}
+
+// One warp per entry.  The medoid is k_medoid's selection over the rows of the good keyframes, a lane per row.  The normal: the lanes
+// compute each observation's ray and its scale in parallel, then every lane runs the sum in observation order (each step rounds on the
+// previous one), reading the terms by shuffle.  Points: el[m][9] = Xw, normal, minInv, maxInv, maxRaw; lines: el[m][12] = SP, EP,
+// normal, minInv, maxInv, maxRaw with the position read from pos[m][6].
+template <bool kLine>
+__global__ void __launch_bounds__(128) k_map_update(const __grid_constant__ MapUpd U) {
+    constexpr int es = kLine ? 17 : 7, oct_at = kLine ? 2 : 5, ew = kLine ? 12 : 9;   // sslpl_keyline / sslpl_keypoint words, octave field
+    constexpr unsigned full = 0xffffffffu;
+    const int u = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (u >= U.nupd) return;
+    const bool geom = U.what & SSLPL_MAPUPD_GEOM, dsc = U.what & SSLPL_MAPUPD_DESC;
+    const int e = U.elem[u], o0 = U.off[u], N = U.off[u + 1] - o0, rk = geom ? U.refkf[u] : 0;
+    bool bad = (unsigned)e >= (unsigned)U.nel || U.first[e] != u || o0 < 0 || N < 0 || N > U.nkf || (unsigned)rk >= (unsigned)U.nkf;
+    if (!bad && N == 0) {
+        if (lane == 0) U.status[u] = SSLPL_MAPUPD_NO_OBS;
+        return;
+    }
+    const int2* obs = U.obs + o0;
+    int refpos = INT_MAX;                                                  // first position of the reference keyframe in the list
+    if (!bad) {
+        bool b = false;
+        for (int i = lane; i < N; i += 32) {
+            const int2 q = obs[i];
+            b |= (unsigned)q.x >= (unsigned)U.nkf || q.y < 0 || q.y >= min(U.n[min(max(q.x, 0), U.nkf - 1)], U.cap);
+            for (int j = 0; j < i && !b; j++) b |= obs[j].x == q.x;
+            if (q.x == rk) refpos = min(refpos, i);
+        }
+        bad = __any_sync(full, b);
+        refpos = __reduce_min_sync(full, refpos);
+    }
+    int oct = 0;
+    if (!bad && geom) {
+        const int ridx = refpos < N ? obs[refpos].y : 0;                  // observations[pRefKF] default-inserts 0
+        if (ridx >= min(U.n[rk], U.cap)) bad = true;
+        else oct = __float_as_int(U.kp[U.kp_fs * rk + (long long)es * ridx + oct_at]);
+    }
+    if (bad) {
+        if (lane == 0) U.status[u] = SSLPL_MAPUPD_BAD;
+        return;
+    }
+    int st = SSLPL_MAPUPD_OK;
+    if (dsc) {
+        const auto good = [&](int j) { return U.kfbad == nullptr || !U.kfbad[obs[j].x]; };
+        const auto row = [&](int j) { const int2 q = obs[j]; return U.desc + U.desc_fs * q.x + 32LL * q.y; };
+        int ng = 0;
+        for (int i = lane; i < N; i += 32) ng += good(i);
+        ng = __reduce_add_sync(full, ng);
+        if (ng == 0) {
+            st = SSLPL_MAPUPD_NO_GOOD_KF;
+        } else {
+            const int r = (int)(0.5 * (double)(ng - 1));
+            unsigned key = 0xffffffffu;
+            for (int i = lane; i < N; i += 32)
+                if (good(i)) key = min(key, medoid_key(row, good, N, r, i));
+            key = __reduce_min_sync(full, key);
+            if (lane < 8) reinterpret_cast<uint32_t*>(U.eldesc + 32LL * e)[lane] = reinterpret_cast<const uint32_t*>(row((int)(key & 0xfffffu)))[lane];
+        }
+    }
+    if (!geom) {
+        if (lane == 0) U.status[u] = st;
+        return;
+    }
+    float* P = U.el + (long long)ew * e;
+    const float* Oref = U.pose + 15LL * rk + 12;
+    float nf[3], X[3];                                                     // the normal as stored; the point whose distance is taken
+    if (!kLine) {
+        // normal = normal + normali / cv::norm(normali): scaleAdd(normali, 1.0 / norm, normal), fma with the scale narrowed to float;
+        // normal / n: convertTo with the scale 1.0 / n narrowed to float
+        X[0] = P[0]; X[1] = P[1]; X[2] = P[2];
+        float s0 = 0.f, s1 = 0.f, s2 = 0.f;
+        for (int b = 0; b < N; b += 32) {
+            float q0 = 0.f, q1 = 0.f, q2 = 0.f, a = 0.f;
+            if (b + lane < N) {
+                const float* Ow = U.pose + 15LL * obs[b + lane].x + 12;
+                q0 = __fsub_rn(X[0], Ow[0]); q1 = __fsub_rn(X[1], Ow[1]); q2 = __fsub_rn(X[2], Ow[2]);
+                a = __double2float_rn(__ddiv_rn(1.0, norm3d_d(q0, q1, q2)));
+            }
+            for (int j = 0; j < min(32, N - b); j++) {
+                const float aj = __shfl_sync(full, a, j);
+                s0 = __fmaf_rn(__shfl_sync(full, q0, j), aj, s0);
+                s1 = __fmaf_rn(__shfl_sync(full, q1, j), aj, s1);
+                s2 = __fmaf_rn(__shfl_sync(full, q2, j), aj, s2);
+            }
+        }
+        const float inv = __double2float_rn(__ddiv_rn(1.0, (double)N));
+        nf[0] = __fadd_rn(__fmul_rn(s0, inv), 0.f); nf[1] = __fadd_rn(__fmul_rn(s1, inv), 0.f); nf[2] = __fadd_rn(__fmul_rn(s2, inv), 0.f);
+    } else {
+        // Eigen in double: middlePos = 0.5 * (head + tail), normali = middlePos - OWi, normal += normali / normali.norm(), normal / n;
+        // the distance from MP = 0.5 * (SP + EP) of the float narrowing (addWeighted)
+        const double* W = U.pos + 6LL * e;
+        const double m0 = __dmul_rn(0.5, __dadd_rn(W[0], W[3])), m1 = __dmul_rn(0.5, __dadd_rn(W[1], W[4])), m2 = __dmul_rn(0.5, __dadd_rn(W[2], W[5]));
+        double s0 = 0.0, s1 = 0.0, s2 = 0.0;
+        for (int b = 0; b < N; b += 32) {
+            double q0 = 0.0, q1 = 0.0, q2 = 0.0;
+            if (b + lane < N) {
+                const float* Ow = U.pose + 15LL * obs[b + lane].x + 12;
+                q0 = __dsub_rn(m0, (double)Ow[0]); q1 = __dsub_rn(m1, (double)Ow[1]); q2 = __dsub_rn(m2, (double)Ow[2]);
+                const double nr = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(q0, q0), __dmul_rn(q1, q1)), __dmul_rn(q2, q2)));
+                q0 = __ddiv_rn(q0, nr); q1 = __ddiv_rn(q1, nr); q2 = __ddiv_rn(q2, nr);
+            }
+            for (int j = 0; j < min(32, N - b); j++) {
+                s0 = __dadd_rn(s0, __shfl_sync(full, q0, j));
+                s1 = __dadd_rn(s1, __shfl_sync(full, q1, j));
+                s2 = __dadd_rn(s2, __shfl_sync(full, q2, j));
+            }
+        }
+        const double dn = (double)N;
+        s0 = __ddiv_rn(s0, dn); s1 = __ddiv_rn(s1, dn); s2 = __ddiv_rn(s2, dn);
+        if (U.nrm64 && lane == 0) { U.nrm64[3LL * e] = s0; U.nrm64[3LL * e + 1] = s1; U.nrm64[3LL * e + 2] = s2; }
+        nf[0] = __double2float_rn(s0); nf[1] = __double2float_rn(s1); nf[2] = __double2float_rn(s2);
+#pragma unroll
+        for (int c = 0; c < 3; c++) X[c] = mid_aw(__double2float_rn(W[c]), __double2float_rn(W[c + 3]));
+    }
+    if (lane != 0) return;
+    P[ew - 6] = nf[0]; P[ew - 5] = nf[1]; P[ew - 4] = nf[2];
+    if (oct < 0 || oct >= U.nlevels) {
+        st = SSLPL_MAPUPD_REF_OCTAVE;
+    } else {
+        const float dist = norm3d(__fsub_rn(X[0], Oref[0]), __fsub_rn(X[1], Oref[1]), __fsub_rn(X[2], Oref[2]));
+        const float mx = __fmul_rn(dist, U.scale[oct]), mn = __fdiv_rn(mx, U.scale[U.nlevels - 1]);
+        P[ew - 3] = __fmul_rn(0.8f, mn); P[ew - 2] = __fmul_rn(1.2f, mx); P[ew - 1] = mx;
+    }
+    U.status[u] = st;
 }
 
 }  // namespace sslpl
@@ -2698,6 +2849,65 @@ int sslpl_fuse_lines_batch_device(sslpl_matcher* m,
            nullptr, th, d_best_idx, d_best_dist, M);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
+}
+
+// The map-element refresh of include/sslpl_map.h: the first entry of every element (k_first_entry over a table in the scratch), then
+// one warp per entry (k_map_update<kLine>, passed as `kernel`).
+static int map_update(sslpl_matcher* m, void (*kernel)(MapUpd), MapUpd& U, int rows, int nel, bool el_ok, const float* scaleFactors, int nlevels,
+                      const int32_t* d_elem, const int32_t* d_refkf, const int32_t* d_obs_off, const int32_t* d_obs, int nupd) {
+    SSLPL_REQUIRE(U.kp && U.desc && U.n, SSLPL_ERR_ARG, "null argument");
+    if (int rc = kf_set_ok(m, U.nkf, U.cap, rows)) return rc;
+    SSLPL_REQUIRE(U.what >= 1 && U.what <= 3, SSLPL_ERR_ARG, "what outside {1, 2, 3}");
+    SSLPL_REQUIRE(nel >= 0 && nupd >= 0, SSLPL_ERR_ARG, "negative count");
+    SSLPL_REQUIRE(nlevels >= 1 && nlevels <= SSLPL_MAX_LEVELS, SSLPL_ERR_ARG, "nlevels outside [1, SSLPL_MAX_LEVELS]");
+    const bool geom = U.what & SSLPL_MAPUPD_GEOM, dsc = U.what & SSLPL_MAPUPD_DESC;
+    SSLPL_REQUIRE((!dsc || U.eldesc) && (!geom || (el_ok && U.pose && scaleFactors)), SSLPL_ERR_ARG, "null argument");
+    if (nupd == 0) return SSLPL_OK;
+    SSLPL_REQUIRE(d_elem && d_obs_off && d_obs && U.status && (!geom || d_refkf), SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(reinterpret_cast<uintptr_t>(d_obs) % 8 == 0, SSLPL_ERR_ARG, "d_obs must be 8-byte aligned (read as int2 pairs)");
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    if (geom) for (int k = 0; k < nlevels; k++) U.scale[k] = scaleFactors[k];
+    U.nlevels = nlevels; U.nel = nel; U.nupd = nupd;
+    U.elem = d_elem; U.refkf = d_refkf; U.off = d_obs_off; U.obs = reinterpret_cast<const int2*>(d_obs);
+    if (int rc = ensure_scratch(m, sizeof(int32_t) * ((size_t)nel + 1))) return rc;
+    int32_t* first = reinterpret_cast<int32_t*>(m->scratch);
+    U.first = first;
+    if (nel > 0) {
+        if (int rc = fill(m, first, nel, INT_MAX)) return rc;
+        launch(m, k_first_entry, (nupd + 255) / 256, 256, 0, d_elem, nupd, nel, first);
+    }
+    launch(m, kernel, (nupd + 3) / 4, 128, 0, U);
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+int sslpl_update_map_points_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nkf, int cap,
+        const float* d_kfpose, const uint8_t* d_kfbad,
+        int nmp, float* d_mp, uint8_t* d_mpdesc,
+        int nupd, const int32_t* d_elem, const int32_t* d_refkf, const int32_t* d_obs_off, const int32_t* d_obs,
+        const float* scaleFactors, int nlevels, int what, int32_t* d_status) {
+    SSLPL_REQUIRE(m, SSLPL_ERR_ARG, "null handle");
+    MapUpd U;
+    memset(&U, 0, sizeof(U));
+    U.kp = reinterpret_cast<const float*>(d_kps); U.kp_fs = 7LL * cap; U.desc = d_desc; U.desc_fs = 32LL * cap; U.n = d_n; U.cap = cap;
+    U.nkf = nkf; U.pose = d_kfpose; U.kfbad = d_kfbad; U.el = d_mp; U.eldesc = d_mpdesc; U.what = what; U.status = d_status;
+    return map_update(m, k_map_update<false>, U, m->p.max_features, nmp, d_mp != nullptr, scaleFactors, nlevels, d_elem, d_refkf, d_obs_off, d_obs, nupd);
+}
+
+int sslpl_update_map_lines_batch_device(sslpl_matcher* m,
+        const sslpl_keyline* d_kl, const uint8_t* d_ldesc, const int* d_nl, int nkf, int capl,
+        const float* d_kfpose, const uint8_t* d_kfbad,
+        int nml, const double* d_mlpos, float* d_ml, uint8_t* d_mldesc, double* d_mlnormal,
+        int nupd, const int32_t* d_elem, const int32_t* d_refkf, const int32_t* d_obs_off, const int32_t* d_obs,
+        const float* scaleFactors, int nlevels, int what, int32_t* d_status) {
+    SSLPL_REQUIRE(m, SSLPL_ERR_ARG, "null handle");
+    MapUpd U;
+    memset(&U, 0, sizeof(U));
+    U.kp = reinterpret_cast<const float*>(d_kl); U.kp_fs = 17LL * capl; U.desc = d_ldesc; U.desc_fs = 32LL * capl; U.n = d_nl; U.cap = capl;
+    U.nkf = nkf; U.pose = d_kfpose; U.kfbad = d_kfbad; U.el = d_ml; U.eldesc = d_mldesc; U.pos = d_mlpos; U.nrm64 = d_mlnormal;
+    U.what = what; U.status = d_status;
+    return map_update(m, k_map_update<true>, U, m->p.max_lines, nml, d_ml && d_mlpos, scaleFactors, nlevels, d_elem, d_refkf, d_obs_off, d_obs, nupd);
 }
 
 }  // extern "C"

@@ -11,8 +11,15 @@ cv2 reaches the same functions: addWeighted and subtract directly, convertTo thr
                from a fused multiply-add; a constructed row whose exact value lies just past a float midpoint does (the double sum
                rounds onto the midpoint, then ties-to-even);
   convertTo    fl(fl(x * (float)scale) + 0): the double scale is narrowed to float first;
-  subtract     fl(a - b).
-tests/create_points_model.py follows these rules; test_create_points_cpu.py re-checks them.  (oracle/refshim/minicv.cpp evaluates
+  subtract     fl(a - b);
+  scaleAdd     normal + normali / cv::norm(normali) of MapPoint::UpdateNormalAndDepth (MapPoint.cc:359): Mat / double is an AddEx
+               expression with alpha = 1.0 / norm, and Mat + that expression assigns through MatOp_AddEx::assign, which calls
+               scaleAdd(normali, alpha, normal) when beta = 1 (an assumption from OpenCV's published matop.cpp: cv2's Python API has
+               no MatExpr, so only scaleAdd itself is measured here).  On CV_32F that is one fused multiply-add with alpha narrowed to float,
+               fma(a, (float)alpha, b) (the build's FMA3 dispatch: a canonical choice).  Random rows tell it from fl(fl(a * alpha) + b);
+               a constructed row (a * alpha = 1 + 2^-11 + 2^-24, a float midpoint, plus b = 2^-80) does at every length.
+tests/create_points_model.py and tests/map_update_model.py follow these rules; test_create_points_cpu.py and test_map_update_cpu.py
+re-check them.  (oracle/refshim/minicv.cpp evaluates
 Mat / double in double and rounds once; that stand-in is not used by this path.)  Usage: python tools/probe_cv_matexpr.py"""
 import numpy as np
 import cv2
@@ -43,6 +50,29 @@ def cvt_float(x, scale):
 
 def cvt_double(x, scale):
     return (x.astype(np.float64) * scale).astype(f32)
+
+
+def scale_add_midpoint(length):
+    """(fused, two roundings) of cv2.scaleAdd on a row whose exact a * alpha + b lies just above a float midpoint."""
+    a = np.full((1, length), 1 + 2.0 ** -12, f32)
+    b = np.full((1, length), 2.0 ** -80, f32)
+    got = cv2.scaleAdd(a, float(a[0, 0]), b)
+    return bool((got == f32(1 + 2.0 ** -11 + 2.0 ** -23)).all()), bool((got == f32(1 + 2.0 ** -11)).all())
+
+
+def probe_scale_add(n=20000, seed=7, length=3):
+    """Counts of random rows on which cv2.scaleAdd equals the fused rule and the two-rounding rule, and the midpoint row per length."""
+    from map_update_model import scale_add, two_roundings
+    rng = np.random.default_rng(seed)
+    A, B = rows(rng, n, length), rows(rng, n, length)
+    s = np.abs(rows(rng, n, 1)[:, 0]).astype(np.float64) + 0.1
+    cnt = dict(fused=0, two_roundings=0)
+    for k in range(n):
+        got = cv2.scaleAdd(A[k:k + 1], float(1.0 / s[k]), B[k:k + 1]).view(np.uint32)
+        cnt["fused"] += np.array_equal(got, scale_add(A[k:k + 1], 1.0 / s[k], B[k:k + 1]).view(np.uint32))
+        cnt["two_roundings"] += np.array_equal(got, two_roundings(A[k:k + 1], 1.0 / s[k], B[k:k + 1]).view(np.uint32))
+    mid = {L: scale_add_midpoint(L) for L in (1, 3, 4, 8)}
+    return cnt, mid
 
 
 def rows(rng, n, length):
@@ -88,3 +118,9 @@ if __name__ == "__main__":
     n, out = probe()
     for (op, length), c in out.items():
         print(f"{op:22s} length {length}: " + "  ".join(f"{k} {v}/{1 if 'midpoint' in op else n}" for k, v in c.items()))
+    import os, sys
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
+    cnt, mid = probe_scale_add()
+    print("scaleAdd               length 3: " + "  ".join(f"{k} {v}/20000" for k, v in cnt.items()))
+    for L, (fused, two) in mid.items():
+        print(f"scaleAdd midpoint      length {L}: fused {int(fused)}/1  two_roundings {int(two)}/1")
