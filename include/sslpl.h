@@ -571,6 +571,10 @@ long long sslpl_frame_launch_count(const sslpl_frame* h);
 /* Camera.fx/fy/cx/cy and k1 k2 p1 p2 [k3] (Tracking.cc:58-86); undistortion is skipped when k1 == 0 (Frame.cc:485) */
 int  sslpl_frame_set_camera(sslpl_frame* h, float fx, float fy, float cx, float cy, const float* dist, int ndist);
 int  sslpl_frame_image_bounds(sslpl_frame* h, int cols, int rows, float* bounds4 /* mnMinX mnMaxX mnMinY mnMaxY */);
+/* debug: k_undistort (mvKeysUn of one keypoint) on n host points xy[2 n] with the camera of the last sslpl_frame_set_camera, into
+   xy_out[2 n] (may alias xy); unchanged points when k1 == 0.  Launches one kernel on the ORB stream, counted by
+   sslpl_frame_launch_count, and waits for it.  sslpl_frame_image_bounds runs its four corners through this call. */
+int  sslpl_frame_debug_undistort(sslpl_frame* h, int n, const float* xy, float* xy_out);
 /* channels 1 (grey), 3 or 4 (interleaved 8-bit; rgb_order 1 = RGB[A], 0 = BGR[A] as Camera.RGB says).  Any output pointer but the
    counts may be NULL.  kps / kps_un / desc hold `cap` entries per frame (>= sslpl_orb_max_keypoints), the line outputs `lcap`. */
 int  sslpl_frame_extract(sslpl_frame* h, const uint8_t* img, int width, int height, int pitch, int channels, int rgb_order,

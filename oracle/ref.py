@@ -288,14 +288,17 @@ def line_extract(img, cap=64):
 
 
 def frame_from_image(img, nfeatures=1000, scale=1.2, nlevels=8, ini=20, mn=7, K=(500, 500, 320, 240), dist=(0, 0, 0, 0)):
-    """Frame::Frame(imGray, ...) (Frame.cc:69-131): dict(keys, keysUn, desc, keylines, ldesc, lineeq, grid_off, grid_idx, bounds)."""
+    """Frame::Frame(imGray, ...) (Frame.cc:69-131): dict(keys, keysUn, desc, keylines, ldesc, lineeq, grid_off, grid_idx, bounds).
+    dist: k1 k2 p1 p2 [k3], 4 or 5 coefficients as Tracking.cc:61-72 builds mDistCoef."""
     img = _u8(img)
+    dist = _f32(dist)
+    assert len(dist) in (4, 5)
     cap = nfeatures * 2 + 64 * nlevels; lcap = 64
     keys = np.zeros(cap, KEYPOINT_DTYPE); keysun = np.zeros(cap, KEYPOINT_DTYPE); desc = np.zeros((cap, 32), np.uint8)
     kl = np.zeros(lcap, KEYLINE_DTYPE); ld = np.zeros((lcap, 32), np.uint8); eq = np.zeros((lcap, 3), np.float64)
     NL = C.c_int(); goff = np.zeros(64 * 48 + 1, np.int32); gidx = np.zeros(cap, np.int32); b = np.zeros(4, np.float32)
     n = lib().ref_frame_from_image(_p(img), img.shape[1], img.shape[0], img.strides[0], nfeatures, C.c_float(scale), nlevels, ini, mn,
-                                   _p(_f32(K)), _p(_f32(dist)), _p(keys), _p(keysun), _p(desc), cap, _p(kl), _p(ld), _p(eq), lcap,
+                                   _p(_f32(K)), _p(dist), len(dist), _p(keys), _p(keysun), _p(desc), cap, _p(kl), _p(ld), _p(eq), lcap,
                                    C.byref(NL), _p(goff), _p(gidx), _p(b))
     nl = NL.value
     return dict(keys=keys[:n].copy(), keysUn=keysun[:n].copy(), desc=desc[:n].copy(), keylines=kl[:nl].copy(), ldesc=ld[:nl].copy(),

@@ -495,7 +495,7 @@ int ref_line_extract(const uint8_t* img, int w, int h, int pitch, orc_keyline* k
 // Outputs: keys (raw), keysUn, descriptors, keylines, line descriptors, line equations, and the 64x48 grid as CSR.
 // ------------------------------------------------------------------------------------------------
 int ref_frame_from_image(const uint8_t* img, int w, int h, int pitch, int nfeatures, float scaleFactor, int nlevels, int iniTh, int minTh,
-                         const float* K4, const float* dist4, orc_keypoint* keys, orc_keypoint* keysUn, uint8_t* desc, int cap,
+                         const float* K4, const float* dist, int ndist, orc_keypoint* keys, orc_keypoint* keysUn, uint8_t* desc, int cap,
                          orc_keyline* kl, uint8_t* ldesc, double* lineeq3, int lcap, int* NL,
                          int32_t* grid_off /*64*48+1*/, int32_t* grid_idx /*cap*/, float* bounds4) {
     BumpScope scope;
@@ -503,7 +503,7 @@ int ref_frame_from_image(const uint8_t* img, int w, int h, int pitch, int nfeatu
     ORBVocabulary voc;
     cv::Mat K = cv::Mat::eye(3, 3, CV_32F);
     K.at<float>(0, 0) = K4[0]; K.at<float>(1, 1) = K4[1]; K.at<float>(0, 2) = K4[2]; K.at<float>(1, 2) = K4[3];
-    cv::Mat D(4, 1, CV_32F); for (int i = 0; i < 4; i++) D.at<float>(i) = dist4[i];
+    cv::Mat D(ndist == 5 ? 5 : 4, 1, CV_32F); for (int i = 0; i < D.rows; i++) D.at<float>(i) = dist[i];   // mDistCoef (Tracking.cc:61-72)
     Frame::mbInitialComputations = true;
     cv::Mat image(h, w, CV_8UC1, (void*)img, (size_t)pitch);
     Frame F(image, 0.0, &ext, &voc, K, D, 0.f, 0.f);

@@ -198,7 +198,8 @@ SVD::SVD(InputArray, int) { assert(!"minicv: SVD is outside the tested path"); a
 void SVD::compute(InputArray, OutputArray, OutputArray, OutputArray, int) { assert(!"minicv: SVD is outside the tested path"); abort(); }
 
 // cv::undistortPoints(src, dst, K, D, noArray(), P=K) for N x 2 CV_32F points (Frame.cc:492-501, :519-527): iterative
-// inverse of the radial/tangential model (k1 k2 p1 p2 [k3]), 5 iterations as in OpenCV 3.4, computed in double.
+// inverse of the radial/tangential model (k1 k2 p1 p2 [k3]), 5 iterations as in OpenCV 4.13, computed in double: on the first iteration
+// whose distortion factor icdist is negative the point goes back to its normalised start and the iteration stops.
 void undistortPoints(InputArray src, OutputArray dst, InputArray cameraMatrix, InputArray distCoeffs, InputArray R, InputArray P) {
     const Mat s = src.getMat().clone(), K = cameraMatrix.getMat(), D = distCoeffs.getMat(), Pm = P.getMat();
     assert(R.empty() && s.depth() == CV_32F);
@@ -215,6 +216,7 @@ void undistortPoints(InputArray src, OutputArray dst, InputArray cameraMatrix, I
         const double x0 = x, y0 = y;
         for (int j = 0; j < 5; j++) {
             const double r2 = x * x + y * y, icdist = 1. / (1 + ((k[4] * r2 + k[1]) * r2 + k[0]) * r2);
+            if (icdist < 0) { x = x0; y = y0; break; }
             const double dx = 2 * k[2] * x * y + k[3] * (r2 + 2 * x * x), dy = k[2] * (r2 + 2 * y * y) + 2 * k[3] * x * y;
             x = (x0 - dx) * icdist; y = (y0 - dy) * icdist;
         }

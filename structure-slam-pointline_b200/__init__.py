@@ -818,6 +818,13 @@ class Frame(_Handle, kind="frame", lifecycle=("sync", "launch_count")):
         _check(lib().sslpl_frame_image_bounds(self._h, cols, rows, _p(b)))
         return b
 
+    def debug_undistort(self, xy):
+        """The device's mvKeysUn arithmetic (k_undistort with this handle's camera) on float32 points [N, 2] -> float32 [N, 2]."""
+        xy = _f32(xy).reshape(-1, 2)
+        out = np.empty_like(xy)
+        _check(lib().sslpl_frame_debug_undistort(self._h, len(xy), _p(xy), _p(out)))
+        return out
+
     def extract(self, image, rgb_order=False):
         """image: HxW (grey) or HxWx3 / HxWx4 uint8 (BGR[A] unless rgb_order)."""
         assert image.dtype == np.uint8 and image.ndim in (2, 3)

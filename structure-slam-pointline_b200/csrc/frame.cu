@@ -8,6 +8,8 @@
 //   * the undistorted keypoints (mvKeysUn) are computed from the device-resident keypoints, no second upload.
 // Product code: no oracle, no CPU fallback.
 #include "common.cuh"
+#include <algorithm>
+#include <memory>
 #include <new>
 
 namespace sslpl {
@@ -27,8 +29,12 @@ __global__ void __launch_bounds__(256) k_cvt_gray(const uint8_t* __restrict__ sr
 
 struct Camera { double fx, fy, cx, cy, k[5]; int distorted; };
 
-// cv::undistortPoints(src, dst, K, D, noArray(), K) on the keypoint coordinates (Frame.cc:492-501): five fixed-point iterations of
-// the radial / tangential model in double, re-projection with K, narrowing to float (bit-equal to cv2 4.13 in the tests).
+// cv::undistortPoints(src, dst, K, D, noArray(), K) on the keypoint coordinates (Frame.cc:492-501) as OpenCV 4.13 computes it: five
+// fixed-point iterations of the radial / tangential model in double, re-projection with K, narrowing to float.  On the first iteration
+// whose distortion factor icdist is negative (the point lies beyond the radius where 1 + k1 r2 + k2 r2^2 + k3 r2^3 changes sign, which
+// wide-angle calibrations reach inside the image) OpenCV puts the point back at its normalised start and stops; without that exit the
+// map diverges and the image bounds come out inverted.  Bit-equal to cv2 4.13 and to tests/undistort_model.py in the tests (frame.cu is
+// built with FMA contraction on, hence the _rn intrinsics).
 __device__ __forceinline__ void undistort_pt(const Camera& c, float xin, float yin, float* xo, float* yo) {
     double x = ((double)xin - c.cx) * (1.0 / c.fx), y = ((double)yin - c.cy) * (1.0 / c.fy);
     const double x0 = x, y0 = y;
@@ -36,6 +42,7 @@ __device__ __forceinline__ void undistort_pt(const Camera& c, float xin, float y
     for (int j = 0; j < 5; j++) {
         const double r2 = __dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y));
         const double icdist = 1.0 / __dadd_rn(1.0, __dmul_rn(__dadd_rn(__dmul_rn(__dadd_rn(__dmul_rn(c.k[4], r2), c.k[1]), r2), c.k[0]), r2));
+        if (icdist < 0.0) { x = x0; y = y0; break; }
         const double dx = __dadd_rn(__dmul_rn(__dmul_rn(__dmul_rn(2.0, c.k[2]), x), y), __dmul_rn(c.k[3], __dadd_rn(r2, __dmul_rn(__dmul_rn(2.0, x), x))));
         const double dy = __dadd_rn(__dmul_rn(c.k[2], __dadd_rn(r2, __dmul_rn(__dmul_rn(2.0, y), y))), __dmul_rn(__dmul_rn(__dmul_rn(2.0, c.k[3]), x), y));
         x = __dmul_rn(__dadd_rn(x0, -dx), icdist); y = __dmul_rn(__dadd_rn(y0, -dy), icdist);
@@ -132,24 +139,35 @@ int sslpl_frame_set_camera(sslpl_frame* h, float fx, float fy, float cx, float c
     return SSLPL_OK;
 }
 
+/* k_undistort over n host points (x, y pairs) with the handle's camera, on its stream; waits for the result */
+int sslpl_frame_debug_undistort(sslpl_frame* h, int n, const float* xy, float* xy_out) {
+    SSLPL_REQUIRE(h && n >= 0 && (n == 0 || (xy && xy_out)), SSLPL_ERR_ARG, "bad argument");
+    if (n == 0) return SSLPL_OK;
+    std::unique_ptr<sslpl_keypoint[]> k(new (std::nothrow) sslpl_keypoint[n]());
+    SSLPL_REQUIRE(k, SSLPL_ERR_ARG, "out of host memory");
+    for (int i = 0; i < n; i++) { k[i].x = xy[2 * i]; k[i].y = xy[2 * i + 1]; }
+    SSLPL_CUDA(cudaSetDevice(h->p.orb.device));
+    if (int rc = ensure_scratch(h, 2 * sizeof(sslpl_keypoint) * (size_t)n + 1024)) return rc;
+    Arena A; A.base = h->scratch;
+    cudaError_t e = cudaSuccess;
+    const sslpl_keypoint* d_in = stage(A, k.get(), n, h->stream, e); const int* d_n = stage(A, &n, 1, h->stream, e);
+    sslpl_keypoint* d_out = A.take<sslpl_keypoint>(n);
+    SSLPL_CUDA(e);
+    launch(h, k_undistort, dim3((n + 255) / 256, 1), 256, 0, d_in, d_n, n, h->cam, d_out);
+    SSLPL_CUDA(cudaGetLastError());
+    SSLPL_CUDA(cudaMemcpyAsync(k.get(), d_out, sizeof(sslpl_keypoint) * (size_t)n, cudaMemcpyDeviceToHost, h->stream));
+    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < n; i++) { xy_out[2 * i] = k[i].x; xy_out[2 * i + 1] = k[i].y; }
+    return SSLPL_OK;
+}
+
 /* Frame::ComputeImageBounds (Frame.cc:515-543): mnMinX, mnMaxX, mnMinY, mnMaxY of a cols x rows image */
 int sslpl_frame_image_bounds(sslpl_frame* h, int cols, int rows, float* bounds4) {
     SSLPL_REQUIRE(h && bounds4, SSLPL_ERR_ARG, "null argument");
     if (!h->cam.distorted) { bounds4[0] = 0.f; bounds4[1] = (float)cols; bounds4[2] = 0.f; bounds4[3] = (float)rows; return SSLPL_OK; }
-    SSLPL_CUDA(cudaSetDevice(h->p.orb.device));
-    sslpl_keypoint c[4]; const int n4 = 4;
-    memset(c, 0, sizeof(c));
-    c[1].x = (float)cols; c[2].y = (float)rows; c[3].x = (float)cols; c[3].y = (float)rows;
-    if (int rc = ensure_scratch(h, 2 * sizeof(c) + 1024)) return rc;
-    Arena A; A.base = h->scratch;
-    cudaError_t e = cudaSuccess;
-    const sslpl_keypoint* d_in = stage(A, c, 4, h->stream, e); const int* d_n = stage(A, &n4, 1, h->stream, e); sslpl_keypoint* d_out = A.take<sslpl_keypoint>(4);
-    SSLPL_CUDA(e);
-    launch(h, k_undistort, dim3(1, 1), 256, 0, d_in, d_n, 4, h->cam, d_out);
-    SSLPL_CUDA(cudaGetLastError());
-    SSLPL_CUDA(cudaMemcpyAsync(c, d_out, sizeof(c), cudaMemcpyDeviceToHost, h->stream));
-    SSLPL_CUDA(cudaStreamSynchronize(h->stream));
-    bounds4[0] = fminf(c[0].x, c[2].x); bounds4[1] = fmaxf(c[1].x, c[3].x); bounds4[2] = fminf(c[0].y, c[1].y); bounds4[3] = fmaxf(c[2].y, c[3].y);
+    float c[8] = {0.f, 0.f, (float)cols, 0.f, 0.f, (float)rows, (float)cols, (float)rows};
+    if (int rc = sslpl_frame_debug_undistort(h, 4, c, c)) return rc;
+    bounds4[0] = std::min(c[0], c[4]); bounds4[1] = std::max(c[2], c[6]); bounds4[2] = std::min(c[1], c[3]); bounds4[3] = std::max(c[5], c[7]);
     return SSLPL_OK;
 }
 

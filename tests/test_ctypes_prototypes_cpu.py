@@ -4,6 +4,7 @@ import ast
 import ctypes as C
 import os
 import re
+import subprocess
 import numpy as np
 import pytest
 
@@ -18,10 +19,19 @@ def _header_arity():
             for name, params in re.findall(r"\b(sslpl_[a-z0-9_]+)\s*\(([^)]*)\)", hdr)}
 
 
-def test_every_header_function_has_its_prototype(pkg):
+def _exported():
+    """The sslpl_* functions the built library exports (its dynamic symbol table), independent of both headers' parsers."""
+    so = os.path.join(PKG_DIR, "libsslpl_b200.so")
+    out = subprocess.run(["nm", "-D", "--defined-only", so], capture_output=True, text=True, check=True).stdout
+    return {line.split()[-1] for line in out.splitlines() if line.split() and line.split()[-1].startswith("sslpl_")}
+
+
+def test_every_exported_function_has_its_header_prototype(pkg):
+    """include/sslpl.h declares exactly the library's exports outside include/sslpl_map.h, and each is bound with its prototype."""
     lib = pkg.lib()
     arity = _header_arity()
-    assert len(arity) == 102
+    map_fns = {"sslpl_update_map_points_batch_device", "sslpl_update_map_lines_batch_device"}
+    assert set(arity) == _exported() - map_fns
     mapped = {C.c_void_p, C.c_int, C.c_float, C.c_double, C.c_size_t, C.c_longlong}
     for name, n in arity.items():
         argtypes = getattr(lib, name).argtypes
@@ -42,6 +52,7 @@ def test_prototype_spot_checks(pkg):
         assert getattr(lib, f"sslpl_{kind}_extract_batch_device").argtypes[-1] is C.c_size_t
     assert lib.sslpl_frame_set_camera.argtypes == [C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_int]
     assert lib.sslpl_frame_stream.argtypes == [C.c_void_p, C.c_int]
+    assert lib.sslpl_frame_debug_undistort.argtypes == [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     assert lib.sslpl_predict_scale_table.argtypes == [C.c_float, C.c_int, C.c_void_p]
 
 

@@ -101,6 +101,15 @@ def test_frame_launch_counts(pkg, synth):
     assert _delta(fr, begin) == base + 1                                             # k1 != 0: mvKeysUn is always computed
 
 
+def test_frame_debug_calls_count_their_kernel(pkg):
+    fr = _handle(pkg, "frame")
+    pts = np.stack([np.linspace(0, W, 300), np.linspace(0, H, 300)], 1).astype(np.float32)
+    assert _delta(fr, lambda: fr.image_bounds(W, H)) == 0                          # k1 == 0: the image itself, nothing launched
+    fr.set_camera(300.0, 300.0, W / 2, H / 2, (0.1, 0.0, 0.0, 0.0))
+    assert _delta(fr, lambda: fr.debug_undistort(pts)) == 1
+    assert _delta(fr, lambda: fr.image_bounds(W, H)) == 1                          # the four corners through the same k_undistort
+
+
 @pytest.mark.parametrize("kind, names", [("orb", ["pyramid", "fast", "octree", "blur", "orient_desc"]),
                                          ("line", ["lsd_prep", "lsd_seeds", "lsd_regions", "lsd_nfa", "keylines_lbd"])])
 def test_profiled_stage_names(pkg, synth, kind, names):

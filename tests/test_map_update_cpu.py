@@ -5,6 +5,7 @@ import ast
 import ctypes as C
 import os
 import re
+import subprocess
 import numpy as np
 import pytest
 
@@ -21,10 +22,15 @@ def _arity(header):
     return {name: params.count(",") + 1 for name, params in re.findall(r"\b(sslpl_[a-z0-9_]+)\s*\(([^)]*)\)", hdr)}
 
 
-def test_map_header_functions_are_bound(pkg):
+def test_map_header_functions_are_bound_and_complete_the_exports(pkg):
     arity = _arity("sslpl_map.h")
     assert set(arity) == {"sslpl_update_map_points_batch_device", "sslpl_update_map_lines_batch_device"}
-    assert len(_arity("sslpl.h")) == 102
+    # the two headers together declare exactly what the library exports, and no function twice
+    so = os.path.join(PKG_DIR, "libsslpl_b200.so")
+    nm = subprocess.run(["nm", "-D", "--defined-only", so], capture_output=True, text=True, check=True).stdout
+    exported = {ln.split()[-1] for ln in nm.splitlines() if ln.split() and ln.split()[-1].startswith("sslpl_")}
+    main = set(_arity("sslpl.h"))
+    assert not main & set(arity) and main | set(arity) == exported
     lib = pkg.lib()
     for name, n in arity.items():
         fn = getattr(lib, name)

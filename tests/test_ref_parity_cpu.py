@@ -391,6 +391,23 @@ def test_frame_constructor(oracle, ref, icl_gray):
         assert np.array_equal(cell, np.flatnonzero((gx == c) & (gy == r)))
 
 
+@pytest.mark.parametrize("name", ["tum1", "euroc", "wide_k1", "wide_tangential"])
+def test_frame_constructor_undistortion_equals_the_model(ref, icl_gray, name):
+    """The reference's own UndistortKeyPoints and ComputeImageBounds (Frame.cc:483-543, with 4 or 5 coefficients as Tracking.cc builds
+    mDistCoef) equal tests/undistort_model.py bit for bit, for real calibrations and for cameras whose distortion factor turns negative
+    inside the image."""
+    import undistort_model as M
+    K, D = M.camera(name)
+    fr = ref.frame_from_image(icl_gray, K=K, dist=D)
+    keys, un = fr["keys"], fr["keysUn"]
+    assert len(keys) > 500
+    want = M.undistort_keypoints(np.stack([keys["x"], keys["y"]], 1), K, D)
+    assert np.array_equal(np.stack([un["x"], un["y"]], 1).view(np.uint32), want.view(np.uint32))
+    for f in ("size", "angle", "response", "octave", "class_id"):
+        assert np.array_equal(un[f], keys[f])
+    assert np.array_equal(fr["bounds"].view(np.uint32), M.image_bounds(640, 480, K, D).view(np.uint32)), fr["bounds"]
+
+
 # ------------------------------------------------------------------------------------------------
 # SURVEY.md 8(f) row 3: line projection matchers and Fuse
 # ------------------------------------------------------------------------------------------------
