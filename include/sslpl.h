@@ -285,10 +285,12 @@ int  sslpl_descriptor_medoid_batch(sslpl_matcher* m, const uint8_t* desc, const 
    (Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1127-1259).  SURVEY.md 8(f) row 1. ---- */
 typedef struct sslpl_vocab sslpl_vocab;
 /* The tree as arrays (what loadFromTextFile :1338-1420 builds): node 0 = root, parent[i] < i (parent[0] ignored),
-   desc[i][32], weight[i], is_leaf[i] (must agree with the structure).  Word ids number the leaves in node order. */
+   desc[i][32], weight[i], is_leaf[i] (must agree with the structure).  Word ids number the leaves in node order.  Such a vocabulary
+   weights TF_IDF and scores L1_NORM, as ORBvoc.txt does (its header is "10 6 0 0"). */
 int  sslpl_vocab_create(int device, int k, int L, int nnodes, const int32_t* parent, const uint8_t* desc, const double* weight,
                         const uint8_t* is_leaf, sslpl_vocab** out);
-/* ORBvoc.txt text format (System.cc:70 mpVocabulary->loadFromTextFile); scoring / weighting = the header's n1 / n2 */
+/* ORBvoc.txt text format (System.cc:70 mpVocabulary->loadFromTextFile); scoring / weighting = the header's n1 / n2, which the
+   vocabulary keeps */
 int  sslpl_vocab_load_text(int device, const char* path, sslpl_vocab** out, int* scoring, int* weighting);
 void sslpl_vocab_destroy(sslpl_vocab* v);
 int  sslpl_vocab_info(const sslpl_vocab* v, int* k, int* L, int* nnodes, int* nwords);
@@ -304,6 +306,54 @@ int  sslpl_bow_transform(sslpl_matcher* m, const sslpl_vocab* v, const uint8_t* 
 int  sslpl_match_bow_batch_device_vocab(sslpl_matcher* m, const uint8_t* d_desc, const sslpl_keypoint* d_kps, const int* d_n,
                                         int nframes, int cap, const sslpl_vocab* v, int levelsup, float nnratio, int checkOrientation,
                                         int32_t* d_match, int32_t* d_nmatch, int32_t* d_word, int32_t* d_node, double* d_weight);
+
+/* ---- KeyFrameDatabase (src/KeyFrameDatabase.cc) over a row set resident in HBM, asynchronous on the matcher's stream like the other
+   *_batch_device calls.  The row set: nrows rows, each a frame or a keyframe, in the extractors' layout d_desc[r][cap][32], d_n[r]
+   (clamped to cap), and their BowVector tables d_bow_word[r][cap] int32, d_bow_val[r][cap] double, d_bow_n[r]: mBowVec as ascending
+   (word, value) entries, (-1, 0.0) past the count.  Needs cap <= max_features + 64 and (P + cap) * 8 <= 200 KB with P the least power of
+   two >= cap (cap <= 8256).  Bad host arguments return SSLPL_ERR_ARG and enqueue nothing.
+
+   Frame::ComputeBoW / KeyFrame::ComputeBoW's mBowVec (Frame.cc:474-481, KeyFrame.cc:71-80) of every row, with the vocabulary tree of
+   TemplatedVocabulary::transform (TemplatedVocabulary.h:1127-1197): stopped words (weight <= 0) left out, the TF_IDF weights of a word
+   added in feature order (BowVector::addWeight, BowVector.cpp:34-46), then divided by the sequential sum of their absolute values in
+   ascending word order (BowVector::normalize :62-84; L1 scoring normalises, so there is no division by the word count).  Only a TF_IDF /
+   L1_NORM vocabulary is supported; any other returns SSLPL_ERR_UNSUPPORTED and enqueues nothing.  nrows <= 65535. */
+int  sslpl_bow_vectors_batch_device(sslpl_matcher* m, const sslpl_vocab* v, const uint8_t* d_desc, const int* d_n, int nrows, int cap,
+                                    int32_t* d_bow_word, double* d_bow_val, int32_t* d_bow_n);
+/* TemplatedVocabulary::score(v1, v2) = L1Scoring::score (ScoringObject.cpp:23-67) of row pairs d_pair[p] = (r1, r2), r1 the first
+   argument (the query): over the common words in ascending order, score += (|vi - wi| - |vi|) - |wi|; d_score[p] = -score / 2.0; NaN for
+   a pair with a row outside [0, nrows).  LoopClosing::DetectLoop's minScore (LoopClosing.cc:122-142) is the float minimum of these over the
+   query's non-bad covisible keyframes, starting at 1. */
+int  sslpl_bow_score_batch_device(sslpl_matcher* m, const int32_t* d_bow_word, const double* d_bow_val, const int32_t* d_bow_n, int nrows,
+                                  int cap, int npairs, const int32_t* d_pair, double* d_score);
+/* KeyFrameDatabase::DetectLoopCandidates(pKF, minScore) (:81-202) and DetectRelocalizationCandidates(F) (:204-314, the call of
+   Tracking::Relocalization, Tracking.cc:1961-1970) for nq query rows d_query[q] against the database d_db[ndb]: its rows in
+   KeyFrameDatabase::add order (:45-51) with erased keyframes (:53-72) left out, which is the order of every inverted-file list.
+   d_covis[nrows][10] = GetBestCovisibilityKeyFrames(10) of each row, padded with -1; an entry outside [0, nrows) or outside the database
+   is a keyframe outside the database.  Loop only: d_conn_off[nq + 1] / d_conn[nconn] = the rows of the query's GetConnectedKeyFrames()
+   (never listed), d_minscore[nq].  Each query starts fresh, as growing frame and keyframe ids guarantee in the reference.
+   Results per query q and database position p (the reference's per-KeyFrame fields, KeyFrame.h:172-177):
+     d_cand[q][ndb]  the candidate rows in the order of the returned vector, -1 after d_ncand[q];
+     d_words[q][ndb] mnLoopWords / mnRelocWords, 0 when the keyframe shares no word with the query or is connected to a loop query;
+     d_score[q][ndb] mLoopScore / mRelocScore written by this query (float), NaN when it did not score the keyframe.
+   Reloc state: the reloc neighbour test reads mRelocScore of listed keyframes the query did not score, left by an earlier query or never
+   initialised (KeyFrame.cc:45).  Query q reads the score such a keyframe got in the latest earlier query of the call that scored it, or
+   else d_relocscore[row]; afterwards d_relocscore holds each keyframe's score after the last query.  So one call equals nq sequential
+   reference calls on keyframes whose mRelocScore starts at d_relocscore (0 is as good as any value for a fresh keyframe).  Finding that
+   earlier query walks back through the call's queries, so a call costs O(nq) per such neighbour; split sequences of thousands of frames
+   into calls chained through d_relocscore.
+   d_ncand[q] = -1 (no candidates, words 0, scores NaN) for a query row outside [0, nrows) or, loop only, connected offsets not within
+   0 <= d_conn_off[q] <= d_conn_off[q + 1] <= nconn; and for every query when a database row is outside [0, nrows) or listed twice.
+   Needs ndb in [1, 25600], nq in [1, 65535] and nconn >= 0; the first call allocates an nrows-int row -> position map (and nq ints),
+   freed with the handle. */
+int  sslpl_detect_loop_candidates_batch_device(sslpl_matcher* m, const int32_t* d_bow_word, const double* d_bow_val, const int32_t* d_bow_n,
+        int nrows, int cap, const int32_t* d_db, int ndb, const int32_t* d_query, int nq, const int32_t* d_covis,
+        const int32_t* d_conn_off, const int32_t* d_conn, int nconn, const float* d_minscore,
+        int32_t* d_cand, int32_t* d_ncand, int32_t* d_words, float* d_score);
+int  sslpl_detect_relocalization_candidates_batch_device(sslpl_matcher* m, const int32_t* d_bow_word, const double* d_bow_val,
+        const int32_t* d_bow_n, int nrows, int cap, const int32_t* d_db, int ndb, const int32_t* d_query, int nq, const int32_t* d_covis,
+        float* d_relocscore, int32_t* d_cand, int32_t* d_ncand, int32_t* d_words, float* d_score);
+
 /* Batched line matching in HBM: knn2 + ratio rule of LSDmatcher::SearchByProjection(KF,F) (:143-183) with all
    KF lines valid: d_lmatch[p*capl + tdx] = qdx or -1; d_nlmatch[p]. */
 int  sslpl_match_lines_batch_device(sslpl_matcher* m, const uint8_t* d_ldesc, const int* d_nl, int nframes, int capl,

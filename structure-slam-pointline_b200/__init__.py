@@ -556,6 +556,35 @@ class Matcher(_Handle, kind="matcher", lifecycle=("sync", "set_stream", "stream"
             self._h, d_kl, d_ldesc, d_nl, nkf, capl, d_kfpose, nml, d_ml, d_mldesc, nentries, d_entry, d_skip or None, _p(_f32(cam)[:4].copy()),
             _p(_f32(bounds)), _p(sf), len(sf), log_scale_factor, th, d_best_idx, d_best_dist))
 
+    def bow_vectors_batch_device(self, vocab, d_desc, d_n, nrows, cap, d_bow_word, d_bow_val, d_bow_n):
+        """Frame::ComputeBoW's mBowVec of nrows rows in HBM (see sslpl_bow_vectors_batch_device): d_desc [nrows, cap, 32] u8, d_n
+        [nrows] i32 -> d_bow_word [nrows, cap] i32, d_bow_val [nrows, cap] f64, d_bow_n [nrows] i32.  TF_IDF / L1_NORM vocabularies
+        only.  Asynchronous on the matcher's stream."""
+        if (vocab.scoring, vocab.weighting) != (0, 0):
+            raise SslplError("BowVectors are built for TF_IDF weighting and L1 scoring only")
+        _check(lib().sslpl_bow_vectors_batch_device(self._h, vocab._h, d_desc, d_n, nrows, cap, d_bow_word, d_bow_val, d_bow_n))
+
+    def bow_score_batch_device(self, d_bow_word, d_bow_val, d_bow_n, nrows, cap, npairs, d_pair, d_score):
+        """TemplatedVocabulary::score (L1) of row pairs d_pair [npairs, 2] i32 -> d_score [npairs] f64 (NaN: a row out of range)."""
+        _check(lib().sslpl_bow_score_batch_device(self._h, d_bow_word, d_bow_val, d_bow_n, nrows, cap, npairs, d_pair, d_score))
+
+    def detect_loop_candidates_batch_device(self, d_bow_word, d_bow_val, d_bow_n, nrows, cap, d_db, ndb, d_query, nq, d_covis,
+                                            d_conn_off, d_conn, nconn, d_minscore, d_cand, d_ncand, d_words, d_score):
+        """KeyFrameDatabase::DetectLoopCandidates for nq query rows against the database rows d_db (add order, erased ones left out):
+        d_covis [nrows, 10] i32, d_conn_off [nq + 1] / d_conn [nconn] i32, d_minscore [nq] f32 -> d_cand [nq, ndb] / d_ncand [nq] /
+        d_words [nq, ndb] i32, d_score [nq, ndb] f32.  Asynchronous on the matcher's stream."""
+        _check(lib().sslpl_detect_loop_candidates_batch_device(self._h, d_bow_word, d_bow_val, d_bow_n, nrows, cap, d_db, ndb, d_query, nq,
+                                                               d_covis, d_conn_off, d_conn, nconn, d_minscore, d_cand, d_ncand, d_words,
+                                                               d_score))
+
+    def detect_relocalization_candidates_batch_device(self, d_bow_word, d_bow_val, d_bow_n, nrows, cap, d_db, ndb, d_query, nq, d_covis,
+                                                      d_relocscore, d_cand, d_ncand, d_words, d_score):
+        """KeyFrameDatabase::DetectRelocalizationCandidates for nq query rows in sequence; d_relocscore [nrows] f32 is the keyframes'
+        mRelocScore, read and updated (see sslpl_detect_relocalization_candidates_batch_device).  Outputs as the loop call."""
+        _check(lib().sslpl_detect_relocalization_candidates_batch_device(self._h, d_bow_word, d_bow_val, d_bow_n, nrows, cap, d_db, ndb,
+                                                                         d_query, nq, d_covis, d_relocscore, d_cand, d_ncand, d_words,
+                                                                         d_score))
+
     def debug_predict_scale(self, ratio, log_scale_factor, nlevels, clamp=True):
         """MapPoint / MapLine::PredictScale on the device for host ratios (see sslpl_matcher_debug_predict_scale) -> int32 levels."""
         r = _f32(ratio).reshape(-1)

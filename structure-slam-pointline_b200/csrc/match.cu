@@ -1633,6 +1633,316 @@ __global__ void __launch_bounds__(128) k_map_update(const __grid_constant__ MapU
     U.status[u] = st;
 }
 
+// -------------------------------------------------------------------------------------------------
+// Keyframe database (src/KeyFrameDatabase.cc) over a row set in HBM.  Every double sum below is sequential in ascending word order,
+// as the reference's std::map walks run; the parallelism is across rows, pairs, queries and database positions only.
+// -------------------------------------------------------------------------------------------------
+struct BowRows { int32_t* word; double* val; int32_t* n; int cap; };
+
+// BowVector of one row (TemplatedVocabulary::transform :1145-1195 with TF_IDF weighting and L1 scoring): k_vocab_transform left the
+// row's word ids and leaf weights in word / val [r][cap].  One CTA per row: the (word, feature) keys of the weighted features are sorted
+// in shared memory (P = a power of two >= cap), each run adds its weights in feature order (BowVector::addWeight :34-46), one thread
+// takes the L1 norm in word order and every value is divided by it (normalize :62-84).  Entries past the count become (-1, 0.0).
+__global__ void __launch_bounds__(512) k_bow_vector(BowRows B, const int* d_n, int P) {
+    extern __shared__ unsigned long long s_key[];      // P keys, then cap weights (doubles)
+    __shared__ int s_warp[33];
+    __shared__ double s_norm;
+    double* s_w = reinterpret_cast<double*>(s_key + P);
+    const int r = blockIdx.x, tid = threadIdx.x, cap = B.cap;
+    const int n = min(max(d_n[r], 0), cap);
+    int32_t* W = B.word + (long long)r * cap; double* V = B.val + (long long)r * cap;
+    for (int i = tid; i < P; i += blockDim.x) {
+        unsigned long long k = ~0ull;
+        if (i < n) {
+            const double w = V[i];
+            s_w[i] = w;
+            if (w > 0) k = ((unsigned long long)(unsigned)W[i] << 32) | (unsigned)i;
+        }
+        s_key[i] = k;
+    }
+    __syncthreads();
+    for (int k = 2; k <= P; k <<= 1)                   // bitonic sort, ascending
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            for (int i = tid; i < P; i += blockDim.x) {
+                const int l = i ^ j;
+                if (l > i) {
+                    const unsigned long long a = s_key[i], b = s_key[l];
+                    if ((a > b) == ((i & k) == 0)) { s_key[i] = b; s_key[l] = a; }
+                }
+            }
+            __syncthreads();
+        }
+    // runs of equal words: run starts are numbered in order by a block scan over chunks of blockDim keys
+    int nruns = 0;
+    for (int base = 0; base < n; base += blockDim.x) {
+        const int i = base + tid;
+        const unsigned long long k = i < n ? s_key[i] : ~0ull;
+        const bool start = k != ~0ull && (i == 0 || (s_key[i - 1] >> 32) != (k >> 32));
+        int total;
+        const int o = nruns + block_exclusive_scan(start ? 1 : 0, s_warp, &total);
+        double sum = 0.0;
+        if (start) {
+            for (int j = i; j < n && (s_key[j] >> 32) == (k >> 32); j++) sum = __dadd_rn(sum, s_w[(unsigned)s_key[j]]);
+        }
+        if (start) { W[o] = (int32_t)(k >> 32); V[o] = sum; }
+        nruns += total;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        double norm = 0.0;
+        for (int o = 0; o < nruns; o++) norm = __dadd_rn(norm, fabs(V[o]));
+        s_norm = norm;
+        B.n[r] = nruns;
+    }
+    __syncthreads();
+    const double norm = s_norm;
+    for (int o = tid; o < cap; o += blockDim.x) {
+        if (o < nruns) { if (norm > 0.0) V[o] = __ddiv_rn(V[o], norm); }
+        else { W[o] = -1; V[o] = 0.0; }
+    }
+}
+
+// L1Scoring::score (ScoringObject.cpp:23-67) of a sorted BowVector (qw, qv, nq) against row r: the common words in ascending order, each
+// term ((|v - w| - |v|) - |w|) added to the sum in that order; the caller negates and halves.  The merge visits the same common words
+// as the reference's lower_bound jumps.
+__device__ __forceinline__ double l1_sum(const int32_t* qw, const double* qv, int nq, const int32_t* dw, const double* dv, int nd) {
+    double s = 0.0;
+    int i = 0, j = 0;
+    while (i < nq && j < nd) {
+        const int a = qw[i], b = dw[j];
+        if (a == b) {
+            const double vi = qv[i], wi = dv[j];
+            s = __dadd_rn(s, __dsub_rn(__dsub_rn(fabs(__dsub_rn(vi, wi)), fabs(vi)), fabs(wi)));
+            i++; j++;
+        } else if (a < b) i++;
+        else j++;
+    }
+    return s;
+}
+
+__device__ __forceinline__ int bow_count(const BowRows& B, int r) { return min(max(B.n[r], 0), B.cap); }
+
+// TemplatedVocabulary::score(v1, v2) for row pairs; NaN for a pair with a row outside [0, nrows).  Thread per pair.
+__global__ void __launch_bounds__(128) k_bow_score(BowRows B, int nrows, int npairs, const int2* pair, double* score) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= npairs) return;
+    const int2 q = pair[p];
+    if ((unsigned)q.x >= (unsigned)nrows || (unsigned)q.y >= (unsigned)nrows) { score[p] = __longlong_as_double(0x7ff8000000000000LL); return; }
+    const long long o1 = (long long)q.x * B.cap, o2 = (long long)q.y * B.cap;
+    const double s = l1_sum(B.word + o1, B.val + o1, bow_count(B, q.x), B.word + o2, B.val + o2, bow_count(B, q.y));
+    score[p] = __ddiv_rn(-s, 2.0);
+}
+
+// The database of one call: its rows in add order, the row -> position map (-1: not in the database), the error word (non-zero: a
+// database row outside [0, nrows) or listed twice, which fails every query) and maxw[q], the largest word count of query q.
+struct KfdbArgs {
+    BowRows B; int nrows;
+    const int32_t* db; int ndb; int32_t* pos_of_row; int32_t* err; int32_t* maxw;
+    const int32_t* query; int nq;
+    const int32_t* covis;                        // [nrows][10], -1 padded
+    const int32_t* conn_off; const int32_t* conn; int nconn; const float* minscore;    // loop only
+    float* relocscore;                           // reloc only
+    int32_t* cand; int32_t* ncand; int32_t* words; float* score;
+};
+constexpr int KFDB_POS_BITS = 15;               // sort key of a listed keyframe: (index of its first common word in the query) << 15 | position
+constexpr int KFDB_CHUNK = 128;                 // database positions per CTA of k_kfdb_count / k_kfdb_score, one per thread
+
+__global__ void k_kfdb_posmap(KfdbArgs A) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= A.ndb) return;
+    const int r = A.db[p];
+    if ((unsigned)r >= (unsigned)A.nrows || atomicCAS(A.pos_of_row + r, -1, p) != -1) atomicOr(A.err, 1);
+}
+
+// a query row outside [0, nrows), or (loop) a connected-keyframe range outside [0, nconn), fails the query; a bad database fails all
+template <bool kLoop>
+__device__ __forceinline__ bool kfdb_query_ok(const KfdbArgs& A, int q) {
+    if (*A.err != 0 || (unsigned)A.query[q] >= (unsigned)A.nrows) return false;
+    if (!kLoop) return true;
+    const int c0 = A.conn_off[q], c1 = A.conn_off[q + 1];
+    return 0 <= c0 && c0 <= c1 && c1 <= A.nconn;
+}
+
+__device__ __forceinline__ int block_max(int v, int* s_red) {
+    for (int o = 16; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    int m = 0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); w++) m = max(m, s_red[w]);
+    return m;
+}
+
+// minCommonWords = maxCommonWords * 0.8f, a float product truncated to int (KeyFrameDatabase.cc:132, 243)
+__device__ __forceinline__ int min_common_words(int maxw) { return (int)__fmul_rn((float)maxw, 0.8f); }
+
+// the query's BowVector into shared memory: cap values, then cap word ids; returns its length
+__device__ __forceinline__ int stage_query(const KfdbArgs& A, int qr, double* s_qv) {
+    const int cap = A.B.cap, nqw = bow_count(A.B, qr);
+    int32_t* s_qw = reinterpret_cast<int32_t*>(s_qv + cap);
+    for (int i = threadIdx.x; i < nqw; i += blockDim.x) { s_qv[i] = A.B.val[(long long)qr * cap + i]; s_qw[i] = A.B.word[(long long)qr * cap + i]; }
+    __syncthreads();
+    return nqw;
+}
+
+// Word counts and first common words of query blockIdx.y against KFDB_CHUNK database positions (a thread per position, a merge of the
+// query's BowVector, staged in shared memory, against the position's).  words[q][p] = mnLoopWords / mnRelocWords (0: not listed,
+// connected keyframes of a loop query included), cand[q][p] = the listed position's sort key (-1: not listed) for k_kfdb_accumulate,
+// score[q][p] = NaN until k_kfdb_score; the chunk's largest count goes to maxw[q].  A failed query leaves 0 / NaN / -1.
+template <bool kLoop>
+__global__ void __launch_bounds__(KFDB_CHUNK) k_kfdb_count(KfdbArgs A) {
+    extern __shared__ double s_qv[];
+    __shared__ int s_red[32];
+    __shared__ unsigned char s_conn[KFDB_CHUNK];
+    const int q = blockIdx.y, tid = threadIdx.x, p0 = blockIdx.x * KFDB_CHUNK, p = p0 + tid;
+    const long long qo = (long long)q * A.ndb;
+    const bool in = p < A.ndb;
+    if (in) { A.words[qo + p] = 0; A.score[qo + p] = __int_as_float(0x7fc00000); A.cand[qo + p] = -1; }
+    if (!kfdb_query_ok<kLoop>(A, q)) return;
+    s_conn[tid] = 0;
+    const int nqw = stage_query(A, A.query[q], s_qv);
+    if (kLoop) {                                  // GetConnectedKeyFrames() of the query: never listed (:98-108)
+        for (int c = A.conn_off[q] + tid; c < A.conn_off[q + 1]; c += blockDim.x) {
+            const int r = A.conn[c];
+            const int cp = (unsigned)r < (unsigned)A.nrows ? A.pos_of_row[r] : -1;
+            if (cp >= p0 && cp < p0 + KFDB_CHUNK) s_conn[cp - p0] = 1;
+        }
+        __syncthreads();
+    }
+    int cnt = 0;
+    if (in && !s_conn[tid]) {
+        const int32_t* s_qw = reinterpret_cast<const int32_t*>(s_qv + A.B.cap);
+        const int r = A.db[p];
+        const int32_t* dw = A.B.word + (long long)r * A.B.cap;
+        const int nd = bow_count(A.B, r);
+        int first = -1, i = 0, j = 0;
+        while (i < nqw && j < nd) {
+            const int a = s_qw[i], b = dw[j];
+            if (a == b) { if (cnt == 0) first = i; cnt++; i++; j++; }
+            else if (a < b) i++;
+            else j++;
+        }
+        A.words[qo + p] = cnt;
+        if (cnt) A.cand[qo + p] = (first << KFDB_POS_BITS) | p;
+    }
+    const int m = block_max(cnt, s_red);
+    if (tid == 0 && m > 0) atomicMax(A.maxw + q, m);
+}
+
+// mLoopScore / mRelocScore, si = (float)score(query, kf), of the positions of the chunk with more than minCommonWords common words
+template <bool kLoop>
+__global__ void __launch_bounds__(KFDB_CHUNK) k_kfdb_score(KfdbArgs A) {
+    extern __shared__ double s_qv[];
+    const int q = blockIdx.y, p = blockIdx.x * KFDB_CHUNK + threadIdx.x;
+    const long long qo = (long long)q * A.ndb;
+    if (!kfdb_query_ok<kLoop>(A, q)) return;
+    const bool need = p < A.ndb && A.words[qo + p] > min_common_words(A.maxw[q]);
+    if (!__syncthreads_or(need)) return;
+    const int nqw = stage_query(A, A.query[q], s_qv);
+    if (!need) return;
+    const long long o = (long long)A.db[p] * A.B.cap;
+    const double s = l1_sum(reinterpret_cast<const int32_t*>(s_qv + A.B.cap), s_qv, nqw, A.B.word + o, A.B.val + o, bow_count(A.B, A.db[p]));
+    A.score[qo + p] = __double2float_rn(__ddiv_rn(-s, 2.0));
+}
+
+// The covisibility accumulation, retention and deduplication of one query (CTA) (:146-201 loop, :259-313 reloc).  lScoreAndMatch is
+// the scored positions (loop: si >= minScore) in the order of their sort keys, sorted here in shared memory; accScore / pBestKF of an
+// entry depend on no other entry, so they are computed in parallel, and the first occurrence of each pBestKF in that order is found with
+// an atomicMin on the entry index in cand[q][pBestKF's position] before cand[q] receives the result.  Reloc: a listed neighbour this
+// query did not score reads the score of the latest earlier query of the call that scored it, else relocscore[row].
+template <bool kLoop>
+__global__ void __launch_bounds__(512) k_kfdb_accumulate(KfdbArgs A) {
+    extern __shared__ int s_ent[];                // per entry: sort key, then pBestKF's position; then accScore (floats)
+    __shared__ int s_red[33];
+    __shared__ int s_cnt;
+    const int q = blockIdx.x, tid = threadIdx.x, ndb = A.ndb;
+    const long long qo = (long long)q * ndb;
+    float* s_acc = reinterpret_cast<float*>(s_ent + ndb);
+    if (!kfdb_query_ok<kLoop>(A, q)) { if (tid == 0) A.ncand[q] = -1; return; }
+    const int minw = min_common_words(A.maxw[q]);
+    const float minScore = kLoop ? A.minscore[q] : 0.f;
+    if (tid == 0) s_cnt = 0;
+    __syncthreads();
+    for (int p = tid; p < ndb; p += blockDim.x)
+        if (A.words[qo + p] > minw && (!kLoop || A.score[qo + p] >= minScore)) s_ent[atomicAdd(&s_cnt, 1)] = A.cand[qo + p];
+    __syncthreads();
+    const int ne = s_cnt;
+    int P = 1;
+    while (P < ne) P <<= 1;
+    for (int k = 2; k <= P; k <<= 1)              // bitonic sort of ne keys; the missing tail of the power of two counts as +inf
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            for (int i = tid; i < ne; i += blockDim.x) {
+                const int l = (j == (k >> 1)) ? (i ^ (k - 1)) : (i ^ j);
+                if (l > i && l < ne) {
+                    const int a = s_ent[i], b = s_ent[l];
+                    if (a > b) { s_ent[i] = b; s_ent[l] = a; }
+                }
+            }
+            __syncthreads();
+        }
+    float best_acc = minScore;
+    for (int e = tid; e < ne; e += blockDim.x) {
+        const int p = s_ent[e] & ((1 << KFDB_POS_BITS) - 1);
+        const float si = A.score[qo + p];
+        float acc = si, bestScore = si;
+        int bestp = p;
+        const int32_t* nb = A.covis + (long long)A.db[p] * 10;
+        for (int c = 0; c < 10; c++) {
+            const int r2 = nb[c];
+            const int p2 = (unsigned)r2 < (unsigned)A.nrows ? A.pos_of_row[r2] : -1;
+            if (p2 < 0) continue;
+            const int w2 = A.words[qo + p2];
+            if (w2 <= (kLoop ? minw : 0)) continue;
+            float s2 = A.score[qo + p2];
+            if (!kLoop && w2 <= minw) {
+                int q2 = q - 1;
+                while (q2 >= 0 && isnan(A.score[(long long)q2 * ndb + p2])) q2--;
+                s2 = q2 >= 0 ? A.score[(long long)q2 * ndb + p2] : A.relocscore[r2];
+            }
+            acc = __fadd_rn(acc, s2);
+            if (s2 > bestScore) { bestp = p2; bestScore = s2; }
+        }
+        s_acc[e] = acc;
+        best_acc = fmaxf(best_acc, acc);
+        s_ent[e] = bestp;
+    }
+    for (int o = 16; o > 0; o >>= 1) best_acc = fmaxf(best_acc, __shfl_xor_sync(0xffffffffu, best_acc, o));
+    __syncthreads();
+    if ((tid & 31) == 0) s_red[tid >> 5] = __float_as_int(best_acc);
+    for (int p = tid; p < ndb; p += blockDim.x) A.cand[qo + p] = INT_MAX;
+    __syncthreads();
+    for (int w = 0; w < (int)(blockDim.x >> 5); w++) best_acc = fmaxf(best_acc, __int_as_float(s_red[w]));
+    const float keep = __fmul_rn(0.75f, best_acc);
+    for (int e = tid; e < ne; e += blockDim.x)
+        if (s_acc[e] > keep) atomicMin(A.cand + qo + s_ent[e], e);
+    __syncthreads();
+    for (int e = tid; e < ne; e += blockDim.x)     // s_acc[e] becomes the entry's output flag
+        s_acc[e] = (s_acc[e] > keep && A.cand[qo + s_ent[e]] == e) ? 1.f : 0.f;
+    __syncthreads();
+    int nout = 0;
+    for (int base = 0; base < ne; base += blockDim.x) {
+        const int e = base + tid;
+        const bool out = e < ne && s_acc[e] != 0.f;
+        int total;
+        const int o = nout + block_exclusive_scan(out ? 1 : 0, s_red, &total);
+        if (out) A.cand[qo + o] = A.db[s_ent[e]];
+        nout += total;
+    }
+    __syncthreads();
+    for (int p = nout + tid; p < ndb; p += blockDim.x) A.cand[qo + p] = -1;
+    if (tid == 0) A.ncand[q] = nout;
+}
+
+// After a reloc call: each database keyframe keeps the score of the last query that scored it (mRelocScore, :241).
+__global__ void k_kfdb_reloc_state(KfdbArgs A) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= A.ndb || *A.err) return;
+    for (int q = A.nq - 1; q >= 0; q--) {
+        const float s = A.score[(long long)q * A.ndb + p];
+        if (!isnan(s)) { A.relocscore[A.db[p]] = s; return; }
+    }
+}
+
 }  // namespace sslpl
 
 // =================================================================================================
@@ -1640,6 +1950,7 @@ using namespace sslpl;
 
 struct sslpl_vocab {
     int device = 0, k = 0, L = 0, nnodes = 0, nwords = 0;
+    int scoring = 0, weighting = 0;      // DBoW2 ScoringType / WeightingType: L1_NORM / TF_IDF unless a text file's header says otherwise
     uint8_t* arena = nullptr;
     sslpl::VocabView view{};
     std::vector<int> depth;              // per node
@@ -1894,6 +2205,13 @@ int matcher_init(sslpl_matcher* m) {
     // the two kernels with data-dependent dynamic shared memory may use the whole 227 KB of an sm_90 CTA
     SSLPL_CUDA(cudaFuncSetAttribute(k_bow_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
     SSLPL_CUDA(cudaFuncSetAttribute(k_build_csr, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
+    SSLPL_CUDA(cudaFuncSetAttribute(k_bow_vector, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
+    SSLPL_CUDA(cudaFuncSetAttribute(k_kfdb_count<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
+    SSLPL_CUDA(cudaFuncSetAttribute(k_kfdb_count<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
+    SSLPL_CUDA(cudaFuncSetAttribute(k_kfdb_score<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
+    SSLPL_CUDA(cudaFuncSetAttribute(k_kfdb_score<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
+    SSLPL_CUDA(cudaFuncSetAttribute(k_kfdb_accumulate<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
+    SSLPL_CUDA(cudaFuncSetAttribute(k_kfdb_accumulate<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
     return SSLPL_OK;
 }
 
@@ -2529,7 +2847,9 @@ int sslpl_vocab_load_text(int device, const char* path, sslpl_vocab** out, int* 
     fclose(f);
     if (scoring) *scoring = n1;
     if (weighting) *weighting = n2;
-    return sslpl_vocab_create(device, k, L, (int)parent.size(), parent.data(), desc.data(), weight.data(), leaf.data(), out);
+    if (int rc = sslpl_vocab_create(device, k, L, (int)parent.size(), parent.data(), desc.data(), weight.data(), leaf.data(), out)) return rc;
+    (*out)->scoring = n1; (*out)->weighting = n2;
+    return SSLPL_OK;
 }
 
 void sslpl_vocab_destroy(sslpl_vocab* v) {
@@ -2590,6 +2910,104 @@ int sslpl_match_bow_batch_device_vocab(sslpl_matcher* m, const uint8_t* d_desc, 
         launch(m, k_vocab_transform, grid, 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup, d_word, d_node, nullptr, d_weight, cap);
     launch(m, k_vocab_transform, grid, 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup, nullptr, nullptr, m->b_node, nullptr, fc);
     return bow_batch_tail(m, d_desc, d_kps, d_n, nframes, cap, nc, nnratio, checkOri, d_match, d_nmatch);
+}
+
+// ---------------- Keyframe database over a row set in HBM (KeyFrameDatabase.cc) ----------------
+// k_bow_vector keeps a power of two >= cap keys and cap weights (bow_rows_ok bounds them), k_kfdb_count / k_kfdb_score the query's
+// cap (word, value) pairs (12 cap bytes, less than the former), k_kfdb_accumulate 8 bytes per database position: each in one CTA's
+// shared memory.
+constexpr int KFDB_MAX_DB = MAX_DYN_SMEM / 8;
+static_assert(KFDB_MAX_DB <= (1 << KFDB_POS_BITS), "database positions must fit the sort key");
+static int bow_pow2(int cap) { int P = 1; while (P < cap) P <<= 1; return P; }
+
+static int bow_rows_ok(const sslpl_matcher* m, const int32_t* w, const double* v, const int32_t* n, int nrows, int cap) {
+    SSLPL_REQUIRE(m && w && v && n, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nrows >= 1, SSLPL_ERR_ARG, "nrows must be >= 1");
+    SSLPL_REQUIRE(cap >= 1 && cap <= m->p.max_features + 64, SSLPL_ERR_ARG, "cap outside [1, max_features + 64]");
+    SSLPL_REQUIRE((size_t)(bow_pow2(cap) + cap) * 8 <= (size_t)MAX_DYN_SMEM && cap < (1 << (31 - KFDB_POS_BITS)), SSLPL_ERR_ARG,
+                  "cap exceeds what one CTA's shared memory holds (a power of two >= cap, plus cap, times 8 bytes <= 200 KB)");
+    return SSLPL_OK;
+}
+
+int sslpl_bow_vectors_batch_device(sslpl_matcher* m, const sslpl_vocab* v, const uint8_t* d_desc, const int* d_n, int nrows, int cap,
+                                   int32_t* d_bow_word, double* d_bow_val, int32_t* d_bow_n) {
+    if (int rc = bow_rows_ok(m, d_bow_word, d_bow_val, d_bow_n, nrows, cap)) return rc;
+    SSLPL_REQUIRE(v && d_desc && d_n, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nrows <= 65535, SSLPL_ERR_ARG, "nrows exceeds 65535");
+    SSLPL_REQUIRE(v->device == m->p.device, SSLPL_ERR_ARG, "vocabulary and matcher live on different devices");
+    SSLPL_REQUIRE(v->scoring == 0 && v->weighting == 0, SSLPL_ERR_UNSUPPORTED, "BowVectors are built for TF_IDF weighting and L1 scoring only");
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    launch(m, k_vocab_transform, dim3((cap + 127) / 128, nrows), 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, 0,
+           d_bow_word, nullptr, nullptr, d_bow_val, cap);
+    const int P = bow_pow2(cap);
+    launch(m, k_bow_vector, nrows, 512, (size_t)(P + cap) * 8, BowRows{d_bow_word, d_bow_val, d_bow_n, cap}, d_n, P);
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+int sslpl_bow_score_batch_device(sslpl_matcher* m, const int32_t* d_bow_word, const double* d_bow_val, const int32_t* d_bow_n, int nrows,
+                                 int cap, int npairs, const int32_t* d_pair, double* d_score) {
+    if (int rc = bow_rows_ok(m, d_bow_word, d_bow_val, d_bow_n, nrows, cap)) return rc;
+    SSLPL_REQUIRE(d_pair && d_score, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(npairs >= 1, SSLPL_ERR_ARG, "npairs must be >= 1");
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    launch(m, k_bow_score, (npairs + 127) / 128, 128, 0, BowRows{const_cast<int32_t*>(d_bow_word), const_cast<double*>(d_bow_val),
+           const_cast<int32_t*>(d_bow_n), cap}, nrows, npairs, reinterpret_cast<const int2*>(d_pair), d_score);
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+// DetectLoopCandidates (kLoop) / DetectRelocalizationCandidates for nq queries: the row -> position map of the database, then the scores
+// of every query, then the accumulation of every query; reloc then leaves the keyframes' final scores in relocscore.
+extern "C++" {
+template <bool kLoop>
+int kfdb_detect(sslpl_matcher* m, KfdbArgs A) {
+    if (int rc = bow_rows_ok(m, A.B.word, A.B.val, A.B.n, A.nrows, A.B.cap)) return rc;
+    SSLPL_REQUIRE(A.db && A.query && A.covis && A.cand && A.ncand && A.words && A.score, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(kLoop ? (A.conn_off && A.conn && A.minscore) : A.relocscore != nullptr, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(A.ndb >= 1 && A.ndb <= KFDB_MAX_DB, SSLPL_ERR_ARG, "ndb outside [1, 25600]");
+    SSLPL_REQUIRE(A.nq >= 1 && A.nq <= 65535, SSLPL_ERR_ARG, "nq outside [1, 65535]");
+    SSLPL_REQUIRE(!kLoop || A.nconn >= 0, SSLPL_ERR_ARG, "nconn must be >= 0");
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    // scratch: the row -> position map, the error word, maxw[nq]
+    const size_t map_bytes = align_up((size_t)A.nrows * 4, 256);
+    if (int rc = ensure_scratch(m, map_bytes + 256 + (size_t)A.nq * 4)) return rc;
+    A.pos_of_row = reinterpret_cast<int32_t*>(m->scratch);
+    A.err = reinterpret_cast<int32_t*>(m->scratch + map_bytes);
+    A.maxw = reinterpret_cast<int32_t*>(m->scratch + map_bytes + 256);
+    fill(m, A.pos_of_row, A.nrows, -1);
+    SSLPL_CUDA(cudaMemsetAsync(A.err, 0, 256 + (size_t)A.nq * 4, m->stream));
+    launch(m, k_kfdb_posmap, (A.ndb + 255) / 256, 256, 0, A);
+    const dim3 chunks((A.ndb + KFDB_CHUNK - 1) / KFDB_CHUNK, A.nq);
+    launch(m, k_kfdb_count<kLoop>, chunks, KFDB_CHUNK, (size_t)A.B.cap * 12, A);
+    launch(m, k_kfdb_score<kLoop>, chunks, KFDB_CHUNK, (size_t)A.B.cap * 12, A);
+    launch(m, k_kfdb_accumulate<kLoop>, A.nq, 512, (size_t)A.ndb * 8, A);
+    if (!kLoop) launch(m, k_kfdb_reloc_state, (A.ndb + 255) / 256, 256, 0, A);
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+}  // extern "C++"
+
+int sslpl_detect_loop_candidates_batch_device(sslpl_matcher* m, const int32_t* d_bow_word, const double* d_bow_val, const int32_t* d_bow_n,
+        int nrows, int cap, const int32_t* d_db, int ndb, const int32_t* d_query, int nq, const int32_t* d_covis,
+        const int32_t* d_conn_off, const int32_t* d_conn, int nconn, const float* d_minscore,
+        int32_t* d_cand, int32_t* d_ncand, int32_t* d_words, float* d_score) {
+    KfdbArgs A; memset(&A, 0, sizeof(A));
+    A.B = BowRows{const_cast<int32_t*>(d_bow_word), const_cast<double*>(d_bow_val), const_cast<int32_t*>(d_bow_n), cap};
+    A.nrows = nrows; A.db = d_db; A.ndb = ndb; A.query = d_query; A.nq = nq; A.covis = d_covis;
+    A.conn_off = d_conn_off; A.conn = d_conn; A.nconn = nconn; A.minscore = d_minscore;
+    A.cand = d_cand; A.ncand = d_ncand; A.words = d_words; A.score = d_score;
+    return kfdb_detect<true>(m, A);
+}
+
+int sslpl_detect_relocalization_candidates_batch_device(sslpl_matcher* m, const int32_t* d_bow_word, const double* d_bow_val,
+        const int32_t* d_bow_n, int nrows, int cap, const int32_t* d_db, int ndb, const int32_t* d_query, int nq, const int32_t* d_covis,
+        float* d_relocscore, int32_t* d_cand, int32_t* d_ncand, int32_t* d_words, float* d_score) {
+    KfdbArgs A; memset(&A, 0, sizeof(A));
+    A.B = BowRows{const_cast<int32_t*>(d_bow_word), const_cast<double*>(d_bow_val), const_cast<int32_t*>(d_bow_n), cap};
+    A.nrows = nrows; A.db = d_db; A.ndb = ndb; A.query = d_query; A.nq = nq; A.covis = d_covis; A.relocscore = d_relocscore;
+    A.cand = d_cand; A.ncand = d_ncand; A.words = d_words; A.score = d_score;
+    return kfdb_detect<false>(m, A);
 }
 
 int sslpl_match_lines_batch_device(sslpl_matcher* m, const uint8_t* d_ldesc, const int* d_nl, int nframes, int capl,
