@@ -354,6 +354,45 @@ int  sslpl_detect_relocalization_candidates_batch_device(sslpl_matcher* m, const
         const int32_t* d_bow_n, int nrows, int cap, const int32_t* d_db, int ndb, const int32_t* d_query, int nq, const int32_t* d_covis,
         float* d_relocscore, int32_t* d_cand, int32_t* d_ncand, int32_t* d_words, float* d_score);
 
+/* ---- Tracking::Relocalization (Tracking.cc:1961-2121) on the device ----
+   sslpl_reloc_pairs_batch_device turns the candidate table of sslpl_detect_relocalization_candidates_batch_device into a pair list:
+   d_pair[q * kmax + k] = (d_cand[q][k], d_query[q]) for k < min(d_ncand[q], kmax, ndb), else (-1, -1).  The slot keeps the candidate's rank,
+   the order Relocalization walks; d_ncand[q] = -1 gives empty slots, and d_ncand[q] > kmax shows truncation.  Needs nq * kmax <=
+   max_batch.  Asynchronous; bad arguments return SSLPL_ERR_ARG and enqueue nothing. */
+int  sslpl_reloc_pairs_batch_device(sslpl_matcher* m, const int32_t* d_query, const int32_t* d_cand, const int32_t* d_ncand, int nq, int ndb,
+        int kmax, int32_t* d_pair);
+/* ORBmatcher::SearchByProjection(Frame &F, KeyFrame *pKF, const set<MapPoint*> &sAlreadyFound, th, ORBdist) (ORBmatcher.cc:1475-1602),
+   which Relocalization runs with ORBmatcher(0.9, true) after PnP and PoseOptimization, at (10, 100) and again at (3, 64).  F.mvpMapPoints
+   is read on entry and written.  One pair, host buffers.  Keyframe feature i: flag1[i] = vpMPs[i] && !isBad() && !sAlreadyFound.count(),
+   Xw[i][3] = GetWorldPos(), dmp[i][32] = GetDescriptor(), dist3[i][3] = GetMinDistanceInvariance(), GetMaxDistanceInvariance(),
+   mfMaxDistance, angle1[i] = mvKeysUn[i].angle.  Frame feature j: descriptor, mvKeysUn x / y / octave / angle, held2[j] =
+   mvpMapPoints[j] != NULL on entry (NULL = none).  Tcw = F.mTcw 3x4 row-major, cam = {fx, fy, cx, cy}, bounds = {mnMinX, mnMaxX, mnMinY,
+   mnMaxY}, the frame's mvScaleFactors[nlevels] and mfLogScaleFactor.  assign2[j] = the keyframe feature whose MapPoint was written to
+   mvpMapPoints[j], -1 untouched, -2 written and then NULLed by the rotation check; *nmatches = the return value.  There is no depth test:
+   a point behind the camera that projects inside the bounds is searched.  ORBdist >= 256 returns SSLPL_ERR_ARG (the reference would
+   write mvpMapPoints[-1] when a window holds no free feature). */
+int  sslpl_search_by_projection_kf(sslpl_matcher* m,
+        int n1, const uint8_t* flag1, const float* Xw, const uint8_t* dmp, const float* dist3, const float* angle1,
+        int n2, const uint8_t* d2, const float* x2, const float* y2, const int32_t* oct2, const float* angle2, const uint8_t* held2,
+        const float* Tcw, const float* cam, const float* bounds, const float* scaleFactors, int nlevels, float logScaleFactor,
+        float th, int ORBdist, int checkOrientation, int32_t* assign2, int* nmatches);
+/* The same matcher over pairs of a row set in HBM, asynchronous on the handle's stream.  Rows (frames and keyframes alike, nrows <=
+   65535) in the extractors' layout: d_kps[r][cap] = mvKeysUn, d_desc[r][cap][32], d_n[r] (clamped to [0, cap]).  Map: d_kfmp[r][cap] =
+   GetMapPointMatches() as element indices (-1 or any index outside [0, nmp) = NULL), d_mpbad[m] = isBad() (NULL = none), d_mp[m][9] =
+   Xw, normal, GetMinDistanceInvariance(), GetMaxDistanceInvariance(), mfMaxDistance and d_mpdesc[m][32] (the table of
+   sslpl_fuse_points_batch_device).  Pair p: d_pair[p] = (keyframe row, frame row), d_Tcw[p][12] = the frame's pose for that candidate,
+   d_found[p][cap] over keyframe features = sAlreadyFound.count(vpMPs[i]) (NULL = none), d_held[p][cap] over frame features =
+   mvpMapPoints[j] != NULL on entry (NULL = none).  Results: d_assign[p][cap] as assign2 above (-1 past the frame's count), d_nmatch[p];
+   a pair with a row outside [0, nrows) gets d_nmatch -1 and no assignment.  Needs npairs <= max_batch and cap <= max_features + 64; the
+   first call of either form allocates a workspace of max_batch pairs, freed with the handle.  Bad host arguments return SSLPL_ERR_ARG and
+   enqueue nothing. */
+int  sslpl_search_by_projection_kf_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nrows, int cap,
+        const int32_t* d_kfmp, const uint8_t* d_mpbad, int nmp, const float* d_mp, const uint8_t* d_mpdesc,
+        int npairs, const int32_t* d_pair, const float* d_Tcw, const uint8_t* d_found, const uint8_t* d_held,
+        const float* cam, const float* bounds, const float* scaleFactors, int nlevels, float logScaleFactor,
+        float th, int ORBdist, int checkOrientation, int32_t* d_assign, int32_t* d_nmatch);
+
 /* Batched line matching in HBM: knn2 + ratio rule of LSDmatcher::SearchByProjection(KF,F) (:143-183) with all
    KF lines valid: d_lmatch[p*capl + tdx] = qdx or -1; d_nlmatch[p]. */
 int  sslpl_match_lines_batch_device(sslpl_matcher* m, const uint8_t* d_ldesc, const int* d_nl, int nframes, int capl,

@@ -585,6 +585,42 @@ class Matcher(_Handle, kind="matcher", lifecycle=("sync", "set_stream", "stream"
                                                                          d_query, nq, d_covis, d_relocscore, d_cand, d_ncand, d_words,
                                                                          d_score))
 
+    def reloc_pairs_batch_device(self, d_query, d_cand, d_ncand, nq, ndb, kmax, d_pair):
+        """The candidate table of detect_relocalization_candidates_batch_device as pairs: d_pair [nq * kmax, 2] i32 = (candidate row,
+        query row) in rank order, (-1, -1) past min(ncand, kmax).  Asynchronous on the matcher's stream."""
+        _check(lib().sslpl_reloc_pairs_batch_device(self._h, d_query, d_cand, d_ncand, nq, ndb, kmax, d_pair))
+
+    def search_by_projection_kf(self, kf, cur, Tcw, cam, bounds, scale_factors, log_scale_factor, th, orb_dist, check_ori=True):
+        """ORBmatcher::SearchByProjection(Frame &F, KeyFrame *pKF, sAlreadyFound, th, ORBdist) (ORBmatcher.cc:1475-1602).
+        kf = dict(flag (MapPoint, not bad, not already found), Xw[n,3], dmp[n,32], dist3[n,3] (minInv, maxInv, mfMaxDistance), angle);
+        cur = dict(desc[n,32], x, y, oct, angle, held|None); Tcw 3x4 (or 4x4); cam = (fx, fy, cx, cy); bounds = (minX, maxX, minY, maxY).
+        Returns (nmatches, assign2): assign2[j] = keyframe feature written to mvpMapPoints[j], -1 untouched, -2 removed by the rotation
+        check."""
+        n1, n2 = len(kf["flag"]), len(cur["x"])
+        fl = _u8(kf["flag"]); Xw = _f32(kf["Xw"]).reshape(-1, 3); dmp = _u8(kf["dmp"]).reshape(-1, 32)
+        d3 = _f32(kf["dist3"]).reshape(-1, 3); a1 = _f32(kf["angle"])
+        d2 = _u8(cur["desc"]).reshape(-1, 32)
+        sf = _f32(scale_factors)
+        out = np.full(max(n2, 1), -1, np.int32); nm = C.c_int()
+        _check(lib().sslpl_search_by_projection_kf(self._h, n1, _p(fl), _p(Xw), _p(dmp), _p(d3), _p(a1), n2, _p(d2), _p(_f32(cur["x"])),
+                                                   _p(_f32(cur["y"])), _p(_i32(cur["oct"])), _p(_f32(cur["angle"])), _p(_u8(cur.get("held"))),
+                                                   _p(_f32(Tcw).reshape(-1)[:12].copy()), _p(_f32(cam)[:4].copy()), _p(_f32(bounds)), _p(sf),
+                                                   len(sf), log_scale_factor, th, orb_dist, int(check_ori), _p(out), C.byref(nm)))
+        return nm.value, out[:n2]
+
+    def search_by_projection_kf_batch_device(self, d_kps, d_desc, d_n, nrows, cap, d_kfmp, d_mpbad, nmp, d_mp, d_mpdesc, npairs, d_pair,
+                                             d_Tcw, d_found, d_held, cam, bounds, scale_factors, log_scale_factor, th, orb_dist,
+                                             check_ori, d_assign, d_nmatch):
+        """SearchByProjection(Frame, KeyFrame, sAlreadyFound, th, ORBdist) over (keyframe row, frame row) pairs of a row set in HBM:
+        d_kfmp [nrows, cap] i32 element indices (-1 NULL), d_mpbad [nmp] u8 or 0, d_mp [nmp, 9] f32 / d_mpdesc [nmp, 32] (the Fuse
+        table), d_pair [npairs, 2] i32, d_Tcw [npairs, 12] f32, d_found [npairs, cap] u8 or 0, d_held [npairs, cap] u8 or 0 ->
+        d_assign [npairs, cap] i32, d_nmatch [npairs] i32 (-1 for a pair outside the rows).  Asynchronous on the matcher's stream."""
+        sf = _f32(scale_factors)
+        _check(lib().sslpl_search_by_projection_kf_batch_device(
+            self._h, d_kps, d_desc, d_n, nrows, cap, d_kfmp, d_mpbad or None, nmp, d_mp, d_mpdesc, npairs, d_pair, d_Tcw, d_found or None,
+            d_held or None, _p(_f32(cam)[:4].copy()), _p(_f32(bounds)), _p(sf), len(sf), log_scale_factor, th, orb_dist, int(check_ori),
+            d_assign, d_nmatch))
+
     def debug_predict_scale(self, ratio, log_scale_factor, nlevels, clamp=True):
         """MapPoint / MapLine::PredictScale on the device for host ratios (see sslpl_matcher_debug_predict_scale) -> int32 levels."""
         r = _f32(ratio).reshape(-1)

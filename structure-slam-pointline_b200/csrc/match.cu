@@ -1943,6 +1943,155 @@ __global__ void k_kfdb_reloc_state(KfdbArgs A) {
     }
 }
 
+// -------------------------------------------------------------------------------------------------
+// Tracking::Relocalization (Tracking.cc:1961-2121) on the device.  k_reloc_pairs turns DetectRelocalizationCandidates' table into
+// (candidate keyframe row, query row) pairs, slot q * kmax + k for the candidate of rank k; (-1, -1) past min(ncand[q], kmax, ndb).
+// -------------------------------------------------------------------------------------------------
+__global__ void k_reloc_pairs(int nq, const int32_t* query, const int32_t* cand, const int32_t* ncand, int ndb, int kmax, int2* pair) {
+    const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= (long long)nq * kmax) return;
+    const int q = (int)(s / kmax), k = (int)(s % kmax);
+    pair[s] = k < min(ncand[q], min(kmax, ndb)) ? make_int2(cand[(long long)q * ndb + k], query[q]) : make_int2(-1, -1);
+}
+
+// ORBmatcher::SearchByProjection(Frame &F, KeyFrame *pKF, sAlreadyFound, th, ORBdist) — ORBmatcher.cc:1475-1602, run after PnP and
+// PoseOptimization on each candidate.  Pair p = (keyframe row, frame row) of a row set (sslpl_keypoint rows, descriptors, counts, all of
+// stride cap); the keyframe's MapPoints are element indices kfmp[row][i] into el[m][9] = Xw, normal, GetMinDistanceInvariance(),
+// GetMaxDistanceInvariance(), mfMaxDistance and eldesc[m][32] (the Fuse / map-refresh element table).
+struct RelocArgs {
+    float fx, fy, cx, cy, minX, maxX, minY, maxY, invW, invH, th;
+    int ORBdist, checkOri;
+    float scale[SSLPL_MAX_LEVELS];                   // the frame's mvScaleFactors
+    PredictTable T;                                  // MapPoint::PredictScale(dist, Frame*) (MapPoint.cc:407-422) with the frame's mfLogScaleFactor
+};
+struct RelocSet {
+    const int2* pair; int npairs, nrows, cap;
+    const float* kp; const uint8_t* desc; const int* n;               // row r at kp + 7 cap r, desc + 32 cap r; n[r] clamped to [0, cap]
+    const int32_t* kfmp; const uint8_t* mpbad; const float* el; const uint8_t* eldesc; int nel;
+    const float* Tcw;                                // pair p's pose at Tcw + 12 p
+    const uint8_t* found; const uint8_t* held;       // [p][cap]: sAlreadyFound.count(vpMPs[i]), F.mvpMapPoints[j] != NULL (NULL = none)
+    float* xy; int* wn; const int* goff; const int* gidx; long long goff_fs;   // per pair: the frame's (x, y) rows and count, its grid CSR
+    uint8_t* claimed; int32_t* sel; uint8_t* rbin; long long ws_fs;            // per pair walker tables
+    int32_t* assign; int32_t* nmatch;                // [p][cap], [p]
+};
+
+__device__ __forceinline__ bool reloc_pair(const RelocSet& R, int p, int& kr, int& fr) {
+    const int2 q = R.pair[p];
+    kr = q.x; fr = q.y;
+    return (unsigned)kr < (unsigned)R.nrows && (unsigned)fr < (unsigned)R.nrows;
+}
+__device__ __forceinline__ int reloc_count(const RelocSet& R, int r) { return min(max(R.n[r], 0), R.cap); }
+
+// The (x, y) of pair p's frame rows into the pair's slot, for k_grid_cells / k_build_csr (an invalid pair gets no features)
+__global__ void __launch_bounds__(128) k_reloc_gather_xy(const __grid_constant__ RelocSet R) {
+    const int p = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+    int kr, fr;
+    const bool ok = reloc_pair(R, p, kr, fr);
+    const int n = ok ? reloc_count(R, fr) : 0;
+    if (i == 0) R.wn[p] = n;
+    if (i >= n) return;
+    const float* k = R.kp + 7LL * R.cap * fr + 7LL * i;
+    R.xy[(long long)p * 2 * R.ws_fs + 2 * i] = k[0];
+    R.xy[(long long)p * 2 * R.ws_fs + 2 * i + 1] = k[1];
+}
+
+// One warp per pair.  The keyframe's MapPoints are walked in index order (an assignment makes the frame feature unavailable to later
+// points); the lanes share each search window.
+__global__ void __launch_bounds__(32) k_proj_match_kf(const __grid_constant__ RelocArgs A, const __grid_constant__ RelocSet R) {
+    __shared__ int s_hist[HISTO_LENGTH];
+    __shared__ int s_keep[3];
+    __shared__ float s_T[12], s_Ow[3];
+    const int lane = threadIdx.x, p = blockIdx.x;
+    int32_t* assign = R.assign + (long long)p * R.cap;
+    for (int j = lane; j < R.cap; j += 32) assign[j] = -1;
+    int kr, fr;
+    if (!reloc_pair(R, p, kr, fr)) { if (lane == 0) R.nmatch[p] = -1; return; }
+    const int n1 = reloc_count(R, kr), n2 = reloc_count(R, fr);
+    const float* kp1 = R.kp + 7LL * R.cap * kr; const float* kp2 = R.kp + 7LL * R.cap * fr;
+    const uint8_t* d2 = R.desc + 32LL * R.cap * fr;
+    const int32_t* kfmp = R.kfmp + (long long)R.cap * kr;
+    const uint8_t* found = R.found ? R.found + (long long)p * R.cap : nullptr;
+    const uint8_t* held = R.held ? R.held + (long long)p * R.cap : nullptr;
+    const int* goff = R.goff + p * R.goff_fs; const int* gidx = R.gidx + p * R.ws_fs;
+    uint8_t* claimed = R.claimed + p * R.ws_fs; int32_t* sel = R.sel + p * R.ws_fs; uint8_t* rbin = R.rbin + p * R.ws_fs;
+    if (lane < 12) s_T[lane] = R.Tcw[12LL * p + lane];
+    if (lane < HISTO_LENGTH) s_hist[lane] = 0;
+    for (int j = lane; j < n2; j += 32) claimed[j] = held && held[j] ? 1 : 0;         // a frame feature holding any MapPoint is skipped (:1543)
+    __syncwarp();
+    // Ow = -Rcw.t()*tcw (:1480): a transposed operand takes cv::gemm's general path, double accumulation (as twc in k_proj_match)
+    if (lane < 3) s_Ow[lane] = __double2float_rn(-__dadd_rn(__dadd_rn(__dmul_rn((double)s_T[lane], (double)s_T[3]),
+                                                                     __dmul_rn((double)s_T[4 + lane], (double)s_T[7])),
+                                                           __dmul_rn((double)s_T[8 + lane], (double)s_T[11])));
+    __syncwarp();
+    const float* T = s_T;
+    int nmatches = 0;
+    for (int i = 0; i < n1; i++) {
+        if (lane == 0) sel[i] = -1;
+        const int e = kfmp[i];
+        if ((unsigned)e >= (unsigned)R.nel) continue;                                  // NULL (:1497)
+        if ((R.mpbad && R.mpbad[e]) || (found && found[i])) continue;                  // :1499
+        const float* P = R.el + 9LL * e;
+        const float X0 = P[0], X1 = P[1], X2 = P[2];
+        // no depth test: a point behind the camera is searched when it projects inside the bounds; z = 0 gives inf / NaN, which either
+        // fails the bounds or finds no feature in the window (every comparison with NaN is false)
+        const float xc = rt_row(T, X0, X1, X2), yc = rt_row(T + 4, X0, X1, X2), zc = rt_row(T + 8, X0, X1, X2);
+        const float invzc = (float)(1.0 / (double)zc);
+        const float u = __fadd_rn(__fmul_rn(__fmul_rn(A.fx, xc), invzc), A.cx), v = __fadd_rn(__fmul_rn(__fmul_rn(A.fy, yc), invzc), A.cy);
+        if (u < A.minX || u > A.maxX || v < A.minY || v > A.maxY) continue;
+        const float dist3D = norm3d(__fsub_rn(X0, s_Ow[0]), __fsub_rn(X1, s_Ow[1]), __fsub_rn(X2, s_Ow[2]));
+        if (dist3D < P[6] || dist3D > P[7]) continue;                                 // :1523-1524
+        const int lvl = predict_scale(__fdiv_rn(P[8], dist3D), A.T.thr, A.T.nlevels, true);
+        const float r = __fmul_rn(A.th, A.scale[lvl]);
+        int cx0, cx1, cy0, cy1;                                                        // GetFeaturesInArea(u, v, r, lvl - 1, lvl + 1)
+        if (!grid_window(A.minX, A.minY, A.invW, A.invH, u, v, r, cx0, cx1, cy0, cy1)) continue;
+        const int ny = cy1 - cy0 + 1, ncell = (cx1 - cx0 + 1) * ny;
+        uint4 a0, a1;
+        load_desc(R.eldesc + 32LL * e, a0, a1);
+        unsigned long long best = ~0ull;                                               // (dist << 40) | (cell rank << 20) | position in the cell
+        for (int c = lane; c < ncell; c += 32) {
+            const int cell = (cx0 + c / ny) * GRID_ROWS + cy0 + c % ny;
+            const int b = goff[cell], en = goff[cell + 1];
+            for (int q = b; q < en; q++) {
+                const int j = gidx[q];
+                const int o = __float_as_int(kp2[7LL * j + 5]);
+                if (o < lvl - 1 || o > lvl + 1) continue;
+                if (!(fabsf(__fsub_rn(kp2[7LL * j], u)) < r && fabsf(__fsub_rn(kp2[7LL * j + 1], v)) < r)) continue;
+                if (claimed[j]) continue;
+                uint4 b0, b1;
+                load_desc(d2 + 32LL * j, b0, b1);
+                const unsigned long long key = ((unsigned long long)popc256(a0, a1, b0, b1) << 40) | ((unsigned long long)c << 20) | (unsigned)(q - b);
+                if (key < best) best = key;
+            }
+        }
+        best = warp_min(best);
+        if (best != ~0ull && (int)(best >> 40) <= A.ORBdist) {                        // :1561 (ORBdist < 256: no candidate never passes)
+            const int j = grid_key_feature(goff, gidx, cx0, cy0, ny, best);
+            if (lane == 0) {
+                assign[j] = i; claimed[j] = 1; sel[i] = j;
+                const int bin = rot_bin(kp1[7LL * i + 3], kp2[7LL * j + 3]);             // pKF->mvKeysUn[i].angle - F.mvKeysUn[j].angle (:1568)
+                rbin[i] = (uint8_t)bin;
+                if (A.checkOri) s_hist[bin]++;
+            }
+            nmatches++;
+        }
+        __syncwarp();
+    }
+    __syncwarp();
+    if (A.checkOri) {
+        if (lane == 0) { const int3 k = three_maxima(s_hist); s_keep[0] = k.x; s_keep[1] = k.y; s_keep[2] = k.z; }
+        __syncwarp();
+        const int k0 = s_keep[0], k1 = s_keep[1], k2 = s_keep[2];
+        for (int i0 = 0; i0 < n1; i0 += 32) {
+            const int i = i0 + lane;
+            bool drop = false;
+            if (i < n1 && sel[i] >= 0) { const int b = rbin[i]; drop = (b != k0 && b != k1 && b != k2); }
+            if (drop) assign[sel[i]] = -2;                                             // assigned, then NULLed by the rotation check (:1595)
+            nmatches -= __popc(__ballot_sync(0xffffffffu, drop));
+        }
+    }
+    if (lane == 0) R.nmatch[p] = nmatches;
+}
+
 }  // namespace sslpl
 
 // =================================================================================================
@@ -1974,6 +2123,13 @@ struct sslpl_matcher : sslpl::StreamHandle {
     int32_t* tw = nullptr;
     // per-pair row table of sslpl_create_new_map_lines_batch_device ([max_batch][max_lines + 64]), allocated by its first call
     int32_t* ltw = nullptr;
+    // workspace of the SearchByProjection(Frame, KeyFrame) calls, allocated by the first one: per pair ([max_batch][cap]) the frame's
+    // (x, y) rows, grid cells and CSR and the walker's tables; the single call's element table, pair and pose
+    uint8_t* rw = nullptr;
+    float* rw_xy = nullptr; int* rw_n = nullptr; int32_t* rw_cell = nullptr; int* rw_off = nullptr; int* rw_idx = nullptr;
+    int32_t* rw_sel = nullptr; uint8_t* rw_claimed = nullptr; uint8_t* rw_rbin = nullptr;
+    float* rw_el = nullptr; uint8_t* rw_eldesc = nullptr; int32_t* rw_kfmp = nullptr; int32_t* rw_pair = nullptr; float* rw_T = nullptr;
+    int32_t* rw_nmatch = nullptr;
 };
 
 namespace {
@@ -2098,6 +2254,23 @@ int grid_batch_build(sslpl_matcher* m, const float* kp, const int* n, int nframe
     const int fc = m->p.max_features + 64, nc = GRID_COLS * GRID_ROWS;
     launch(m, k_grid_cells, dim3((cap + 127) / 128, nframes), 128, 0, kp, kp + 1, 7, 7LL * cap, n, 0, cap, minX, minY, invW, invH, m->pw_cell, fc);
     launch(m, k_build_csr, nframes, 128, (nc + 1 + cap) * sizeof(int), m->pw_cell, fc, n, cap, nc, m->pw_off, nc + 1, m->pw_idx, fc);
+    return SSLPL_OK;
+}
+
+int ensure_reloc_ws(sslpl_matcher* m) {
+    const int B = m->p.max_batch, W = m->cap, nc = GRID_COLS * GRID_ROWS;
+    Arena A;
+    for (int k = 0; k < 2; k++) {
+        m->rw_xy = A.take<float>((size_t)B * W * 2); m->rw_n = A.take<int>(B); m->rw_cell = A.take<int32_t>((size_t)B * W);
+        m->rw_off = A.take<int>((size_t)B * (nc + 1)); m->rw_idx = A.take<int>((size_t)B * W);
+        m->rw_sel = A.take<int32_t>((size_t)B * W); m->rw_claimed = A.take<uint8_t>((size_t)B * W); m->rw_rbin = A.take<uint8_t>((size_t)B * W);
+        m->rw_el = A.take<float>((size_t)W * 9); m->rw_eldesc = A.take<uint8_t>((size_t)W * 32); m->rw_kfmp = A.take<int32_t>((size_t)2 * W);
+        m->rw_pair = A.take<int32_t>(2); m->rw_T = A.take<float>(12); m->rw_nmatch = A.take<int32_t>(1);
+        if (k == 0) {
+            if (int rc = first_use(m->rw, A.used)) return rc;
+            A.base = m->rw; A.size = A.used; A.used = 0;
+        }
+    }
     return SSLPL_OK;
 }
 
@@ -2240,6 +2413,7 @@ void sslpl_matcher_destroy(sslpl_matcher* m) {
     if (m->pw) cudaFree(m->pw);
     if (m->tw) cudaFree(m->tw);
     if (m->ltw) cudaFree(m->ltw);
+    if (m->rw) cudaFree(m->rw);
     delete m;
 }
 
@@ -3326,6 +3500,132 @@ int sslpl_update_map_lines_batch_device(sslpl_matcher* m,
     U.nkf = nkf; U.pose = d_kfpose; U.kfbad = d_kfbad; U.el = d_ml; U.eldesc = d_mldesc; U.pos = d_mlpos; U.nrm64 = d_mlnormal;
     U.what = what; U.status = d_status;
     return map_update(m, k_map_update<true>, U, m->p.max_lines, nml, d_ml && d_mlpos, scaleFactors, nlevels, d_elem, d_refkf, d_obs_off, d_obs, nupd);
+}
+
+// The arguments of SearchByProjection(Frame, KeyFrame) common to the single and the batched call
+static int reloc_args(RelocArgs& A, const float* cam, const float* bounds, const float* scaleFactors, int nlevels, float logScaleFactor, float th,
+               int ORBdist, int checkOri) {
+    SSLPL_REQUIRE(cam && bounds && scaleFactors, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nlevels >= 1 && nlevels <= SSLPL_MAX_LEVELS, SSLPL_ERR_ARG, "nlevels outside [1, SSLPL_MAX_LEVELS]");
+    SSLPL_REQUIRE(bounds[1] > bounds[0] && bounds[3] > bounds[2], SSLPL_ERR_ARG, "degenerate image bounds");
+    SSLPL_REQUIRE(th > 0.f, SSLPL_ERR_ARG, "th must be positive");
+    // with no candidate in the window bestDist stays 256 and bestIdx2 -1: ORBdist >= 256 would make the reference write mvpMapPoints[-1]
+    SSLPL_REQUIRE(ORBdist < 256, SSLPL_ERR_ARG, "ORBdist must be below 256");
+    memset(&A, 0, sizeof(A));
+    if (int rc = predict_table(A.T, logScaleFactor, nlevels)) return rc;
+    A.fx = cam[0]; A.fy = cam[1]; A.cx = cam[2]; A.cy = cam[3];
+    A.minX = bounds[0]; A.maxX = bounds[1]; A.minY = bounds[2]; A.maxY = bounds[3];
+    A.invW = (float)GRID_COLS / (bounds[1] - bounds[0]); A.invH = (float)GRID_ROWS / (bounds[3] - bounds[2]);   // Frame.cc:115-116
+    A.th = th; A.ORBdist = ORBdist; A.checkOri = checkOri ? 1 : 0;
+    for (int k = 0; k < nlevels; k++) A.scale[k] = scaleFactors[k];
+    return SSLPL_OK;
+}
+
+// The grid of every pair's frame (AssignFeaturesToGrid over the pair's gathered rows), then one walker warp per pair.  R's row set, map,
+// pairs and outputs are set; the workspace is ensure_reloc_ws's.
+static int reloc_run(sslpl_matcher* m, const RelocArgs& A, RelocSet& R) {
+    const int nc = GRID_COLS * GRID_ROWS, W = m->cap;
+    R.xy = m->rw_xy; R.wn = m->rw_n; R.goff = m->rw_off; R.gidx = m->rw_idx; R.goff_fs = nc + 1;
+    R.claimed = m->rw_claimed; R.sel = m->rw_sel; R.rbin = m->rw_rbin; R.ws_fs = W;
+    launch(m, k_reloc_gather_xy, dim3((R.cap + 127) / 128, R.npairs), 128, 0, R);
+    launch(m, k_grid_cells, dim3((R.cap + 127) / 128, R.npairs), 128, 0, m->rw_xy, m->rw_xy + 1, 2, 2LL * W, m->rw_n, 0, R.cap,
+           A.minX, A.minY, A.invW, A.invH, m->rw_cell, (long long)W);
+    launch(m, k_build_csr, R.npairs, 128, (nc + 1 + R.cap) * sizeof(int), m->rw_cell, (long long)W, m->rw_n, R.cap, nc, m->rw_off,
+           (long long)(nc + 1), m->rw_idx, (long long)W);
+    launch(m, k_proj_match_kf, R.npairs, 32, 0, A, R);
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+
+int sslpl_search_by_projection_kf(sslpl_matcher* m,
+        int n1, const uint8_t* flag1, const float* Xw, const uint8_t* dmp, const float* dist3, const float* angle1,
+        int n2, const uint8_t* d2, const float* x2, const float* y2, const int32_t* oct2, const float* angle2, const uint8_t* held2,
+        const float* Tcw, const float* cam, const float* bounds, const float* scaleFactors, int nlevels, float logScaleFactor,
+        float th, int ORBdist, int checkOrientation, int32_t* assign2, int* nmatches) {
+    SSLPL_REQUIRE(m && Tcw && assign2 && nmatches, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(n1 >= 0 && n2 >= 0 && n1 <= m->p.max_features && n2 <= m->p.max_features, SSLPL_ERR_ARG, "feature count exceeds max_features");
+    SSLPL_REQUIRE(n1 == 0 || (flag1 && Xw && dmp && dist3 && angle1), SSLPL_ERR_ARG, "null keyframe array");
+    SSLPL_REQUIRE(n2 == 0 || (d2 && x2 && y2 && oct2 && angle2), SSLPL_ERR_ARG, "null frame array");
+    RelocArgs A;
+    if (int rc = reloc_args(A, cam, bounds, scaleFactors, nlevels, logScaleFactor, th, ORBdist, checkOrientation)) return rc;
+    const int W = m->cap, nc = GRID_COLS * GRID_ROWS;
+    if (int rc = csr_fits(nc, W)) return rc;
+    for (int j = 0; j < n2; j++) assign2[j] = -1;
+    *nmatches = 0;
+    if (n1 == 0 || n2 == 0) return SSLPL_OK;
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    if (int rc = ensure_reloc_ws(m)) return rc;
+    cudaStream_t st = m->stream;
+    // row 0 = the keyframe (mvKeysUn angles), row 1 = the frame; MapPoint i of the keyframe is element i
+    std::vector<sslpl_keypoint> kp((size_t)W + n2);
+    memset(kp.data(), 0, kp.size() * sizeof(sslpl_keypoint));
+    for (int i = 0; i < n1; i++) kp[i].angle = angle1[i];
+    for (int j = 0; j < n2; j++) { sslpl_keypoint& k = kp[(size_t)W + j]; k.x = x2[j]; k.y = y2[j]; k.octave = oct2[j]; k.angle = angle2[j]; }
+    std::vector<float> el((size_t)n1 * 9, 0.f);
+    std::vector<int32_t> kfmp(n1), misc = {n1, n2, 0, 1};
+    for (int i = 0; i < n1; i++) {
+        kfmp[i] = flag1[i] ? i : -1;
+        for (int c = 0; c < 3; c++) { el[9 * (size_t)i + c] = Xw[3 * (size_t)i + c]; el[9 * (size_t)i + 6 + c] = dist3[3 * (size_t)i + c]; }
+    }
+    SSLPL_CUDA(cudaMemcpyAsync(m->kpf, kp.data(), kp.size() * sizeof(sslpl_keypoint), cudaMemcpyHostToDevice, st));
+    SSLPL_CUDA(cudaMemcpyAsync(m->desc + 32LL * W, d2, (size_t)n2 * 32, cudaMemcpyHostToDevice, st));
+    SSLPL_CUDA(cudaMemcpyAsync(m->ncnt, misc.data(), 2 * sizeof(int), cudaMemcpyHostToDevice, st));
+    SSLPL_CUDA(cudaMemcpyAsync(m->rw_pair, misc.data() + 2, 2 * sizeof(int), cudaMemcpyHostToDevice, st));
+    SSLPL_CUDA(cudaMemcpyAsync(m->rw_T, Tcw, 12 * sizeof(float), cudaMemcpyHostToDevice, st));
+    SSLPL_CUDA(cudaMemcpyAsync(m->rw_kfmp, kfmp.data(), (size_t)n1 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    SSLPL_CUDA(cudaMemcpyAsync(m->rw_el, el.data(), el.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+    SSLPL_CUDA(cudaMemcpyAsync(m->rw_eldesc, dmp, (size_t)n1 * 32, cudaMemcpyHostToDevice, st));
+    if (held2) SSLPL_CUDA(cudaMemcpyAsync(m->flag, held2, n2, cudaMemcpyHostToDevice, st));
+    RelocSet R; memset(&R, 0, sizeof(R));
+    R.pair = reinterpret_cast<const int2*>(m->rw_pair); R.npairs = 1; R.nrows = 2; R.cap = W;
+    R.kp = m->kpf; R.desc = m->desc; R.n = m->ncnt;
+    R.kfmp = m->rw_kfmp; R.el = m->rw_el; R.eldesc = m->rw_eldesc; R.nel = n1;
+    R.Tcw = m->rw_T; R.held = held2 ? m->flag : nullptr;
+    R.assign = m->out; R.nmatch = m->rw_nmatch;
+    if (int rc = reloc_run(m, A, R)) return rc;
+    SSLPL_CUDA(cudaMemcpyAsync(assign2, m->out, sizeof(int32_t) * n2, cudaMemcpyDeviceToHost, st));
+    SSLPL_CUDA(cudaMemcpyAsync(m->h_small, m->rw_nmatch, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    SSLPL_CUDA(cudaStreamSynchronize(st));
+    *nmatches = m->h_small[0];
+    return SSLPL_OK;
+}
+
+int sslpl_search_by_projection_kf_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nrows, int cap,
+        const int32_t* d_kfmp, const uint8_t* d_mpbad, int nmp, const float* d_mp, const uint8_t* d_mpdesc,
+        int npairs, const int32_t* d_pair, const float* d_Tcw, const uint8_t* d_found, const uint8_t* d_held,
+        const float* cam, const float* bounds, const float* scaleFactors, int nlevels, float logScaleFactor,
+        float th, int ORBdist, int checkOrientation, int32_t* d_assign, int32_t* d_nmatch) {
+    SSLPL_REQUIRE(m && d_kps && d_desc && d_n && d_kfmp && d_pair && d_Tcw && d_assign && d_nmatch, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nmp >= 0 && (nmp == 0 || (d_mp && d_mpdesc)), SSLPL_ERR_ARG, "null element table");
+    SSLPL_REQUIRE(nrows >= 1 && nrows <= 65535, SSLPL_ERR_ARG, "nrows outside [1, 65535]");
+    SSLPL_REQUIRE(cap >= 1 && cap <= m->p.max_features + 64, SSLPL_ERR_ARG, "cap outside [1, max_features + 64]");
+    SSLPL_REQUIRE(npairs >= 1 && npairs <= m->p.max_batch, SSLPL_ERR_ARG, "npairs outside [1, max_batch]");
+    RelocArgs A;
+    if (int rc = reloc_args(A, cam, bounds, scaleFactors, nlevels, logScaleFactor, th, ORBdist, checkOrientation)) return rc;
+    if (int rc = csr_fits(GRID_COLS * GRID_ROWS, cap)) return rc;
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    if (int rc = ensure_reloc_ws(m)) return rc;
+    RelocSet R; memset(&R, 0, sizeof(R));
+    R.pair = reinterpret_cast<const int2*>(d_pair); R.npairs = npairs; R.nrows = nrows; R.cap = cap;
+    R.kp = reinterpret_cast<const float*>(d_kps); R.desc = d_desc; R.n = d_n;
+    R.kfmp = d_kfmp; R.mpbad = d_mpbad; R.el = d_mp; R.eldesc = d_mpdesc; R.nel = nmp;
+    R.Tcw = d_Tcw; R.found = d_found; R.held = d_held;
+    R.assign = d_assign; R.nmatch = d_nmatch;
+    return reloc_run(m, A, R);
+}
+
+int sslpl_reloc_pairs_batch_device(sslpl_matcher* m, const int32_t* d_query, const int32_t* d_cand, const int32_t* d_ncand, int nq, int ndb,
+                                   int kmax, int32_t* d_pair) {
+    SSLPL_REQUIRE(m && d_query && d_cand && d_ncand && d_pair, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nq >= 1 && ndb >= 1 && kmax >= 1, SSLPL_ERR_ARG, "nq, ndb and kmax must be positive");
+    SSLPL_REQUIRE((long long)nq * kmax <= m->p.max_batch, SSLPL_ERR_ARG, "nq * kmax exceeds max_batch");
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    const int ns = nq * kmax;
+    launch(m, k_reloc_pairs, (ns + 127) / 128, 128, 0, nq, d_query, d_cand, d_ncand, ndb, kmax, reinterpret_cast<int2*>(d_pair));
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
 }
 
 }  // extern "C"

@@ -9,6 +9,7 @@
 #include "ORBmatcher.h"
 #include "LSDmatcher.h"
 #include "sslpl.h"
+#include <mutex>
 #include <set>
 #include <stdexcept>
 #include <string>
@@ -88,6 +89,60 @@ int ORBmatcher::SearchByProjection(Frame &CurrentFrame, const Frame &LastFrame, 
     {
         if(assign[j] >= 0) CurrentFrame.mvpMapPoints[j] = LastFrame.mvpMapPoints[assign[j]];
         else if(assign[j] == -2) CurrentFrame.mvpMapPoints[j] = static_cast<MapPoint*>(NULL);   // removed by the rotation check, ORBmatcher.cc:1461
+    }
+    return nmatches;
+}
+
+// MapPoint::PredictScale(dist, Frame*) reads mfMaxDistance under mMutexPos (MapPoint.cc:407-422); both are protected and have no accessor,
+// so they are reached through member pointers formed in a derived class (never instantiated).
+struct MapPointFields : MapPoint {
+    static float MapPoint::* MaxDistance() { return &MapPointFields::mfMaxDistance; }
+    static std::mutex MapPoint::* MutexPos() { return &MapPointFields::mMutexPos; }
+};
+
+// ORBmatcher::SearchByProjection(Frame &CurrentFrame, KeyFrame *pKF, sAlreadyFound, th, ORBdist) — ORBmatcher.cc:1475-1602, run by
+// Tracking::Relocalization (Tracking.cc:2071, :2085) after PnP and PoseOptimization.  Frame features the kernel never touched keep what
+// they held; features removed by the rotation check are set to NULL (:1595).
+int ORBmatcher::SearchByProjection(Frame &CurrentFrame, KeyFrame *pKF, const set<MapPoint*> &sAlreadyFound, const float th, const int ORBdist)
+{
+    const vector<MapPoint*> vpMPs = pKF->GetMapPointMatches();
+    const int n1 = (int)vpMPs.size(), n2 = CurrentFrame.N;
+    if(n1 == 0 || n2 == 0) return 0;
+    std::vector<uint8_t> flag1(n1, 0), dmp((size_t)n1*32, 0), held2(n2, 0), d2((size_t)n2*32);
+    std::vector<float> Xw((size_t)3*n1, 0.f), dist3((size_t)3*n1, 0.f), a1(n1), x2(n2), y2(n2), a2(n2);
+    std::vector<int32_t> o2(n2), assign(n2);
+    for(int i=0; i<n1; i++) {
+        a1[i] = pKF->mvKeysUn[i].angle;
+        MapPoint* p = vpMPs[i];
+        if(!p || p->isBad() || sAlreadyFound.count(p)) continue;
+        flag1[i] = 1;
+        const cv::Mat X = p->GetWorldPos();
+        for(int k=0; k<3; k++) Xw[3*i+k] = X.at<float>(k);
+        const cv::Mat d = p->GetDescriptor();
+        std::copy(d.ptr<uchar>(), d.ptr<uchar>() + 32, &dmp[(size_t)32*i]);
+        dist3[3*i] = p->GetMinDistanceInvariance(); dist3[3*i+1] = p->GetMaxDistanceInvariance();
+        unique_lock<mutex> lock(p->*MapPointFields::MutexPos());
+        dist3[3*i+2] = p->*MapPointFields::MaxDistance();
+    }
+    for(int j=0; j<n2; j++) {
+        const cv::KeyPoint &kp = CurrentFrame.mvKeysUn[j];
+        x2[j] = kp.pt.x; y2[j] = kp.pt.y; a2[j] = kp.angle; o2[j] = kp.octave;
+        held2[j] = CurrentFrame.mvpMapPoints[j] ? 1 : 0;
+        std::copy(CurrentFrame.mDescriptors.ptr<uchar>(j), CurrentFrame.mDescriptors.ptr<uchar>(j) + 32, &d2[(size_t)32*j]);
+    }
+    float Tcw[12];
+    for(int r=0; r<3; r++) for(int c=0; c<4; c++) Tcw[4*r+c] = CurrentFrame.mTcw.at<float>(r,c);
+    const float cam[4] = {CurrentFrame.fx, CurrentFrame.fy, CurrentFrame.cx, CurrentFrame.cy};
+    const float bounds[4] = {CurrentFrame.mnMinX, CurrentFrame.mnMaxX, CurrentFrame.mnMinY, CurrentFrame.mnMaxY};
+    int nmatches = 0;
+    Check(sslpl_search_by_projection_kf(Ctx(), n1, &flag1[0], &Xw[0], &dmp[0], &dist3[0], &a1[0], n2, &d2[0], &x2[0], &y2[0], &o2[0], &a2[0],
+                                        &held2[0], Tcw, cam, bounds, &CurrentFrame.mvScaleFactors[0], CurrentFrame.mnScaleLevels,
+                                        CurrentFrame.mfLogScaleFactor, th, ORBdist, mbCheckOrientation ? 1 : 0, &assign[0], &nmatches),
+          "sslpl_search_by_projection_kf");
+    for(int j=0; j<n2; j++)
+    {
+        if(assign[j] >= 0) CurrentFrame.mvpMapPoints[j] = vpMPs[assign[j]];
+        else if(assign[j] == -2) CurrentFrame.mvpMapPoints[j] = static_cast<MapPoint*>(NULL);
     }
     return nmatches;
 }
