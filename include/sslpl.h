@@ -393,6 +393,38 @@ int  sslpl_search_by_projection_kf_batch_device(sslpl_matcher* m,
         const float* cam, const float* bounds, const float* scaleFactors, int nlevels, float logScaleFactor,
         float th, int ORBdist, int checkOrientation, int32_t* d_assign, int32_t* d_nmatch);
 
+/* ---- Keyframe-to-frame matching over (keyframe row, frame row) pairs in HBM, asynchronous on the handle's stream.  Tracking runs it in
+   Relocalization (ORBmatcher(0.75, true).SearchByBoW(pKF, F) for every candidate: the pairs of sslpl_reloc_pairs_batch_device),
+   TrackReferenceKeyFrame (ORBmatcher(0.9, true).SearchByBoW(mpReferenceKF, F) and LSDmatcher::SearchByProjection(mpReferenceKF, F)) and
+   TrackWithMotionModel (the line matcher against the reference keyframe).
+   sslpl_search_by_bow_batch_device: ORBmatcher::SearchByBoW(KeyFrame* pKF, Frame& F, vector<MapPoint*>&) (ORBmatcher.cc:159-291) for
+   every pair d_pair[p] = (keyframe row, frame row).  The row set and element map are those of sslpl_search_by_projection_kf_batch_device:
+   d_kps[r][cap] = mvKeysUn, d_desc[r][cap][32], d_n[r] (clamped to [0, cap]), d_kfmp[r][cap] = GetMapPointMatches() as element indices
+   (-1 or any index outside [0, nmp) = NULL), d_mpbad[m] = isBad() (NULL = none bad).  A keyframe feature takes part iff its element is
+   non-NULL and not bad.  Both FeatureVectors come from the vocabulary at level L - levelsup (stopped words left out), built once per row
+   the pairs name.  d_match[p][cap]: the keyframe feature matched to frame feature j, or -1 (also where the rotation check dropped it, and
+   past the frame's count); d_nmatch[p] = the return value.  A pair with a row outside [0, nrows), such as the (-1, -1) slots of
+   sslpl_reloc_pairs_batch_device, gets d_nmatch -1 and an all -1 row.  Needs npairs <= max_batch, nrows <= 65535, cap <= max_features + 64
+   and (nc + 1 + cap) * 4 <= 200 KB for the level's nc nodes; the first call allocates a workspace of 2 max_batch FeatureVectors, freed
+   with the handle.  The caller keeps Relocalization's isBad() skip of a candidate and its nmatches < 15 discard. */
+int  sslpl_search_by_bow_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nrows, int cap,
+        const int32_t* d_kfmp, const uint8_t* d_mpbad, int nmp,
+        const sslpl_vocab* v, int levelsup,
+        int npairs, const int32_t* d_pair, float nnratio, int checkOrientation,
+        int32_t* d_match, int32_t* d_nmatch);
+/* sslpl_match_lines_kf_batch_device: LSDmatcher::SearchByProjection(KeyFrame* pKF, Frame& F, vector<MapLine*>&) (LSDmatcher.cpp:143-183)
+   for every pair d_pair[p] = (keyframe row, frame row) of a line row set in the layout of sslpl_line_device_results: d_ldesc[r][capl][32],
+   d_nl[r] (clamped to [0, capl]), d_kfml[r][capl] = GetMapLineMatches() as element indices (-1 or any index outside [0, nml) = NULL; the
+   reference tests no isBad() here).  d_lmatch[p][capl][tdx] = the qdx whose MapLine ends in vpMapLineMatches[tdx] (the last accepted),
+   or -1; d_nlmatch[p] = the return value, which counts overwritten acceptances.  d_nlmatch[p] = -1 for a row outside [0, nrows), and
+   where the keyframe has lines and the frame fewer than 2 (knnMatch leaves lmatches[i][1] undefined there).  Needs npairs <= max_batch,
+   nrows <= 65535 and capl <= max_lines + 64. */
+int  sslpl_match_lines_kf_batch_device(sslpl_matcher* m,
+        const uint8_t* d_ldesc, const int* d_nl, int nrows, int capl,
+        const int32_t* d_kfml, int nml,
+        int npairs, const int32_t* d_pair, int32_t* d_lmatch, int32_t* d_nlmatch);
+
 /* Batched line matching in HBM: knn2 + ratio rule of LSDmatcher::SearchByProjection(KF,F) (:143-183) with all
    KF lines valid: d_lmatch[p*capl + tdx] = qdx or -1; d_nlmatch[p]. */
 int  sslpl_match_lines_batch_device(sslpl_matcher* m, const uint8_t* d_ldesc, const int* d_nl, int nframes, int capl,

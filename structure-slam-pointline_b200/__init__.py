@@ -621,6 +621,24 @@ class Matcher(_Handle, kind="matcher", lifecycle=("sync", "set_stream", "stream"
             d_held or None, _p(_f32(cam)[:4].copy()), _p(_f32(bounds)), _p(sf), len(sf), log_scale_factor, th, orb_dist, int(check_ori),
             d_assign, d_nmatch))
 
+    def search_by_bow_batch_device(self, d_kps, d_desc, d_n, nrows, cap, d_kfmp, d_mpbad, nmp, vocab, levelsup, npairs, d_pair, nnratio,
+                                   check_ori, d_match, d_nmatch):
+        """ORBmatcher::SearchByBoW(KeyFrame*, Frame&) (ORBmatcher.cc:159-291) over (keyframe row, frame row) pairs of a row set in HBM
+        (see sslpl_search_by_bow_batch_device): the rows and d_kfmp [nrows, cap] i32 / d_mpbad [nmp] u8 or 0 as
+        search_by_projection_kf_batch_device, d_pair [npairs, 2] i32 -> d_match [npairs, cap] i32 (keyframe feature of frame feature j,
+        -1 none), d_nmatch [npairs] i32 (-1 for a pair outside the rows).  Asynchronous on the matcher's stream."""
+        _check(lib().sslpl_search_by_bow_batch_device(self._h, d_kps, d_desc, d_n, nrows, cap, d_kfmp, d_mpbad or None, nmp, vocab._h,
+                                                      levelsup, npairs, d_pair, nnratio, int(check_ori), d_match, d_nmatch))
+
+    def match_lines_kf_batch_device(self, d_ldesc, d_nl, nrows, capl, d_kfml, nml, npairs, d_pair, d_lmatch, d_nlmatch):
+        """LSDmatcher::SearchByProjection(KeyFrame*, Frame&) (LSDmatcher.cpp:143-183) over (keyframe row, frame row) pairs of a line row
+        set in HBM (see sslpl_match_lines_kf_batch_device): d_ldesc [nrows, capl, 32], d_nl [nrows], d_kfml [nrows, capl] i32 element
+        indices (-1 NULL), d_pair [npairs, 2] -> d_lmatch [npairs, capl] i32 (the last accepted qdx per tdx, -1 none), d_nlmatch
+        [npairs] i32 (-1: a row outside the set, or a keyframe with lines against a frame with fewer than 2).  Asynchronous on the
+        matcher's stream."""
+        _check(lib().sslpl_match_lines_kf_batch_device(self._h, d_ldesc, d_nl, nrows, capl, d_kfml, nml, npairs, d_pair, d_lmatch,
+                                                       d_nlmatch))
+
     def debug_predict_scale(self, ratio, log_scale_factor, nlevels, clamp=True):
         """MapPoint / MapLine::PredictScale on the device for host ratios (see sslpl_matcher_debug_predict_scale) -> int32 levels."""
         r = _f32(ratio).reshape(-1)

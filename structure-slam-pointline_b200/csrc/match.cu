@@ -148,18 +148,20 @@ __global__ void __launch_bounds__(128) k_bow_assign(const uint8_t* desc, long lo
 //   word  = word id of the leaf,  node = NodeId at level L - levelsup (0 if the leaf comes earlier),
 //   rank  = dense index of `node` among the possible values (0 = root / early leaf, 1 + rank inside the level), or -1 for a
 //           stopped word (weight <= 0), which the reference keeps out of the FeatureVector (:1162-1166).
+// kMap: output row f reads its descriptors from row row_of[f] of desc (n_arr stays indexed by f); kMap = false compiles that out.
 // -------------------------------------------------------------------------------------------------
 struct VocabView { const int* child_off; const int* child_ids; const uint8_t* desc; const double* weight; const int* word_id; const int* level_rank; };
 
+template <bool kMap>
 __global__ void __launch_bounds__(128) k_vocab_transform(const uint8_t* desc, long long desc_fs, const int* n_arr, int n_const, int cap,
                                                           VocabView V, int nid_level, int32_t* word, int32_t* node, int32_t* rank,
-                                                          double* weight, long long out_fs) {
+                                                          double* weight, long long out_fs, const int32_t* row_of) {
     const int f = blockIdx.y;
     const int n = n_arr ? min(n_arr[f], cap) : n_const;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     uint4 a0, a1;
-    load_desc(desc + f * desc_fs + (long long)i * 32, a0, a1);
+    load_desc(desc + (kMap ? row_of[f] : f) * desc_fs + (long long)i * 32, a0, a1);
     int cur = 0, nid = 0, level = 0;
     int cb = __ldg(V.child_off), ce = __ldg(V.child_off + 1);
     while (ce > cb) {
@@ -244,27 +246,41 @@ __device__ __forceinline__ int find_node(const int* nodes, int nn, int id) {   /
     return (lo < nn && nodes[lo] == id) ? lo : -1;
 }
 
+// kMap (mode 0 only): pair p is the rows (S.pmap[p].x, S.pmap[p].y) of [0, S.nframes) for descriptors and angles, and the FeatureVector
+// slots pslot[p] for the CSR; the keyframe row's MapPoints are kfmp[row][cap] element indices (outside [0, nmp): NULL) with isBad() flags
+// mpbad[nmp] (NULL: none bad), which replace S.flag.  kMap = false compiles all of it out.
+template <bool kMap>
 __global__ void __launch_bounds__(128) k_bow_match(FrameSet S, int mode, float nnratio, int cap,
                                                     int32_t* out, long long out_fs, uint8_t* rot, long long rot_fs,
-                                                    uint8_t* taken, long long taken_fs) {
+                                                    uint8_t* taken, long long taken_fs,
+                                                    const int2* pslot, const int32_t* kfmp, const uint8_t* mpbad, int nmp) {
     const int pair = blockIdx.y, lane = threadIdx.x & 31, a = blockIdx.x * 4 + (threadIdx.x >> 5);
-    const int f1 = pair, f2 = pair + 1;
-    const int nn1 = S.nn ? S.nn[f1] : S.nn_const, nn2 = S.nn ? S.nn[f2] : S.nn_const;
+    int f1 = pair, f2 = pair + 1, s1 = f1, s2 = f2;                          // rows (descriptors, angles) and FeatureVector slots
+    if (kMap) {
+        if (!pair_frames(S.pmap, S.nframes, pair, f1, f2)) return;
+        const int2 s = pslot[pair];
+        s1 = s.x; s2 = s.y;
+    }
+    const int nn1 = S.nn ? S.nn[s1] : S.nn_const, nn2 = S.nn ? S.nn[s2] : S.nn_const;
     if (a >= nn1) return;
-    const int* nodes1 = S.nodes + f1 * S.nodes_fs; const int* nodes2 = S.nodes + f2 * S.nodes_fs;
+    const int* nodes1 = S.nodes + s1 * S.nodes_fs; const int* nodes2 = S.nodes + s2 * S.nodes_fs;
     const int b = find_node(nodes2, nn2, nodes1[a]);
     if (b < 0) return;
-    const int* off1 = S.off + f1 * S.off_fs; const int* off2 = S.off + f2 * S.off_fs;
-    const int* idx1 = S.idx + f1 * S.idx_fs; const int* idx2 = S.idx + f2 * S.idx_fs;
+    const int* off1 = S.off + s1 * S.off_fs; const int* off2 = S.off + s2 * S.off_fs;
+    const int* idx1 = S.idx + s1 * S.idx_fs; const int* idx2 = S.idx + s2 * S.idx_fs;
     const uint8_t* D1 = S.desc + f1 * S.desc_fs; const uint8_t* D2 = S.desc + f2 * S.desc_fs;
     const uint8_t* v1 = S.flag ? S.flag + f1 * S.flag_fs : nullptr;
     const uint8_t* v2 = S.flag ? S.flag + f2 * S.flag_fs : nullptr;
+    const int32_t* mp1 = kMap ? kfmp + (long long)f1 * cap : nullptr;
     const float* A1 = S.angle + f1 * S.angle_fs; const float* A2 = S.angle + f2 * S.angle_fs;
     int32_t* O = out + pair * out_fs; uint8_t* R = rot + pair * rot_fs; uint8_t* TK = taken + pair * taken_fs;
     const int b1 = off1[a], e1 = off1[a + 1], b2 = off2[b], e2 = off2[b + 1];
     for (int i1 = b1; i1 < e1; i1++) {
         const int id1 = idx1[i1];
-        if (v1 && !v1[id1]) continue;                                            // :196-200 / :563-567
+        if (kMap) {                                                              // :196-200
+            const int e = mp1[id1];
+            if ((unsigned)e >= (unsigned)nmp || (mpbad && mpbad[e])) continue;
+        } else if (v1 && !v1[id1]) continue;                                     // :196-200 / :563-567
         uint4 a0, a1;
         load_desc(D1 + (long long)id1 * 32, a0, a1);
         // per-lane best / second best over this lane's candidates, in list order: key = dist << 20 | position
@@ -1058,17 +1074,31 @@ __global__ void k_fill_i32(int32_t* p, long long n, int v) {
 
 // LSDmatcher::SearchByProjection(KF,F) ratio rule on a knn2 table (LSDmatcher.cpp:161-180): out[tdx] = qdx, the
 // LAST accepted query wins (atomicMax over ascending qdx), nmatch counts every acceptance like the reference.
+// kMap: pair p is the rows (pmap[p].x, pmap[p].y) of [0, nrows) (keyframe, frame), the keyframe's MapLines are kfml[row][cap] element
+// indices (outside [0, nml): NULL) and n_arr is indexed by row; the pair's count (zeroed by the caller) becomes -1 when a row is outside
+// the set or when the keyframe has lines and the frame fewer than 2.  kMap = false compiles all of it out.
+template <bool kMap>
 __global__ void __launch_bounds__(128) k_line_ratio(const int32_t* knn, long long knn_fs, const int* n_arr, int n_const, int cap,
                                                      const uint8_t* has_ml1, long long ml_fs,
-                                                     int32_t* out, long long out_fs, int32_t* nmatch) {
+                                                     int32_t* out, long long out_fs, int32_t* nmatch,
+                                                     const int2* pmap, int nrows, const int32_t* kfml, int nml) {
     const int pair = blockIdx.y, q = blockIdx.x * blockDim.x + threadIdx.x;
-    const int nq = n_arr ? min(n_arr[pair], cap) : n_const;
+    int nq, fk = pair, ff;
+    if (kMap) {
+        const bool ok = pair_frames(pmap, nrows, pair, fk, ff);
+        nq = ok ? max(0, min(n_arr[fk], cap)) : 0;
+        if (!ok || (nq > 0 && min(n_arr[ff], cap) < 2)) {                       // knnMatch would leave lmatches[i][1] undefined (:167)
+            if (q == 0) nmatch[pair] = -1;
+            return;
+        }
+    } else nq = n_arr ? min(n_arr[pair], cap) : n_const;
     if (q >= nq) return;
     const int4 r = reinterpret_cast<const int4*>(knn + pair * knn_fs)[q];
     if (r.x < 0 || r.z < 0) return;
     const float ratio = __fdiv_rn((float)r.y, (float)r.w);                         // :167
     if ((double)ratio < (double)(1.0f / 1.5f)) {                                    // :169
-        if (has_ml1 && !has_ml1[pair * ml_fs + q]) return;
+        if (kMap) { if ((unsigned)kfml[(long long)fk * cap + q] >= (unsigned)nml) return; }   // :173-174
+        else if (has_ml1 && !has_ml1[pair * ml_fs + q]) return;
         atomicMax(&out[pair * out_fs + r.x], q);
         atomicAdd(&nmatch[pair], 1);
     }
@@ -1079,6 +1109,31 @@ __global__ void k_bad_pairs(const int2* pmap, int npairs, int nframes, int32_t* 
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     int f1, f2;
     if (p < npairs && !pair_frames(pmap, nframes, p, f1, f2)) nmatch[p] = -1;
+}
+
+// SearchByBoW(KeyFrame, Frame) over (keyframe row, frame row) pairs builds the FeatureVector of each row the pairs name once, in a slot:
+// side k of pair p (0 keyframe, 1 frame) is slot 2p + k, and a row's FeatureVector lives in the smallest slot that names it.
+// k_kfbow_claim leaves that slot in slot_of_row[row] (filled with INT_MAX before); k_kfbow_slots then gives each slot its row (-1 for a
+// slot whose row an earlier slot holds) and clamped count (0 there), and each pair its two slots and its frame's clamped count.
+__global__ void k_kfbow_claim(const int2* pmap, int npairs, int nrows, int32_t* slot_of_row) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x, p = t >> 1;
+    int kr, fr;
+    if (p >= npairs || !pair_frames(pmap, nrows, p, kr, fr)) return;
+    atomicMin(slot_of_row + ((t & 1) ? fr : kr), t);
+}
+__global__ void k_kfbow_slots(const int2* pmap, int npairs, int nrows, const int* n, int cap, const int32_t* slot_of_row,
+                              int32_t* slot_row, int* slot_n, int2* pslot, int* frame_n) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x, p = t >> 1;
+    if (p >= npairs) return;
+    int kr, fr;
+    const bool ok = pair_frames(pmap, nrows, p, kr, fr);
+    const int r = (t & 1) ? fr : kr;
+    const bool own = ok && slot_of_row[r] == t;
+    slot_row[t] = own ? r : -1;
+    slot_n[t] = own ? min(max(n[r], 0), cap) : 0;
+    if (t & 1) return;
+    pslot[p] = ok ? make_int2(slot_of_row[kr], slot_of_row[fr]) : make_int2(0, 0);
+    frame_n[p] = ok ? min(max(n[fr], 0), cap) : 0;
 }
 
 // LSDmatcher::SearchForTriangulation (LSDmatcher.cpp:382-415), one CTA per keyframe pair, on the knn2 table of (KF1 lines, KF2 lines):
@@ -2130,6 +2185,11 @@ struct sslpl_matcher : sslpl::StreamHandle {
     int32_t* rw_sel = nullptr; uint8_t* rw_claimed = nullptr; uint8_t* rw_rbin = nullptr;
     float* rw_el = nullptr; uint8_t* rw_eldesc = nullptr; int32_t* rw_kfmp = nullptr; int32_t* rw_pair = nullptr; float* rw_T = nullptr;
     int32_t* rw_nmatch = nullptr;
+    // workspace of sslpl_search_by_bow_batch_device, allocated by its first call: per slot ([2 max_batch]) its row, count, node indices
+    // and FeatureVector CSR; per pair its two slots and its frame's count
+    uint8_t* kb = nullptr;
+    int32_t* kb_row = nullptr; int* kb_n = nullptr; int32_t* kb_node = nullptr; int* kb_off = nullptr; int* kb_idx = nullptr;
+    int2* kb_pslot = nullptr; int* kb_fn = nullptr;
 };
 
 namespace {
@@ -2274,6 +2334,21 @@ int ensure_reloc_ws(sslpl_matcher* m) {
     return SSLPL_OK;
 }
 
+int ensure_kfbow_ws(sslpl_matcher* m) {
+    const int S = 2 * m->p.max_batch, B = m->p.max_batch, fc = m->p.max_features + 64, NN = m->p.max_nodes + 1;
+    Arena A;
+    for (int k = 0; k < 2; k++) {
+        m->kb_row = A.take<int32_t>(S); m->kb_n = A.take<int>(S);
+        m->kb_node = A.take<int32_t>((size_t)S * fc); m->kb_off = A.take<int>((size_t)S * (NN + 1)); m->kb_idx = A.take<int>((size_t)S * fc);
+        m->kb_pslot = A.take<int2>(B); m->kb_fn = A.take<int>(B);
+        if (k == 0) {
+            if (int rc = first_use(m->kb, A.used)) return rc;
+            A.base = m->kb; A.size = A.used; A.used = 0;
+        }
+    }
+    return SSLPL_OK;
+}
+
 // the sizes of a batched call over a keyframe set: nkf keyframes of cap rows (cap <= rows + 64: max_features or max_lines)
 int kf_set_ok(const sslpl_matcher* m, int nkf, int cap, int rows) {
     SSLPL_REQUIRE(nkf >= 1 && nkf <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nkf outside [1, max_batch + 1]");
@@ -2322,7 +2397,8 @@ int common_bow(sslpl_matcher* m, int mode, const uint8_t* d1, int n1, const uint
     SSLPL_CUDA(cudaMemsetAsync(m->rot, 255, nout, st));
     SSLPL_CUDA(cudaMemsetAsync(m->taken, 0, std::max(n2, 1), st));
     if (fv1->nn > 0 && fv2->nn > 0)
-        launch(m, k_bow_match, dim3((fv1->nn + 3) / 4, 1), 128, 0, staging_set(m), mode, nnratio, cap, m->out, 0, m->rot, 0, m->taken, 0);
+        launch(m, k_bow_match<false>, dim3((fv1->nn + 3) / 4, 1), 128, 0, staging_set(m), mode, nnratio, cap, m->out, 0, m->rot, 0, m->taken, 0,
+               nullptr, nullptr, nullptr, 0);
     launch(m, k_rot_filter, 1, 256, 0, m->out, 0, m->rot, 0, nullptr, 0, nout, cap, checkOri, m->nmatch, nullptr, 0);
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(match, m->out, sizeof(int32_t) * nout, cudaMemcpyDeviceToHost, st));
@@ -2414,6 +2490,7 @@ void sslpl_matcher_destroy(sslpl_matcher* m) {
     if (m->tw) cudaFree(m->tw);
     if (m->ltw) cudaFree(m->ltw);
     if (m->rw) cudaFree(m->rw);
+    if (m->kb) cudaFree(m->kb);
     delete m;
 }
 
@@ -2564,8 +2641,8 @@ static int bow_batch_tail(sslpl_matcher* m, const uint8_t* d_desc, const sslpl_k
     fill(m, d_match, (long long)npairs * cap, -1);
     SSLPL_CUDA(cudaMemsetAsync(m->b_rot, 255, (size_t)npairs * fc, st));
     SSLPL_CUDA(cudaMemsetAsync(m->b_taken, 0, (size_t)npairs * fc, st));
-    launch(m, k_bow_match, dim3((nc + 3) / 4, npairs), 128, 0, dense_set(m, d_desc, d_kps, cap, nc, nullptr), 0, nnratio, cap, d_match, cap,
-           m->b_rot, fc, m->b_taken, fc);
+    launch(m, k_bow_match<false>, dim3((nc + 3) / 4, npairs), 128, 0, dense_set(m, d_desc, d_kps, cap, nc, nullptr), 0, nnratio, cap, d_match, cap,
+           m->b_rot, fc, m->b_taken, fc, nullptr, nullptr, nullptr, 0);
     launch(m, k_rot_filter, npairs, 256, 0, d_match, cap, m->b_rot, fc, d_n, 1, 0, cap, checkOri, d_nmatch, nullptr, 0);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
@@ -3057,8 +3134,8 @@ int sslpl_bow_transform(sslpl_matcher* m, const sslpl_vocab* v, const uint8_t* d
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
     SSLPL_CUDA(cudaMemcpyAsync(m->desc, desc, (size_t)n * 32, cudaMemcpyHostToDevice, st));
-    launch(m, k_vocab_transform, dim3((n + 127) / 128, 1), 128, 0, m->desc, 0, nullptr, n, n, v->view, v->L - levelsup, m->word, m->node, nullptr,
-           m->wgt, 0);
+    launch(m, k_vocab_transform<false>, dim3((n + 127) / 128, 1), 128, 0, m->desc, 0, nullptr, n, n, v->view, v->L - levelsup, m->word, m->node,
+           nullptr, m->wgt, 0, nullptr);
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(word, m->word, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaMemcpyAsync(node, m->node, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
@@ -3081,8 +3158,10 @@ int sslpl_match_bow_batch_device_vocab(sslpl_matcher* m, const uint8_t* d_desc, 
     const dim3 grid((cap + 127) / 128, nframes);
     // optional per-feature outputs use the caller's [nframes][cap] layout; the dense node index goes to the workspace ([..][fc])
     if (d_word || d_node || d_weight)
-        launch(m, k_vocab_transform, grid, 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup, d_word, d_node, nullptr, d_weight, cap);
-    launch(m, k_vocab_transform, grid, 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup, nullptr, nullptr, m->b_node, nullptr, fc);
+        launch(m, k_vocab_transform<false>, grid, 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup, d_word, d_node, nullptr,
+               d_weight, cap, nullptr);
+    launch(m, k_vocab_transform<false>, grid, 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup, nullptr, nullptr, m->b_node,
+           nullptr, fc, nullptr);
     return bow_batch_tail(m, d_desc, d_kps, d_n, nframes, cap, nc, nnratio, checkOri, d_match, d_nmatch);
 }
 
@@ -3111,8 +3190,8 @@ int sslpl_bow_vectors_batch_device(sslpl_matcher* m, const sslpl_vocab* v, const
     SSLPL_REQUIRE(v->device == m->p.device, SSLPL_ERR_ARG, "vocabulary and matcher live on different devices");
     SSLPL_REQUIRE(v->scoring == 0 && v->weighting == 0, SSLPL_ERR_UNSUPPORTED, "BowVectors are built for TF_IDF weighting and L1 scoring only");
     SSLPL_CUDA(cudaSetDevice(m->p.device));
-    launch(m, k_vocab_transform, dim3((cap + 127) / 128, nrows), 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, 0,
-           d_bow_word, nullptr, nullptr, d_bow_val, cap);
+    launch(m, k_vocab_transform<false>, dim3((cap + 127) / 128, nrows), 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, 0,
+           d_bow_word, nullptr, nullptr, d_bow_val, cap, nullptr);
     const int P = bow_pow2(cap);
     launch(m, k_bow_vector, nrows, 512, (size_t)(P + cap) * 8, BowRows{d_bow_word, d_bow_val, d_bow_n, cap}, d_n, P);
     SSLPL_CUDA(cudaGetLastError());
@@ -3195,7 +3274,8 @@ int sslpl_match_lines_batch_device(sslpl_matcher* m, const uint8_t* d_ldesc, con
            d_nl, 0, m->b_knn, (long long)lc * 4, capl, nullptr, 0);
     fill(m, d_lmatch, (long long)npairs * capl, -1);
     SSLPL_CUDA(cudaMemsetAsync(d_nlmatch, 0, sizeof(int32_t) * npairs, st));
-    launch(m, k_line_ratio, dim3((capl + 127) / 128, npairs), 128, 0, m->b_knn, (long long)lc * 4, d_nl, 0, capl, nullptr, 0, d_lmatch, capl, d_nlmatch);
+    launch(m, k_line_ratio<false>, dim3((capl + 127) / 128, npairs), 128, 0, m->b_knn, (long long)lc * 4, d_nl, 0, capl, nullptr, 0, d_lmatch, capl,
+           d_nlmatch, nullptr, 0, nullptr, 0);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
@@ -3217,8 +3297,8 @@ static int tri_match_stage(sslpl_matcher* m,
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     const int fc = m->p.max_features + 64, NN = m->p.max_nodes + 1;
     if (int rc = first_use(m->tw, sizeof(int32_t) * (size_t)m->p.max_batch * fc)) return rc;
-    launch(m, k_vocab_transform, dim3((cap + 127) / 128, nkf), 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup,
-           nullptr, nullptr, m->b_node, nullptr, fc);
+    launch(m, k_vocab_transform<false>, dim3((cap + 127) / 128, nkf), 128, 0, d_desc, (long long)cap * 32, d_n, 0, cap, v->view, v->L - levelsup,
+           nullptr, nullptr, m->b_node, nullptr, fc, nullptr);
     launch(m, k_build_csr, nkf, 128, (nc + 1 + cap) * sizeof(int), m->b_node, fc, d_n, cap, nc, m->b_off, NN + 1, m->b_idx, fc);
     fill(m, m->tw, (long long)npairs * cap, -1);
     FrameSet S = dense_set(m, d_desc, d_kps, cap, nc, d_has_mp);
@@ -3624,6 +3704,77 @@ int sslpl_reloc_pairs_batch_device(sslpl_matcher* m, const int32_t* d_query, con
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     const int ns = nq * kmax;
     launch(m, k_reloc_pairs, (ns + 127) / 128, 128, 0, nq, d_query, d_cand, d_ncand, ndb, kmax, reinterpret_cast<int2*>(d_pair));
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+// ORBmatcher::SearchByBoW(KeyFrame*, Frame&) over (keyframe row, frame row) pairs: the row -> slot map (k_kfbow_claim / k_kfbow_slots),
+// the FeatureVector of every named row once (k_vocab_transform<true>, k_build_csr), k_bow_match<true>, the rotation filter and count,
+// then -1 for the pairs outside the rows.
+int sslpl_search_by_bow_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nrows, int cap,
+        const int32_t* d_kfmp, const uint8_t* d_mpbad, int nmp,
+        const sslpl_vocab* v, int levelsup,
+        int npairs, const int32_t* d_pair, float nnratio, int checkOrientation,
+        int32_t* d_match, int32_t* d_nmatch) {
+    SSLPL_REQUIRE(m && d_kps && d_desc && d_n && d_kfmp && v && d_pair && d_match && d_nmatch, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nmp >= 0, SSLPL_ERR_ARG, "nmp must be >= 0");
+    SSLPL_REQUIRE(nrows >= 1 && nrows <= 65535, SSLPL_ERR_ARG, "nrows outside [1, 65535]");
+    SSLPL_REQUIRE(cap >= 1 && cap <= m->p.max_features + 64, SSLPL_ERR_ARG, "cap outside [1, max_features + 64]");
+    SSLPL_REQUIRE(npairs >= 1 && npairs <= m->p.max_batch, SSLPL_ERR_ARG, "npairs outside [1, max_batch]");
+    SSLPL_REQUIRE(npairs <= 32767, SSLPL_ERR_ARG, "npairs exceeds 32767 (two FeatureVector slots per pair on one grid axis)");
+    const int nc = vocab_level_nodes(v, levelsup);
+    SSLPL_REQUIRE(nc <= m->p.max_nodes, SSLPL_ERR_ARG, "the vocabulary level exceeds the matcher capacity (max_nodes)");
+    SSLPL_REQUIRE(v->device == m->p.device, SSLPL_ERR_ARG, "vocabulary and matcher live on different devices");
+    if (int rc = csr_fits(nc, cap)) return rc;
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    if (int rc = ensure_kfbow_ws(m)) return rc;
+    if (int rc = ensure_scratch(m, (size_t)nrows * 4)) return rc;
+    cudaStream_t st = m->stream;
+    const int fc = m->p.max_features + 64, NN = m->p.max_nodes + 1, ns = 2 * npairs;
+    const int2* pmap = reinterpret_cast<const int2*>(d_pair);
+    int32_t* slot_of_row = reinterpret_cast<int32_t*>(m->scratch);
+    fill(m, slot_of_row, nrows, INT_MAX);
+    launch(m, k_kfbow_claim, (ns + 127) / 128, 128, 0, pmap, npairs, nrows, slot_of_row);
+    launch(m, k_kfbow_slots, (ns + 127) / 128, 128, 0, pmap, npairs, nrows, d_n, cap, (const int32_t*)slot_of_row, m->kb_row, m->kb_n,
+           m->kb_pslot, m->kb_fn);
+    launch(m, k_vocab_transform<true>, dim3((cap + 127) / 128, ns), 128, 0, d_desc, (long long)cap * 32, (const int*)m->kb_n, 0, cap, v->view,
+           v->L - levelsup, nullptr, nullptr, m->kb_node, nullptr, fc, (const int32_t*)m->kb_row);
+    launch(m, k_build_csr, ns, 128, (nc + 1 + cap) * sizeof(int), m->kb_node, fc, m->kb_n, cap, nc, m->kb_off, NN + 1, m->kb_idx, fc);
+    fill(m, d_match, (long long)npairs * cap, -1);
+    SSLPL_CUDA(cudaMemsetAsync(m->b_taken, 0, (size_t)npairs * fc, st));
+    FrameSet S = dense_set(m, d_desc, d_kps, cap, nc, nullptr);
+    S.off = m->kb_off; S.idx = m->kb_idx; S.pmap = pmap; S.nframes = nrows;
+    // b_rot is only read where the table holds a match, and k_bow_match writes both together
+    launch(m, k_bow_match<true>, dim3((nc + 3) / 4, npairs), 128, 0, S, 0, nnratio, cap, d_match, cap, m->b_rot, fc, m->b_taken, fc,
+           (const int2*)m->kb_pslot, d_kfmp, d_mpbad, nmp);
+    launch(m, k_rot_filter, npairs, 256, 0, d_match, cap, m->b_rot, fc, (const int*)m->kb_fn, 0, 0, cap, checkOrientation ? 1 : 0, d_nmatch,
+           nullptr, 0);
+    launch(m, k_bad_pairs, (npairs + 127) / 128, 128, 0, pmap, npairs, nrows, d_nmatch);
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+// LSDmatcher::SearchByProjection(KeyFrame*, Frame&) over (keyframe row, frame row) pairs: k_knn2 over the pair map (query = the keyframe's
+// lines, train = the frame's), then the ratio rule with the keyframe's MapLines.
+int sslpl_match_lines_kf_batch_device(sslpl_matcher* m,
+        const uint8_t* d_ldesc, const int* d_nl, int nrows, int capl,
+        const int32_t* d_kfml, int nml,
+        int npairs, const int32_t* d_pair, int32_t* d_lmatch, int32_t* d_nlmatch) {
+    SSLPL_REQUIRE(m && d_ldesc && d_nl && d_kfml && d_pair && d_lmatch && d_nlmatch, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nml >= 0, SSLPL_ERR_ARG, "nml must be >= 0");
+    SSLPL_REQUIRE(nrows >= 1 && nrows <= 65535, SSLPL_ERR_ARG, "nrows outside [1, 65535]");
+    SSLPL_REQUIRE(capl >= 1 && capl <= m->p.max_lines + 64, SSLPL_ERR_ARG, "capl outside [1, max_lines + 64]");
+    SSLPL_REQUIRE(npairs >= 1 && npairs <= m->p.max_batch, SSLPL_ERR_ARG, "npairs outside [1, max_batch]");
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    const int lc = m->p.max_lines + 64;
+    const int2* pmap = reinterpret_cast<const int2*>(d_pair);
+    launch(m, k_knn2<true>, dim3((capl + 7) / 8, npairs), 256, 0, d_ldesc, (long long)capl * 32, d_nl, 0, d_ldesc, (long long)capl * 32, d_nl, 0,
+           m->b_knn, (long long)lc * 4, capl, pmap, nrows);
+    fill(m, d_lmatch, (long long)npairs * capl, -1);
+    SSLPL_CUDA(cudaMemsetAsync(d_nlmatch, 0, sizeof(int32_t) * npairs, m->stream));
+    launch(m, k_line_ratio<true>, dim3((capl + 127) / 128, npairs), 128, 0, m->b_knn, (long long)lc * 4, d_nl, 0, capl, nullptr, 0, d_lmatch,
+           capl, d_nlmatch, pmap, nrows, d_kfml, nml);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
