@@ -82,7 +82,11 @@ int  sslpl_orb_tables(const sslpl_orb* h, float* scale, float* invscale, float* 
 /* the same tables without a device or a handle (host arithmetic only: the adapter's constructor runs before any frame is seen) */
 int  sslpl_orb_tables_host(int nfeatures, float scaleFactor, int nlevels, float* scale, float* invscale, float* sigma2, float* invsigma2,
                            int* nfeat_per_level, int* umax16);
-int  sslpl_orb_max_keypoints(const sslpl_orb* h);  /* capacity per frame: sum_l (mnFeaturesPerLevel[l] + 3) */
+/* Keypoint capacity per frame, a bound for every frame up to max_width: sum_l max(mnFeaturesPerLevel[l] + 16, 4 * nIni_l), with
+   nIni_l = round((w_l - 32) / 30) at level l's width w_l for max_width.  DistributeOctTree splits its nIni = round(dx / dy) root
+   nodes once before it looks at the level's budget, so a wide frame can keep up to 4 nIni keypoints on a level
+   (ORBextractor.cc:542-669); otherwise a level keeps at most mnFeaturesPerLevel[l] + 2. */
+int  sslpl_orb_max_keypoints(const sslpl_orb* h);
 
 /* ORBextractor::operator() (ORBextractor.cc:1043) on one HOST frame (CV_8UC1, `pitch` bytes per row).
    kps[cap], desc[cap*32]; *n = number of keypoints (0 for an empty image, as the reference's silent return). */

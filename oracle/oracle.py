@@ -170,12 +170,16 @@ class OrbOracle:
         return dict(scale=sc, invscale=isc, sigma2=s2, invsigma2=is2, nfeat=nf, umax=um)
 
     def extract(self, img):
+        """(keypoints, descriptors) of every level.  The C side returns the full count; a level may keep more keypoints than its
+        share of nfeatures (up to 4 * nIni after the octree's first split), so a short buffer is sized again from that count."""
         img = _u8(img)
         cap = self.nfeatures + 4 * self.nlevels + 64
-        kps = np.zeros(cap, KEYPOINT_DTYPE); desc = np.zeros((cap, 32), np.uint8)
-        n = lib().orc_orb_extract(self.h, _p(img), img.shape[1], img.shape[0], img.strides[0], _p(kps), _p(desc), cap)
-        assert n <= cap
-        return kps[:n].copy(), desc[:n].copy()
+        while True:
+            kps = np.zeros(cap, KEYPOINT_DTYPE); desc = np.zeros((cap, 32), np.uint8)
+            n = lib().orc_orb_extract(self.h, _p(img), img.shape[1], img.shape[0], img.strides[0], _p(kps), _p(desc), cap)
+            if n <= cap:
+                return kps[:n].copy(), desc[:n].copy()
+            cap = n
 
     def level_size(self, l):
         w = C.c_int(); h = C.c_int()
@@ -196,13 +200,18 @@ class OrbOracle:
         return out
 
     def candidates(self, l, cap=1 << 16):
+        """FAST candidates of level l of the last call; the C side returns the full count, and a short buffer is sized again."""
         xs = np.empty(cap, np.int32); ys = np.empty(cap, np.int32); rs = np.empty(cap, np.int32)
         n = lib().orc_orb_candidates(self.h, l, _p(xs), _p(ys), _p(rs), cap)
+        if n > cap:
+            return self.candidates(l, n)
         return xs[:n].copy(), ys[:n].copy(), rs[:n].copy()
 
     def level_keypoints(self, l, cap=1 << 14):
         xs = np.empty(cap, np.int32); ys = np.empty(cap, np.int32); rs = np.empty(cap, np.int32); an = np.empty(cap, np.float32)
         n = lib().orc_orb_level_keypoints(self.h, l, _p(xs), _p(ys), _p(rs), _p(an), cap)
+        if n > cap:
+            return self.level_keypoints(l, n)
         return xs[:n].copy(), ys[:n].copy(), rs[:n].copy(), an[:n].copy()
 
     def stage_ms(self):

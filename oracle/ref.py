@@ -50,7 +50,8 @@ def orb_extract(img, nfeatures=1000, scale=1.2, nlevels=8, ini=20, mn=7, cap=Non
     kps = np.zeros(cap, KEYPOINT_DTYPE); desc = np.zeros((cap, 32), np.uint8); lc = np.zeros(nlevels, np.int32)
     n = lib().ref_orb_extract(nfeatures, C.c_float(scale), nlevels, ini, mn, _p(img), img.shape[1], img.shape[0], img.strides[0],
                               _p(kps), _p(desc), cap, _p(lc))
-    assert n <= cap
+    if n > cap:             # wide frames and small budgets keep more than 2 * nfeatures: run again with room for the full count
+        return orb_extract(img, nfeatures, scale, nlevels, ini, mn, n)
     return kps[:n].copy(), desc[:n].copy(), lc
 
 

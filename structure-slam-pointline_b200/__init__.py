@@ -296,12 +296,15 @@ class ORBextractor(_Handle, kind="orb", lifecycle=("sync", "set_stream", "stream
     def candidates(self, l, frame=0, cap=1 << 17):
         xs = np.empty(cap, np.int32); ys = np.empty(cap, np.int32); rs = np.empty(cap, np.int32); n = C.c_int()
         _check(lib().sslpl_orb_download_candidates(self._h, frame, l, _p(xs), _p(ys), _p(rs), cap, C.byref(n)))
-        assert n.value <= cap
+        if n.value > cap:                  # *n is the full count: a wide level of noise can hold more
+            return self.candidates(l, frame, n.value)
         return xs[:n.value].copy(), ys[:n.value].copy(), rs[:n.value].copy()
 
     def level_keypoints(self, l, frame=0, cap=1 << 15):
         xs = np.empty(cap, np.int32); ys = np.empty(cap, np.int32); rs = np.empty(cap, np.int32); n = C.c_int()
         _check(lib().sslpl_orb_download_level_keypoints(self._h, frame, l, _p(xs), _p(ys), _p(rs), cap, C.byref(n)))
+        if n.value > cap:
+            return self.level_keypoints(l, frame, n.value)
         return xs[:n.value].copy(), ys[:n.value].copy(), rs[:n.value].copy()
 
 

@@ -539,7 +539,7 @@ __global__ void __launch_bounds__(256) k_octree(const __grid_constant__ OrbGeom 
     __syncthreads();
     const int dx = L.maxBX - MINB, dy = L.maxBY - MINB;
     const int nIni = (int)roundf(__fdiv_rn((float)dx, (float)dy));                      // ORBextractor.cc:542
-    if (C == 0 || nIni <= 0 || nIni > o.pool_cap) { if (tid == 0) *lvl_cnt = 0; return; }
+    if (C == 0 || nIni <= 0 || nIni > o.pool_cap) { if (tid == 0) *lvl_cnt = 0; return; }   // pool_cap > 5 nIni (make_geometry): no pool drop
     const float hX = __fdiv_rn((float)dx, (float)nIni);                                  // :544
     for (int i = tid; i < nIni; i += T) {
         const int idx = nIni - 1 - i;
@@ -809,6 +809,7 @@ struct sslpl_orb : sslpl::StreamHandle {
     uint8_t* d_input = nullptr;         // staging for host frames
     int cur_w = 0, cur_h = 0, cur_frames = 0;
     int octree_smem = 0;
+    int kp_max = 0;                     // keypoints per frame: make_geometry's kp_total_cap, the same for every frame size
     TMaps tm;                           // per-level tensor maps (level 0 re-encoded per call: the input view moves)
     PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
     bool tma_levels_ok = false, use_tma = true;
@@ -841,7 +842,26 @@ void make_tables(sslpl_orb* h) {
     for (v = HALF_PATCH, v0 = 0; v >= vmin; --v) { while (h->umax[v0] == h->umax[v0 + 1]) ++v0; h->umax[v] = v0; ++v0; }
 }
 
+// Upper bound of DistributeOctTree's nIni = round(dx / dy) (ORBextractor.cc:542) on level l of any frame the handle accepts.  Only a
+// level with a 30-px cell has keypoints, and there dy >= 30, so nIni <= round(dx / 30); dx = w_l - 32 grows with the frame width, so
+// the level width at max_width bounds it.  (dx + 15) / 30 is that rounding: dx / 30 is never within a float ulp of k + 0.5 unless equal.
+int max_nini(const sslpl_orb* h, int l) {
+    const int dx = cvRoundF((float)h->p.max_width * h->invscale[l]) - 2 * MINB;
+    return dx >= 30 ? (dx + 15) / 30 : 0;
+}
+
 // Geometry for a frame size; with alloc==nullptr only sizes are computed.
+// The per-level keypoint and node-pool capacities depend on the handle's parameters and max_width only, never on W x H: so
+// sslpl_orb_max_keypoints() bounds every frame, and the pool and key arrays of any frame fit where orb_init sized them.
+//   keypoints  DistributeOctTree first splits each of its nIni roots once, whatever N: up to 4 nIni nodes.  A later pass runs only
+//              while the level holds < N nodes; a whole pass runs only if it cannot pass N (:673), and the careful pass stops at
+//              the first division that reaches N (:730), which adds <= 3.  So a level keeps <= max(N + 2, 4 nIni) keypoints.
+//   pool       k_octree never reuses a node: the pool holds the nIni roots, <= 4 nIni first-pass children, and the children of
+//              every later division.  A division of c children grows the list by c - 1, so a later pass creates E + G nodes
+//              for E divisions and a growth G.  Each divided node is in the list, which holds < N nodes: E <= N - 1.  The growth
+//              of all later passes sums to <= N + 2.  Every division halves a node's box, both sides < 4096 px and its keys on
+//              distinct pixels, so no node 13 halvings deep holds 2 keys: at most 12 passes after the first.
+//              Total <= 5 nIni + 12 (N - 1) + N + 2 < 5 nIni + 13 N + 64.
 void make_geometry(const sslpl_orb* h, int W, int H, OrbGeom& g, std::vector<int2>* rtab) {
     memset(&g, 0, sizeof(g));
     const int L = h->p.nlevels;
@@ -866,8 +886,9 @@ void make_geometry(const sslpl_orb* h, int W, int H, OrbGeom& g, std::vector<int
         G.cell_cap = ((G.wCell + 1) / 2) * ((G.hCell + 1) / 2);        // NMS survivors are pairwise non-adjacent
         G.cand_off = cand; cand += (long long)G.ncells * G.cell_cap;
         G.key_cap = G.ncells * G.cell_cap; G.key_off = key; key += align_up(G.key_cap, 64);
-        G.nfeat = h->nfeat[l]; G.kp_cap = G.nfeat + 16; G.kp_base = kpc; kpc += G.kp_cap;
-        G.pool_cap = 16 * (G.nfeat + 4) + 64; G.pool_off = pool; pool += align_up(G.pool_cap, 64);
+        const int nini = max_nini(h, l);
+        G.nfeat = h->nfeat[l]; G.kp_cap = std::max(G.nfeat + 16, 4 * nini); G.kp_base = kpc; kpc += G.kp_cap;
+        G.pool_cap = 5 * nini + 13 * G.nfeat + 64; G.pool_off = pool; pool += align_up(G.pool_cap, 64);
         maxN = std::max(maxN, G.nfeat);
         G.xtab_off = rt; rt += G.w; G.ytab_off = rt; rt += G.h;
         G.tiles_x = (G.w + BLUR_TW - 1) / BLUR_TW; G.tiles_y = (G.h + BLUR_TH - 1) / BLUR_TH;
@@ -1008,6 +1029,7 @@ int orb_init(sslpl_orb* h) {
     make_tables(h);
     OrbGeom g;
     make_geometry(h, p->max_width, p->max_height, g, nullptr);
+    h->kp_max = g.kp_total_cap;
     SSLPL_REQUIRE(g.sort_cap * 8 <= 200 * 1024, SSLPL_ERR_UNSUPPORTED, "nfeatures too large for the octree sort buffer");
     Arena A;                                   // dry run for the size
     carve(h, A, g, p->max_batch, p->max_width, p->max_height);
@@ -1071,8 +1093,7 @@ int sslpl_orb_tables_host(int nfeatures, float scaleFactor, int nlevels, float* 
 
 int sslpl_orb_max_keypoints(const sslpl_orb* h) {
     if (!h) return 0;
-    int s = 0; for (int l = 0; l < h->p.nlevels; l++) s += h->nfeat[l] + 16;
-    return s;
+    return h->kp_max;
 }
 
 int sslpl_orb_extract_batch_device(sslpl_orb* h, const uint8_t* d_imgs, int nframes, int width, int height, int pitch, size_t frame_stride) {
