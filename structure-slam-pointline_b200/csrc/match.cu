@@ -395,15 +395,28 @@ __global__ void __launch_bounds__(128) k_tri_match(FrameSet S, TriArgs T, const 
 constexpr int GRID_COLS = 64, GRID_ROWS = 48;        // Frame.h:45-46
 constexpr int TH_HIGH = 100;                         // ORBmatcher.cc:37
 
+// The image bounds (mnMinX, mnMaxX, mnMinY, mnMaxY), the inverse grid cell size and mvScaleFactors of a frame
+struct GridGeom { float minX, maxX, minY, maxY, invW, invH; float scale[32]; };
+
+// G from bounds = (minX, maxX, minY, maxY) and scaleFactors[nlevels] (NULL with nlevels = 0: no scale table; the caller bounds nlevels
+// by 32).  Degenerate bounds would give an infinite or negative cell size: SSLPL_ERR_ARG.
+static int grid_geom(GridGeom& G, const float* bounds, const float* scaleFactors, int nlevels) {
+    SSLPL_REQUIRE(bounds[1] > bounds[0] && bounds[3] > bounds[2], SSLPL_ERR_ARG, "degenerate image bounds");
+    G = GridGeom{};
+    G.minX = bounds[0]; G.maxX = bounds[1]; G.minY = bounds[2]; G.maxY = bounds[3];
+    G.invW = (float)GRID_COLS / (bounds[1] - bounds[0]); G.invH = (float)GRID_ROWS / (bounds[3] - bounds[2]);   // Frame.cc:115-116
+    for (int k = 0; k < nlevels; k++) G.scale[k] = scaleFactors[k];
+    return SSLPL_OK;
+}
+
 struct ProjArgs {
     float T[12];                                     // Tcw, 3x4 row-major (when ProjPair::Tcw is NULL)
     float fx, fy, cx, cy, mbf;
-    float minX, maxX, minY, maxY, invW, invH;
+    GridGeom G;
     float th;
     int forward, backward, checkOri, use_right;
     int nlevels;                                     // a last-frame point whose octave is outside [0, nlevels) is skipped
     int retry_below;                                 // a pair with fewer matches reruns with 2 * th (Tracking.cc:1240-1244); <= 0: never
-    float scale[32];                                 // mvScaleFactors
 };
 
 // Where the walker of pair p reads and writes: the last frame at the *1 pointers + p * (their frame stride), the current frame at
@@ -425,37 +438,101 @@ struct ProjPair {
 
 // Frame::AssignFeaturesToGrid's cell of every feature (PosInGrid, Frame.cc:462-472): frame f = blockIdx.y, fields at element stride es
 __global__ void __launch_bounds__(128) k_grid_cells(const float* x, const float* y, int es, long long fs, const int* n_arr, int n_const, int cap,
-                                                    float minX, float minY, float invW, float invH, int32_t* cell, long long cell_fs) {
+                                                    const __grid_constant__ GridGeom G, int32_t* cell, long long cell_fs) {
     const int f = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
     const int n = n_arr ? min(n_arr[f], cap) : n_const;
     if (i >= n) return;
     const long long e = f * fs + (long long)i * es;
-    const int px = (int)roundf(__fmul_rn(__fsub_rn(x[e], minX), invW)), py = (int)roundf(__fmul_rn(__fsub_rn(y[e], minY), invH));
+    const int px = (int)roundf(__fmul_rn(__fsub_rn(x[e], G.minX), G.invW)), py = (int)roundf(__fmul_rn(__fsub_rn(y[e], G.minY), G.invH));
     cell[f * cell_fs + i] = (px < 0 || px >= GRID_COLS || py < 0 || py >= GRID_ROWS) ? -1 : px * GRID_ROWS + py;
 }
 
-// the cell range of Frame::GetFeaturesInArea(x, y, r) (Frame.cc:375-393) on the grid of k_grid_cells; false when the window misses it
-__device__ __forceinline__ bool grid_window(float minX, float minY, float invW, float invH, float x, float y, float r,
-                                            int& cx0, int& cx1, int& cy0, int& cy1) {
-    cx0 = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(x, minX), r), invW)));
+// The cells of Frame::GetFeaturesInArea(x, y, r) (Frame.cc:375-393) on the grid of k_grid_cells, in its traversal order: cell rank
+// c = 0 .. ncell - 1 is cell (cx0 + c / ny, cy0 + c % ny).
+struct GridWin { int cx0, cy0, ny, ncell; };
+
+// false when the window misses the grid
+__device__ __forceinline__ bool grid_window(const GridGeom& G, float x, float y, float r, GridWin& w) {
+    const int cx0 = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(x, G.minX), r), G.invW)));
     if (cx0 >= GRID_COLS) return false;
-    cx1 = min(GRID_COLS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(x, minX), r), invW)));
+    const int cx1 = min(GRID_COLS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(x, G.minX), r), G.invW)));
     if (cx1 < 0) return false;
-    cy0 = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(y, minY), r), invH)));
+    const int cy0 = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(y, G.minY), r), G.invH)));
     if (cy0 >= GRID_ROWS) return false;
-    cy1 = min(GRID_ROWS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(y, minY), r), invH)));
-    return cy1 >= 0;
+    const int cy1 = min(GRID_ROWS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(y, G.minY), r), G.invH)));
+    if (cy1 < 0) return false;
+    w.cx0 = cx0; w.cy0 = cy0; w.ny = cy1 - cy0 + 1; w.ncell = (cx1 - cx0 + 1) * w.ny;
+    return true;
 }
-// the feature of a window key (dist << 40 | cell rank << 20 | position in the cell) over the window from (cx0, cy0), ny cells high
-__device__ __forceinline__ int grid_key_feature(const int* goff, const int* gidx, int cx0, int cy0, int ny, unsigned long long key) {
+
+// The candidates of window w, lane by lane: lane l walks the cells of rank l, l + 32, ... and passes each feature j of the grid CSR
+// to cand(j, dist), which applies the caller's filters and returns false to skip j, or sets dist to the descriptor distance and returns
+// true.  take() gets the key (dist << 40) | (cell rank << 20) | position in the cell: ascending keys are ascending distances in
+// GetFeaturesInArea's order, so the smallest key is the reference's first strict minimum and the two smallest are its best /
+// second-best pair.  (A bool rather than a sentinel distance: each filter then branches straight to the next feature; with a
+// sentinel, k_point_fuse_search<true> needs 3 more registers.)
+template <class Cand, class Take>
+__device__ __forceinline__ void grid_scan(const int* goff, const int* gidx, const GridWin& w, int lane, Cand cand, Take take) {
+    for (int c = lane; c < w.ncell; c += 32) {
+        const int cell = (w.cx0 + c / w.ny) * GRID_ROWS + w.cy0 + c % w.ny;
+        const int b = goff[cell], e = goff[cell + 1];
+        for (int q = b; q < e; q++) {
+            int d;
+            if (cand(gidx[q], d)) take(((unsigned long long)d << 40) | ((unsigned long long)c << 20) | (unsigned)(q - b));
+        }
+    }
+}
+// the smallest key of the window, in every lane (~0 when no candidate)
+template <class Cand>
+__device__ __forceinline__ unsigned long long grid_min(const int* goff, const int* gidx, const GridWin& w, int lane, Cand cand) {
+    unsigned long long best = ~0ull;
+    grid_scan(goff, gidx, w, lane, cand, [&](unsigned long long k) { if (k < best) best = k; });
+    return warp_min(best);
+}
+// the two smallest keys of the window, in every lane (~0 for a missing one)
+template <class Cand>
+__device__ __forceinline__ void grid_top2(const int* goff, const int* gidx, const GridWin& w, int lane, Cand cand,
+                                          unsigned long long& b1, unsigned long long& b2) {
+    b1 = ~0ull; b2 = ~0ull;
+    grid_scan(goff, gidx, w, lane, cand, [&](unsigned long long k) { top2_push(b1, b2, k); });
+    top2_warp(b1, b2);
+}
+// the feature of a window key
+__device__ __forceinline__ int grid_key_feature(const int* goff, const int* gidx, const GridWin& w, unsigned long long key) {
     const int c = (int)((key >> 20) & 0xfffff), pos = (int)(key & 0xfffff);
-    return gidx[goff[(cx0 + c / ny) * GRID_ROWS + cy0 + c % ny] + pos];
+    return gidx[goff[(w.cx0 + c / w.ny) * GRID_ROWS + w.cy0 + c % w.ny] + pos];
+}
+
+// The rotation check of the one-warp walkers (ComputeThreeMaxima, ORBmatcher.cc:1604-1645, over the histogram s_hist) on matches
+// [0, n): bin(i) is the rotation bin of match i, or -1 when i has none; drop(i) removes a match outside the three kept bins.  Returns
+// the number removed, in every lane.
+template <class Bin, class Drop>
+__device__ __forceinline__ int warp_rot_check(const int* s_hist, int n, int lane, Bin bin, Drop drop) {
+    __shared__ int s_keep[3];
+    if (lane == 0) { const int3 k = three_maxima(s_hist); s_keep[0] = k.x; s_keep[1] = k.y; s_keep[2] = k.z; }
+    __syncwarp();
+    const int k0 = s_keep[0], k1 = s_keep[1], k2 = s_keep[2];
+    int ndrop = 0;
+    for (int i0 = 0; i0 < n; i0 += 32) {
+        const int i = i0 + lane;
+        const int b = i < n ? bin(i) : -1;
+        const bool d = b >= 0 && b != k0 && b != k1 && b != k2;
+        if (d) drop(i);
+        ndrop += __popc(__ballot_sync(0xffffffffu, d));
+    }
+    return ndrop;
+}
+
+// Rcw * x + tcw of a pose (Tcw 3x4 row-major): cv::gemm runs a plain 3x3 * 3x1 (+ 3x1) CV_32F product in FLOAT, products summed left
+// to right, the addend last (probed on cv2 4.13, tools/probe_cv_gemm.py; the reference compiled over that model agrees with the oracle
+// in tests/test_ref_parity_cpu.py).  Explicit _rn intrinsics: no FMA contraction.
+__device__ __forceinline__ float rt_row(const float* T, float x0, float x1, float x2) {
+    return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[0], x0), __fmul_rn(T[1], x1)), __fmul_rn(T[2], x2)), T[3]);
 }
 
 // One warp per frame pair (blockIdx.x); see ProjPair for the layout.
 __global__ void __launch_bounds__(32) k_proj_match(const __grid_constant__ ProjArgs A, const __grid_constant__ ProjPair P) {
     __shared__ int s_hist[HISTO_LENGTH];
-    __shared__ int s_keep[3];
     __shared__ float s_T[12];
     const int lane = threadIdx.x, p = blockIdx.x;
     const int n1 = P.n ? min(P.n[p], P.cap) : P.n1, n2 = P.n ? min(P.n[p + 1], P.cap) : P.n2;
@@ -485,52 +562,39 @@ __global__ void __launch_bounds__(32) k_proj_match(const __grid_constant__ ProjA
             const int fl = flag1[i];
             if (!(fl & 1)) continue;
             const float X0 = Xw[3 * i], X1 = Xw[3 * i + 1], X2 = Xw[3 * i + 2];
-            const float* T = s_T;
-            // Rcw * x3Dw + tcw (ORBmatcher.cc:1364): cv::gemm runs a plain 3x3 * 3x1 (+ 3x1) CV_32F product in FLOAT, products summed
-            // left to right, the addend last (probed on cv2 4.13, tools/probe_cv_gemm.py; the reference compiled over that model
-            // agrees with the oracle in tests/test_ref_parity_cpu.py).  Explicit _rn intrinsics: no FMA contraction.
-            const float xc = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[0], X0), __fmul_rn(T[1], X1)), __fmul_rn(T[2], X2)), T[3]);
-            const float yc = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[4], X0), __fmul_rn(T[5], X1)), __fmul_rn(T[6], X2)), T[7]);
-            const float zc = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[8], X0), __fmul_rn(T[9], X1)), __fmul_rn(T[10], X2)), T[11]);
+            const float xc = rt_row(s_T, X0, X1, X2), yc = rt_row(s_T + 4, X0, X1, X2), zc = rt_row(s_T + 8, X0, X1, X2);   // :1364
             const float invzc = (float)(1.0 / (double)zc);
             if (invzc < 0) continue;
             const float u = __fadd_rn(__fmul_rn(__fmul_rn(A.fx, xc), invzc), A.cx), v = __fadd_rn(__fmul_rn(__fmul_rn(A.fy, yc), invzc), A.cy);
-            if (u < A.minX || u > A.maxX || v < A.minY || v > A.maxY) continue;
+            if (u < A.G.minX || u > A.G.maxX || v < A.G.minY || v > A.G.maxY) continue;
             const int lo = oct1[i * es1];
             if ((unsigned)lo >= (unsigned)A.nlevels) continue;        // outside mvScaleFactors: never read scale[] out of range
-            const float r = __fmul_rn(th, A.scale[lo]);
+            const float r = __fmul_rn(th, A.G.scale[lo]);
             const int minLevel = A.forward ? lo : (A.backward ? 0 : lo - 1), maxLevel = A.forward ? -1 : (A.backward ? lo : lo + 1);
-            int cx0, cx1, cy0, cy1;                                  // GetFeaturesInArea (Frame.cc:368-421)
-            if (!grid_window(A.minX, A.minY, A.invW, A.invH, u, v, r, cx0, cx1, cy0, cy1)) continue;
+            GridWin w;                                               // GetFeaturesInArea (Frame.cc:368-421)
+            if (!grid_window(A.G, u, v, r, w)) continue;
             const bool checkLevels = (minLevel > 0) || (maxLevel >= 0);
-            const int ny = cy1 - cy0 + 1, ncell = (cx1 - cx0 + 1) * ny;
             uint4 a0, a1;
             load_desc(dmp + (long long)i * 32, a0, a1);
             const float ur = __fsub_rn(u, __fmul_rn(A.mbf, invzc));
-            unsigned long long best = ~0ull;                         // (dist << 40) | (cell rank << 20) | position in the cell
-            for (int c = lane; c < ncell; c += 32) {
-                const int ix = cx0 + c / ny, iy = cy0 + c % ny, cell = ix * GRID_ROWS + iy;
-                const int b = goff[cell], e = goff[cell + 1];
-                for (int q = b; q < e; q++) {
-                    const int j = gidx[q];
-                    if (checkLevels) {
-                        const int o = oct2[j * es2];
-                        if (o < minLevel) continue;
-                        if (maxLevel >= 0 && o > maxLevel) continue;
-                    }
-                    if (!(fabsf(__fsub_rn(x2[j * es2], u)) < r && fabsf(__fsub_rn(y2[j * es2], v)) < r)) continue;
-                    if (claimed[j]) continue;                        // :1400-1402
-                    if (A.use_right && uright2[j * es2] > 0) { if (fabsf(__fsub_rn(ur, uright2[j * es2])) > r) continue; }
-                    uint4 b0, b1;
-                    load_desc(d2 + (long long)j * 32, b0, b1);
-                    const unsigned long long key = ((unsigned long long)popc256(a0, a1, b0, b1) << 40) | ((unsigned long long)c << 20) | (unsigned)(q - b);
-                    if (key < best) best = key;
+            // captured by value: by reference, ptxas spills at this kernel's 64 registers
+            const unsigned long long best = grid_min(goff, gidx, w, lane, [=](int j, int& d) {
+                if (checkLevels) {
+                    const int o = oct2[j * es2];
+                    if (o < minLevel) return false;
+                    if (maxLevel >= 0 && o > maxLevel) return false;
                 }
-            }
-            best = warp_min(best);
+                if (!(fabsf(__fsub_rn(x2[j * es2], u)) < r && fabsf(__fsub_rn(y2[j * es2], v)) < r)) return false;
+                if (claimed[j]) return false;                           // :1400-1402
+                if (A.use_right && uright2[j * es2] > 0) { if (fabsf(__fsub_rn(ur, uright2[j * es2])) > r) return false; }
+                uint4 b0, b1;
+                load_desc(d2 + (long long)j * 32, b0, b1);
+                d = popc256(a0, a1, b0, b1);
+                return true;
+            });
             const int bestDist = best == ~0ull ? 256 : (int)(best >> 40);
             if (bestDist <= TH_HIGH) {
-                const int j = grid_key_feature(goff, gidx, cx0, cy0, ny, best);
+                const int j = grid_key_feature(goff, gidx, w, best);
                 if (lane == 0) {
                     assign2[j] = i; claimed[j] = (fl >> 1) & 1;
                     sel[i] = j;
@@ -543,18 +607,9 @@ __global__ void __launch_bounds__(32) k_proj_match(const __grid_constant__ ProjA
             __syncwarp();
         }
         __syncwarp();
-        if (A.checkOri) {
-            if (lane == 0) { const int3 k = three_maxima(s_hist); s_keep[0] = k.x; s_keep[1] = k.y; s_keep[2] = k.z; }
-            __syncwarp();
-            const int k0 = s_keep[0], k1 = s_keep[1], k2 = s_keep[2];
-            for (int i0 = 0; i0 < n1; i0 += 32) {
-                const int i = i0 + lane;
-                bool drop = false;
-                if (i < n1 && sel[i] >= 0) { const int b = rbin[i]; drop = (b != k0 && b != k1 && b != k2); }
-                if (drop) assign2[sel[i]] = -2;                       // assigned, then removed by the rotation check: the reference NULLs it explicitly (:1461)
-                nmatches -= __popc(__ballot_sync(0xffffffffu, drop));
-            }
-        }
+        if (A.checkOri)                                              // assigned, then removed: the reference NULLs it explicitly (:1461)
+            nmatches -= warp_rot_check(s_hist, n1, lane, [&](int i) { return sel[i] >= 0 ? (int)rbin[i] : -1; },
+                                       [&](int i) { assign2[sel[i]] = -2; });
         if (pass > 0 || nmatches >= A.retry_below) break;
         __syncwarp();                                                // the rotation check's writes land before the next pass resets
     }
@@ -570,7 +625,7 @@ __global__ void __launch_bounds__(32) k_proj_match(const __grid_constant__ ProjA
 // (distance, traversal position) order: that is what the two-key reduction below computes.
 // -------------------------------------------------------------------------------------------------
 constexpr int TH_LOW_I = 50;                        // ORBmatcher.cc:38
-struct WinArgs { float minX, minY, invW, invH, th, nnratio; int bFactor, use_right, checkOri, window; float scale[32]; };
+struct WinArgs { GridGeom G; float th, nnratio; int bFactor, use_right, checkOri, window; };
 
 __global__ void __launch_bounds__(32) k_proj_match_mps(const __grid_constant__ WinArgs A, int nmp, const uint8_t* flag /* bit0 in view && !bad, bit1 obs>0 */,
                                                         const float* px, const float* py, const float* pxr, const int* level, const float* viewcos, const uint8_t* dmp,
@@ -586,39 +641,31 @@ __global__ void __launch_bounds__(32) k_proj_match_mps(const __grid_constant__ W
         const int lvl = level[i];
         float r = (double)viewcos[i] > 0.998 ? 2.5f : 4.0f;       // RadiusByViewingCos (:131-137)
         if (A.bFactor) r = __fmul_rn(r, A.th);
-        const float rad = __fmul_rn(r, A.scale[lvl]);
+        const float rad = __fmul_rn(r, A.G.scale[lvl]);
         const float u = px[i], v = py[i];
-        int cx0, cx1, cy0, cy1;
-        if (!grid_window(A.minX, A.minY, A.invW, A.invH, u, v, rad, cx0, cx1, cy0, cy1)) continue;
+        GridWin w;
+        if (!grid_window(A.G, u, v, rad, w)) continue;
         const int minLevel = lvl - 1, maxLevel = lvl;            // GetFeaturesInArea(..., nPredictedLevel-1, nPredictedLevel)
         const bool checkLevels = (minLevel > 0) || (maxLevel >= 0);
-        const int ny = cy1 - cy0 + 1, ncell = (cx1 - cx0 + 1) * ny;
         uint4 a0, a1;
         load_desc(dmp + (long long)i * 32, a0, a1);
-        unsigned long long b1 = ~0ull, b2 = ~0ull;                // (dist << 40) | (cell rank << 20) | position in the cell
-        for (int c = lane; c < ncell; c += 32) {
-            const int ix = cx0 + c / ny, iy = cy0 + c % ny, cell = ix * GRID_ROWS + iy;
-            const int b = goff[cell], e = goff[cell + 1];
-            for (int q = b; q < e; q++) {
-                const int j = gidx[q];
-                if (checkLevels) { const int o = oct2[j]; if (o < minLevel) continue; if (maxLevel >= 0 && o > maxLevel) continue; }
-                if (!(fabsf(__fsub_rn(x2[j], u)) < rad && fabsf(__fsub_rn(y2[j], v)) < rad)) continue;
-                if (claimed[j]) continue;                         // holds a MapPoint with observations (:86-88)
-                if (A.use_right && uright2[j] > 0) { if (fabsf(__fsub_rn(pxr[i], uright2[j])) > rad) continue; }
-                uint4 c0, c1;
-                load_desc(d2 + (long long)j * 32, c0, c1);
-                const int dist = popc256(a0, a1, c0, c1);
-                if (dist >= 256) continue;                        // never below the initial bestDist = bestDist2 = 256
-                top2_push(b1, b2, ((unsigned long long)dist << 40) | ((unsigned long long)c << 20) | (unsigned)(q - b));
-            }
-        }
-        top2_warp(b1, b2);
+        unsigned long long b1, b2;
+        grid_top2(goff, gidx, w, lane, [&](int j, int& d) {
+            if (checkLevels) { const int o = oct2[j]; if (o < minLevel) return false; if (maxLevel >= 0 && o > maxLevel) return false; }
+            if (!(fabsf(__fsub_rn(x2[j], u)) < rad && fabsf(__fsub_rn(y2[j], v)) < rad)) return false;
+            if (claimed[j]) return false;                            // holds a MapPoint with observations (:86-88)
+            if (A.use_right && uright2[j] > 0) { if (fabsf(__fsub_rn(pxr[i], uright2[j])) > rad) return false; }
+            uint4 c0, c1;
+            load_desc(d2 + (long long)j * 32, c0, c1);
+            d = popc256(a0, a1, c0, c1);
+            return d < 256;                                       // never below the initial bestDist = bestDist2 = 256
+        }, b1, b2);
         if (b1 == ~0ull) continue;
         const int bestDist = (int)(b1 >> 40);
         if (bestDist <= TH_HIGH) {
-            const int j = grid_key_feature(goff, gidx, cx0, cy0, ny, b1);
+            const int j = grid_key_feature(goff, gidx, w, b1);
             int bestDist2 = 256, bestLevel2 = -1;
-            if (b2 != ~0ull) { bestDist2 = (int)(b2 >> 40); bestLevel2 = oct2[grid_key_feature(goff, gidx, cx0, cy0, ny, b2)]; }
+            if (b2 != ~0ull) { bestDist2 = (int)(b2 >> 40); bestLevel2 = oct2[grid_key_feature(goff, gidx, w, b2)]; }
             if (oct2[j] == bestLevel2 && (float)bestDist > __fmul_rn(A.nnratio, (float)bestDist2)) continue;   // :117
             if (lane == 0) { assign2[j] = i; claimed[j] = (fl >> 1) & 1; }
             nmatches++;
@@ -720,10 +767,6 @@ __global__ void k_predict_scale(int n, const float* ratio, const __grid_constant
     if (i < n) level[i] = predict_scale(ratio[i], T.thr, T.nlevels, clamp != 0);
 }
 
-// Rcw * x + tcw of a KeyFrame pose (Tcw 3x4 row-major): cv::gemm's float path, products summed left to right, the addend last
-__device__ __forceinline__ float rt_row(const float* T, float x0, float x1, float x2) {
-    return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[0], x0), __fmul_rn(T[1], x1)), __fmul_rn(T[2], x2)), T[3]);
-}
 // Mat::dot of two float rows of 3 (double products and sum; the reference's sum starts from 0.0, which changes only the sign of an
 // exact zero, and no caller reads that sign), cv::norm (double accumulation, the double it returns) and (float)cv::norm(d), and the
 // double dot product with the normal of the viewing-angle gate
@@ -743,10 +786,10 @@ struct FuseMap {
     const float* kp; long long kp_fs; const uint8_t* desc; long long desc_fs; const int* n; int cap;
     const float* pose; const float* el; const uint8_t* eldesc;
     const int* goff; const int* gidx; long long goff_fs, gidx_fs;      // points: the 64 x 48 grid CSR of every keyframe
-    float fx, fy, cx, cy, minX, maxX, minY, maxY;
+    float fx, fy, cx, cy;
+    GridGeom G;
     PredictTable T;
     float invSigma2[SSLPL_MAX_LEVELS];
-    float scale[SSLPL_MAX_LEVELS];
 };
 
 // entry e of a batched call: false (and (-1, -1) written) when its keyframe or element index is out of range
@@ -769,7 +812,7 @@ __device__ __forceinline__ bool fuse_project_point(const FuseMap& M, int k, int 
     const float invz = __fdiv_rn(1.0f, zc);
     u = __fadd_rn(__fmul_rn(M.fx, __fmul_rn(rt_row(T, X0, X1, X2), invz)), M.cx);
     v = __fadd_rn(__fmul_rn(M.fy, __fmul_rn(rt_row(T + 4, X0, X1, X2), invz)), M.cy);
-    if (!(u >= M.minX && u < M.maxX && v >= M.minY && v < M.maxY)) return false;     // KeyFrame::IsInImage KeyFrame.cc:686-689
+    if (!(u >= M.G.minX && u < M.G.maxX && v >= M.G.minY && v < M.G.maxY)) return false;     // KeyFrame::IsInImage KeyFrame.cc:686-689
     const float d0 = __fsub_rn(X0, T[12]), d1 = __fsub_rn(X1, T[13]), d2 = __fsub_rn(X2, T[14]);
     const float dist = norm3d(d0, d1, d2);
     if (dist < P[6] || dist > P[7]) return false;
@@ -789,10 +832,10 @@ __device__ __forceinline__ bool fuse_project_line(const FuseMap& M, int k, int p
     const float iz1 = __fdiv_rn(1.0f, sz), iz2 = __fdiv_rn(1.0f, ez);
     q.x = __fadd_rn(__fmul_rn(__fmul_rn(M.fx, rt_row(T, s0, s1, s2)), iz1), M.cx);
     q.y = __fadd_rn(__fmul_rn(__fmul_rn(M.fy, rt_row(T + 4, s0, s1, s2)), iz1), M.cy);
-    if (q.x < M.minX || q.x > M.maxX || q.y < M.minY || q.y > M.maxY) return false;
+    if (q.x < M.G.minX || q.x > M.G.maxX || q.y < M.G.minY || q.y > M.G.maxY) return false;
     q.z = __fadd_rn(__fmul_rn(__fmul_rn(M.fx, rt_row(T, e0, e1, e2)), iz2), M.cx);
     q.w = __fadd_rn(__fmul_rn(__fmul_rn(M.fy, rt_row(T + 4, e0, e1, e2)), iz2), M.cy);
-    if (q.z < M.minX || q.z > M.maxX || q.w < M.minY || q.w > M.maxY) return false;
+    if (q.z < M.G.minX || q.z > M.G.maxX || q.w < M.G.minY || q.w > M.G.maxY) return false;
     const float d0 = __fsub_rn(__fmul_rn(0.5f, __fadd_rn(s0, e0)), T[12]), d1 = __fsub_rn(__fmul_rn(0.5f, __fadd_rn(s1, e1)), T[13]),
                 d2 = __fsub_rn(__fmul_rn(0.5f, __fadd_rn(s2, e2)), T[14]);
     const float dist = norm3d(d0, d1, d2);
@@ -821,7 +864,7 @@ __global__ void __launch_bounds__(128) k_line_fuse_search(int nml, const uint8_t
         if (!fuse_entry(M, i, lane, k, e, best_idx, best_dist)) return;
         act = e >= 0 && !(M.skip && M.skip[i]) && fuse_project_line(M, k, e, p, lvl);
         nl2 = min(M.n[k], M.cap); ld2 = M.desc + k * M.desc_fs; kl2 = M.kp + k * M.kp_fs;
-        oct2 = reinterpret_cast<const int*>(kl2 + 2); scale = M.scale; dml = M.eldesc + (long long)e * 32;
+        oct2 = reinterpret_cast<const int*>(kl2 + 2); scale = M.G.scale; dml = M.eldesc + (long long)e * 32;
     } else {
         act = active[i];
         dml += (long long)i * 32;
@@ -857,7 +900,7 @@ __global__ void __launch_bounds__(128) k_point_fuse_search(const __grid_constant
     if (i >= nmp) return;
     constexpr int es = kMap ? 7 : 1;                     // keypoint fields: separate arrays or sslpl_keypoint rows
     unsigned long long b = ~0ull;
-    int cx0 = 0, cx1 = -1, cy0 = 0, cy1 = -1;
+    GridWin w;
     bool act;
     int lvl;
     float u, v, ur;
@@ -874,43 +917,34 @@ __global__ void __launch_bounds__(128) k_point_fuse_search(const __grid_constant
     }
     if (act) {
         if (!kMap) { lvl = level[i]; u = pu[i]; v = pv[i]; ur = pur[i]; }
-        const float rad = __fmul_rn(A.th, A.scale[lvl]);
-        if (grid_window(A.minX, A.minY, A.invW, A.invH, u, v, rad, cx0, cx1, cy0, cy1)) {
-            const int ny = cy1 - cy0 + 1, ncell = (cx1 - cx0 + 1) * ny;
+        const float rad = __fmul_rn(A.th, A.G.scale[lvl]);
+        if (grid_window(A.G, u, v, rad, w)) {
             uint4 a0, a1;
             load_desc(dmp, a0, a1);
-            for (int c = lane; c < ncell; c += 32) {
-                const int ix = cx0 + c / ny, iy = cy0 + c % ny, cell = ix * GRID_ROWS + iy;
-                const int qb = goff[cell], qe = goff[cell + 1];
-                for (int q = qb; q < qe; q++) {
-                    const int j = gidx[q];
-                    const float kx = x2[es * j], ky = y2[es * j];
-                    if (!(fabsf(__fsub_rn(kx, u)) < rad && fabsf(__fsub_rn(ky, v)) < rad)) continue;     // KeyFrame::GetFeaturesInArea KeyFrame.cc:642
-                    const int o = oct2[es * j];
-                    if (o < lvl - 1 || o > lvl) continue;                                                 // :905
-                    if (kMap && o < 0) continue;
-                    const float ex = __fsub_rn(u, kx), ey = __fsub_rn(v, ky);
-                    float e2 = __fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey));
-                    const float kr = A.use_right ? uright2[j] : -1.f;
-                    if (kr >= 0) {                                                                        // stereo chi-square, 3 dof (:908-921)
-                        const float er = __fsub_rn(ur, kr);
-                        e2 = __fadd_rn(e2, __fmul_rn(er, er));
-                        if ((double)__fmul_rn(e2, invSigma2[o]) > 7.8) continue;
-                    } else if ((double)__fmul_rn(e2, invSigma2[o]) > 5.99) continue;                      // :923-932
-                    uint4 c0, c1;
-                    load_desc(d2 + (long long)j * 32, c0, c1);
-                    const int dist = popc256(a0, a1, c0, c1);
-                    if (dist >= 256) continue;                                                            // bestDist starts at 256, strict <
-                    const unsigned long long k = ((unsigned long long)dist << 40) | ((unsigned long long)c << 20) | (unsigned)(q - qb);
-                    b = k < b ? k : b;
-                }
-            }
-            b = warp_min(b);
+            b = grid_min(goff, gidx, w, lane, [&](int j, int& d) {
+                const float kx = x2[es * j], ky = y2[es * j];
+                if (!(fabsf(__fsub_rn(kx, u)) < rad && fabsf(__fsub_rn(ky, v)) < rad)) return false;        // KeyFrame::GetFeaturesInArea KeyFrame.cc:642
+                const int o = oct2[es * j];
+                if (o < lvl - 1 || o > lvl) return false;                                                    // :905
+                if (kMap && o < 0) return false;
+                const float ex = __fsub_rn(u, kx), ey = __fsub_rn(v, ky);
+                float e2 = __fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey));
+                const float kr = A.use_right ? uright2[j] : -1.f;
+                if (kr >= 0) {                                                                            // stereo chi-square, 3 dof (:908-921)
+                    const float er = __fsub_rn(ur, kr);
+                    e2 = __fadd_rn(e2, __fmul_rn(er, er));
+                    if ((double)__fmul_rn(e2, invSigma2[o]) > 7.8) return false;
+                } else if ((double)__fmul_rn(e2, invSigma2[o]) > 5.99) return false;                         // :923-932
+                uint4 c0, c1;
+                load_desc(d2 + (long long)j * 32, c0, c1);
+                d = popc256(a0, a1, c0, c1);
+                return d < 256;                                                                           // bestDist starts at 256, strict <
+            });
         }
     }
     if (lane == 0) {
         int bi = -1, bd = 256;
-        if (b != ~0ull) { bi = grid_key_feature(goff, gidx, cx0, cy0, cy1 - cy0 + 1, b); bd = (int)(b >> 40); }
+        if (b != ~0ull) { bi = grid_key_feature(goff, gidx, w, b); bd = (int)(b >> 40); }
         best_idx[i] = bi; best_dist[i] = bd;
     }
 }
@@ -920,7 +954,6 @@ __global__ void __launch_bounds__(32) k_init_match(const __grid_constant__ WinAr
                                                     const float* angle2, const int* goff, const int* gidx, int* matchedDist, int* matches21,
                                                     int32_t* matches12, uint8_t* rbin, int32_t* nmatch) {
     __shared__ int s_hist[HISTO_LENGTH];
-    __shared__ int s_keep[3];
     const int lane = threadIdx.x;
     for (int j = lane; j < n2; j += 32) { matchedDist[j] = 0x7fffffff; matches21[j] = -1; }
     for (int i = lane; i < n1; i += 32) { matches12[i] = -1; rbin[i] = 255; }
@@ -932,32 +965,24 @@ __global__ void __launch_bounds__(32) k_init_match(const __grid_constant__ WinAr
         const int level1 = oct1[i1];
         if (level1 > 0) continue;                                 // :426
         const float u = prevx[i1], v = prevy[i1];
-        int cx0, cx1, cy0, cy1;
-        if (!grid_window(A.minX, A.minY, A.invW, A.invH, u, v, rad, cx0, cx1, cy0, cy1)) continue;
-        const int ny = cy1 - cy0 + 1, ncell = (cx1 - cx0 + 1) * ny;
+        GridWin w;
+        if (!grid_window(A.G, u, v, rad, w)) continue;
         uint4 a0, a1;
         load_desc(d1 + (long long)i1 * 32, a0, a1);
-        unsigned long long b1 = ~0ull, b2 = ~0ull;
-        for (int c = lane; c < ncell; c += 32) {
-            const int ix = cx0 + c / ny, iy = cy0 + c % ny, cell = ix * GRID_ROWS + iy;
-            const int b = goff[cell], e = goff[cell + 1];
-            for (int q = b; q < e; q++) {
-                const int j = gidx[q];
-                { const int o = oct2[j]; if (o < level1 || o > level1) continue; }      // GetFeaturesInArea(..., level1, level1): levels are checked (maxLevel >= 0)
-                if (!(fabsf(__fsub_rn(x2[j], u)) < rad && fabsf(__fsub_rn(y2[j], v)) < rad)) continue;
-                uint4 c0, c1;
-                load_desc(d2 + (long long)j * 32, c0, c1);
-                const int dist = popc256(a0, a1, c0, c1);
-                if (matchedDist[j] <= dist) continue;             // :448
-                top2_push(b1, b2, ((unsigned long long)dist << 40) | ((unsigned long long)c << 20) | (unsigned)(q - b));
-            }
-        }
-        top2_warp(b1, b2);
+        unsigned long long b1, b2;
+        grid_top2(goff, gidx, w, lane, [&](int j, int& d) {
+            { const int o = oct2[j]; if (o < level1 || o > level1) return false; }     // GetFeaturesInArea(..., level1, level1): levels are checked (maxLevel >= 0)
+            if (!(fabsf(__fsub_rn(x2[j], u)) < rad && fabsf(__fsub_rn(y2[j], v)) < rad)) return false;
+            uint4 c0, c1;
+            load_desc(d2 + (long long)j * 32, c0, c1);
+            d = popc256(a0, a1, c0, c1);
+            return matchedDist[j] > d;                            // :448
+        }, b1, b2);
         if (b1 == ~0ull) continue;
         const int bestDist = (int)(b1 >> 40);
         const float bestDist2 = b2 == ~0ull ? (float)0x7fffffff : (float)(int)(b2 >> 40);
         if (bestDist <= TH_LOW_I && (float)bestDist < __fmul_rn(bestDist2, A.nnratio)) {       // :462-464
-            const int j = grid_key_feature(goff, gidx, cx0, cy0, ny, b1);
+            const int j = grid_key_feature(goff, gidx, w, b1);
             const int old = matches21[j];
             if (old >= 0) nmatches--;
             if (lane == 0) {
@@ -970,18 +995,9 @@ __global__ void __launch_bounds__(32) k_init_match(const __grid_constant__ WinAr
         __syncwarp();
     }
     __syncwarp();
-    if (A.checkOri) {
-        if (lane == 0) { const int3 k = three_maxima(s_hist); s_keep[0] = k.x; s_keep[1] = k.y; s_keep[2] = k.z; }
-        __syncwarp();
-        const int k0 = s_keep[0], k1 = s_keep[1], k2 = s_keep[2];
-        for (int i0 = 0; i0 < n1; i0 += 32) {
-            const int i = i0 + lane;
-            bool drop = false;
-            if (i < n1 && rbin[i] != 255) { const int b = rbin[i]; drop = (b != k0 && b != k1 && b != k2) && matches12[i] >= 0; }
-            if (drop) matches12[i] = -1;
-            nmatches -= __popc(__ballot_sync(0xffffffffu, drop));
-        }
-    }
+    if (A.checkOri)                                               // rbin[i] stays set when a later feature takes match i's j
+        nmatches -= warp_rot_check(s_hist, n1, lane, [&](int i) { return rbin[i] != 255 && matches12[i] >= 0 ? (int)rbin[i] : -1; },
+                                   [&](int i) { matches12[i] = -1; });
     __syncwarp();
     for (int i = lane; i < n1; i += 32) { const int j = matches12[i]; if (j >= 0) { prevx[i] = x2[j]; prevy[i] = y2[j]; } }   // :517-520
     if (lane == 0) *nmatch = nmatches;
@@ -2014,9 +2030,9 @@ __global__ void k_reloc_pairs(int nq, const int32_t* query, const int32_t* cand,
 // stride cap); the keyframe's MapPoints are element indices kfmp[row][i] into el[m][9] = Xw, normal, GetMinDistanceInvariance(),
 // GetMaxDistanceInvariance(), mfMaxDistance and eldesc[m][32] (the Fuse / map-refresh element table).
 struct RelocArgs {
-    float fx, fy, cx, cy, minX, maxX, minY, maxY, invW, invH, th;
+    float fx, fy, cx, cy, th;
     int ORBdist, checkOri;
-    float scale[SSLPL_MAX_LEVELS];                   // the frame's mvScaleFactors
+    GridGeom G;                                      // the frame's bounds, grid and mvScaleFactors
     PredictTable T;                                  // MapPoint::PredictScale(dist, Frame*) (MapPoint.cc:407-422) with the frame's mfLogScaleFactor
 };
 struct RelocSet {
@@ -2054,7 +2070,6 @@ __global__ void __launch_bounds__(128) k_reloc_gather_xy(const __grid_constant__
 // points); the lanes share each search window.
 __global__ void __launch_bounds__(32) k_proj_match_kf(const __grid_constant__ RelocArgs A, const __grid_constant__ RelocSet R) {
     __shared__ int s_hist[HISTO_LENGTH];
-    __shared__ int s_keep[3];
     __shared__ float s_T[12], s_Ow[3];
     const int lane = threadIdx.x, p = blockIdx.x;
     int32_t* assign = R.assign + (long long)p * R.cap;
@@ -2092,35 +2107,27 @@ __global__ void __launch_bounds__(32) k_proj_match_kf(const __grid_constant__ Re
         const float xc = rt_row(T, X0, X1, X2), yc = rt_row(T + 4, X0, X1, X2), zc = rt_row(T + 8, X0, X1, X2);
         const float invzc = (float)(1.0 / (double)zc);
         const float u = __fadd_rn(__fmul_rn(__fmul_rn(A.fx, xc), invzc), A.cx), v = __fadd_rn(__fmul_rn(__fmul_rn(A.fy, yc), invzc), A.cy);
-        if (u < A.minX || u > A.maxX || v < A.minY || v > A.maxY) continue;
+        if (u < A.G.minX || u > A.G.maxX || v < A.G.minY || v > A.G.maxY) continue;
         const float dist3D = norm3d(__fsub_rn(X0, s_Ow[0]), __fsub_rn(X1, s_Ow[1]), __fsub_rn(X2, s_Ow[2]));
         if (dist3D < P[6] || dist3D > P[7]) continue;                                 // :1523-1524
         const int lvl = predict_scale(__fdiv_rn(P[8], dist3D), A.T.thr, A.T.nlevels, true);
-        const float r = __fmul_rn(A.th, A.scale[lvl]);
-        int cx0, cx1, cy0, cy1;                                                        // GetFeaturesInArea(u, v, r, lvl - 1, lvl + 1)
-        if (!grid_window(A.minX, A.minY, A.invW, A.invH, u, v, r, cx0, cx1, cy0, cy1)) continue;
-        const int ny = cy1 - cy0 + 1, ncell = (cx1 - cx0 + 1) * ny;
+        const float r = __fmul_rn(A.th, A.G.scale[lvl]);
+        GridWin w;                                                                     // GetFeaturesInArea(u, v, r, lvl - 1, lvl + 1)
+        if (!grid_window(A.G, u, v, r, w)) continue;
         uint4 a0, a1;
         load_desc(R.eldesc + 32LL * e, a0, a1);
-        unsigned long long best = ~0ull;                                               // (dist << 40) | (cell rank << 20) | position in the cell
-        for (int c = lane; c < ncell; c += 32) {
-            const int cell = (cx0 + c / ny) * GRID_ROWS + cy0 + c % ny;
-            const int b = goff[cell], en = goff[cell + 1];
-            for (int q = b; q < en; q++) {
-                const int j = gidx[q];
-                const int o = __float_as_int(kp2[7LL * j + 5]);
-                if (o < lvl - 1 || o > lvl + 1) continue;
-                if (!(fabsf(__fsub_rn(kp2[7LL * j], u)) < r && fabsf(__fsub_rn(kp2[7LL * j + 1], v)) < r)) continue;
-                if (claimed[j]) continue;
-                uint4 b0, b1;
-                load_desc(d2 + 32LL * j, b0, b1);
-                const unsigned long long key = ((unsigned long long)popc256(a0, a1, b0, b1) << 40) | ((unsigned long long)c << 20) | (unsigned)(q - b);
-                if (key < best) best = key;
-            }
-        }
-        best = warp_min(best);
+        const unsigned long long best = grid_min(goff, gidx, w, lane, [&](int j, int& d) {
+            const int o = __float_as_int(kp2[7LL * j + 5]);
+            if (o < lvl - 1 || o > lvl + 1) return false;
+            if (!(fabsf(__fsub_rn(kp2[7LL * j], u)) < r && fabsf(__fsub_rn(kp2[7LL * j + 1], v)) < r)) return false;
+            if (claimed[j]) return false;
+            uint4 b0, b1;
+            load_desc(d2 + 32LL * j, b0, b1);
+            d = popc256(a0, a1, b0, b1);
+            return true;
+        });
         if (best != ~0ull && (int)(best >> 40) <= A.ORBdist) {                        // :1561 (ORBdist < 256: no candidate never passes)
-            const int j = grid_key_feature(goff, gidx, cx0, cy0, ny, best);
+            const int j = grid_key_feature(goff, gidx, w, best);
             if (lane == 0) {
                 assign[j] = i; claimed[j] = 1; sel[i] = j;
                 const int bin = rot_bin(kp1[7LL * i + 3], kp2[7LL * j + 3]);             // pKF->mvKeysUn[i].angle - F.mvKeysUn[j].angle (:1568)
@@ -2132,18 +2139,9 @@ __global__ void __launch_bounds__(32) k_proj_match_kf(const __grid_constant__ Re
         __syncwarp();
     }
     __syncwarp();
-    if (A.checkOri) {
-        if (lane == 0) { const int3 k = three_maxima(s_hist); s_keep[0] = k.x; s_keep[1] = k.y; s_keep[2] = k.z; }
-        __syncwarp();
-        const int k0 = s_keep[0], k1 = s_keep[1], k2 = s_keep[2];
-        for (int i0 = 0; i0 < n1; i0 += 32) {
-            const int i = i0 + lane;
-            bool drop = false;
-            if (i < n1 && sel[i] >= 0) { const int b = rbin[i]; drop = (b != k0 && b != k1 && b != k2); }
-            if (drop) assign[sel[i]] = -2;                                             // assigned, then NULLed by the rotation check (:1595)
-            nmatches -= __popc(__ballot_sync(0xffffffffu, drop));
-        }
-    }
+    if (A.checkOri)                                                                    // assigned, then NULLed by the rotation check (:1595)
+        nmatches -= warp_rot_check(s_hist, n1, lane, [&](int i) { return sel[i] >= 0 ? (int)rbin[i] : -1; },
+                                   [&](int i) { assign[sel[i]] = -2; });
     if (lane == 0) R.nmatch[p] = nmatches;
 }
 
@@ -2281,13 +2279,12 @@ int grid_staging_ok(const sslpl_matcher* m) {
 }
 // Frame::AssignFeaturesToGrid of the n2 features at (x[i], y[i]) into goff / gidx.  h_small is written here: the caller has synchronised
 // the stream since h_small's last asynchronous copy, and does not write it again before its next synchronisation.
-int grid_staging_build(sslpl_matcher* m, const float* x, const float* y, int n2, float minX, float minY, float invW, float invH,
-                       int*& goff, int*& gidx) {
+int grid_staging_build(sslpl_matcher* m, const float* x, const float* y, int n2, const GridGeom& G, int*& goff, int*& gidx) {
     const int nc = GRID_COLS * GRID_ROWS;
     goff = m->off + (m->p.max_nodes + 2); gidx = m->idx + m->cap;
     m->h_small[0] = n2;
     SSLPL_CUDA(cudaMemcpyAsync(m->ncnt, m->h_small, sizeof(int), cudaMemcpyHostToDevice, m->stream));
-    launch(m, k_grid_cells, (n2 + 127) / 128, 128, 0, x, y, 1, 0, nullptr, n2, n2, minX, minY, invW, invH, m->node, 0);
+    launch(m, k_grid_cells, (n2 + 127) / 128, 128, 0, x, y, 1, 0, nullptr, n2, n2, G, m->node, 0);
     launch(m, k_build_csr, 1, 128, (nc + 1 + m->cap) * sizeof(int), m->node, 0, m->ncnt, m->cap, nc, goff, 0, gidx, 0);
     return SSLPL_OK;
 }
@@ -2309,10 +2306,10 @@ int ensure_grid_ws(sslpl_matcher* m) {
 }
 // Frame::AssignFeaturesToGrid of nframes frames in HBM (sslpl_keypoint rows from kp, frame stride 7 cap floats, counts n[f]): the grid CSR
 // of frame f at pw_off + f (nc + 1), pw_idx + f fc; the caller has checked csr_fits(3072, cap)
-int grid_batch_build(sslpl_matcher* m, const float* kp, const int* n, int nframes, int cap, float minX, float minY, float invW, float invH) {
+int grid_batch_build(sslpl_matcher* m, const float* kp, const int* n, int nframes, int cap, const GridGeom& G) {
     if (int rc = ensure_grid_ws(m)) return rc;
     const int fc = m->p.max_features + 64, nc = GRID_COLS * GRID_ROWS;
-    launch(m, k_grid_cells, dim3((cap + 127) / 128, nframes), 128, 0, kp, kp + 1, 7, 7LL * cap, n, 0, cap, minX, minY, invW, invH, m->pw_cell, fc);
+    launch(m, k_grid_cells, dim3((cap + 127) / 128, nframes), 128, 0, kp, kp + 1, 7, 7LL * cap, n, 0, cap, G, m->pw_cell, fc);
     launch(m, k_build_csr, nframes, 128, (nc + 1 + cap) * sizeof(int), m->pw_cell, fc, n, cap, nc, m->pw_off, nc + 1, m->pw_idx, fc);
     return SSLPL_OK;
 }
@@ -2675,6 +2672,8 @@ int sslpl_search_by_projection_frame(sslpl_matcher* m,
     SSLPL_REQUIRE(n1 == 0 || (valid1 && obs1 && Xw && dmp && oct1 && angle1), SSLPL_ERR_ARG, "null last-frame array");
     SSLPL_REQUIRE(n2 == 0 || (d2 && x2 && y2 && oct2 && angle2), SSLPL_ERR_ARG, "null current-frame array");
     SSLPL_REQUIRE(bMono || Tlw, SSLPL_ERR_ARG, "the stereo direction test needs the last frame's pose");
+    ProjArgs A; memset(&A, 0, sizeof(A));
+    if (int rc = grid_geom(A.G, bounds, scaleFactors, nlevels)) return rc;
     for (int j = 0; j < n2; j++) assign2[j] = -1;
     *nmatches = 0;
     if (n1 == 0 || n2 == 0) return SSLPL_OK;
@@ -2682,13 +2681,9 @@ int sslpl_search_by_projection_frame(sslpl_matcher* m,
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
     const int cap = m->cap;
-    ProjArgs A; memset(&A, 0, sizeof(A));
     for (int k = 0; k < 12; k++) A.T[k] = Tcw[k];
     A.fx = cam[0]; A.fy = cam[1]; A.cx = cam[2]; A.cy = cam[3]; A.mbf = cam[4];
-    A.minX = bounds[0]; A.maxX = bounds[1]; A.minY = bounds[2]; A.maxY = bounds[3];
-    A.invW = (float)GRID_COLS / (bounds[1] - bounds[0]); A.invH = (float)GRID_ROWS / (bounds[3] - bounds[2]);   // Frame.cc:115-116
     A.th = th; A.checkOri = checkOri ? 1 : 0; A.use_right = uright2 ? 1 : 0; A.nlevels = nlevels;
-    for (int k = 0; k < nlevels; k++) A.scale[k] = scaleFactors[k];
     if (!bMono) {                                                        // tlc = Rlw * (-Rcw^T tcw) + tlw against the baseline (:1352-1353)
         float twc[3];
         for (int r = 0; r < 3; r++) twc[r] = (float)(-((double)Tcw[r] * Tcw[3] + (double)Tcw[4 + r] * Tcw[7] + (double)Tcw[8 + r] * Tcw[11]));
@@ -2717,7 +2712,7 @@ int sslpl_search_by_projection_frame(sslpl_matcher* m,
     else SSLPL_CUDA(cudaMemsetAsync(m->flag + cap, 0, n2, st));
     SSLPL_CUDA(cudaStreamSynchronize(st));                               // fl (pageable) is reused by the caller
     int *goff, *gidx;
-    if (int rc = grid_staging_build(m, k1, k1 + cap, n2, A.minX, A.minY, A.invW, A.invH, goff, gidx)) return rc;
+    if (int rc = grid_staging_build(m, k1, k1 + cap, n2, A.G, goff, gidx)) return rc;
     ProjPair P; memset(&P, 0, sizeof(P));
     P.n1 = n1; P.n2 = n2; P.cap = cap;
     P.flag1 = m->flag; P.Xw = k0; P.dmp = m->desc; P.angle1 = k0 + 3 * (size_t)cap; P.oct1 = reinterpret_cast<const int*>(k0 + 4 * (size_t)cap); P.es1 = 1;
@@ -2747,20 +2742,17 @@ int sslpl_search_by_projection_frame_batch_device(sslpl_matcher* m, const sslpl_
     SSLPL_REQUIRE(cap >= 1 && cap <= m->p.max_features + 64, SSLPL_ERR_ARG, "cap outside [1, max_features + 64]");
     SSLPL_REQUIRE(nlevels >= 1 && nlevels <= 32, SSLPL_ERR_ARG, "nlevels out of range");
     SSLPL_REQUIRE(th > 0.f, SSLPL_ERR_ARG, "th must be positive");
-    SSLPL_REQUIRE(bounds[1] > bounds[0] && bounds[3] > bounds[2], SSLPL_ERR_ARG, "degenerate image bounds");
+    ProjArgs A; memset(&A, 0, sizeof(A));
+    if (int rc = grid_geom(A.G, bounds, scaleFactors, nlevels)) return rc;
     const int nc = GRID_COLS * GRID_ROWS, npairs = nframes - 1;
     if (int rc = csr_fits(nc, cap)) return rc;
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     const int fc = m->p.max_features + 64;
-    ProjArgs A; memset(&A, 0, sizeof(A));
     A.fx = cam[0]; A.fy = cam[1]; A.cx = cam[2]; A.cy = cam[3];
-    A.minX = bounds[0]; A.maxX = bounds[1]; A.minY = bounds[2]; A.maxY = bounds[3];
-    A.invW = (float)GRID_COLS / (bounds[1] - bounds[0]); A.invH = (float)GRID_ROWS / (bounds[3] - bounds[2]);   // Frame.cc:115-116
     A.th = th; A.checkOri = checkOri ? 1 : 0; A.nlevels = nlevels; A.retry_below = retry_below;
-    for (int k = 0; k < nlevels; k++) A.scale[k] = scaleFactors[k];
     const float* kf = reinterpret_cast<const float*>(d_kps);            // sslpl_keypoint = 7 x 4 B: x y size angle response octave class_id
     const long long kfs = 7LL * cap;
-    if (int rc = grid_batch_build(m, kf + kfs, d_n + 1, npairs, cap, A.minX, A.minY, A.invW, A.invH)) return rc;
+    if (int rc = grid_batch_build(m, kf + kfs, d_n + 1, npairs, cap, A.G)) return rc;
     ProjPair P; memset(&P, 0, sizeof(P));
     P.n = d_n; P.cap = cap; P.Tcw = d_Tcw + 12;
     P.flag1 = d_mpflag; P.Xw = d_Xw; P.dmp = d_dmp ? d_dmp : d_desc; P.angle1 = kf + 3; P.oct1 = reinterpret_cast<const int*>(kf + 5);
@@ -2775,13 +2767,6 @@ int sslpl_search_by_projection_frame_batch_device(sslpl_matcher* m, const sslpl_
     return SSLPL_OK;
 }
 
-static void fill_win(WinArgs& A, const float* bounds, const float* scaleFactors, int nlevels) {
-    memset(&A, 0, sizeof(A));
-    A.minX = bounds[0]; A.minY = bounds[2];
-    A.invW = (float)GRID_COLS / (bounds[1] - bounds[0]); A.invH = (float)GRID_ROWS / (bounds[3] - bounds[2]);   // Frame.cc:115-116
-    for (int k = 0; k < nlevels && k < 32; k++) A.scale[k] = scaleFactors ? scaleFactors[k] : 1.f;
-}
-
 int sslpl_search_by_projection_mps(sslpl_matcher* m,
         int nmp, const uint8_t* inview, const uint8_t* bad, const uint8_t* obs, const float* projx, const float* projy, const float* projxr,
         const int32_t* level, const float* viewcos, const uint8_t* dmp,
@@ -2794,6 +2779,8 @@ int sslpl_search_by_projection_mps(sslpl_matcher* m,
     SSLPL_REQUIRE(nmp == 0 || (inview && projx && projy && level && viewcos && dmp), SSLPL_ERR_ARG, "null MapPoint array");
     SSLPL_REQUIRE(n2 == 0 || (d2 && x2 && y2 && oct2), SSLPL_ERR_ARG, "null frame array");
     SSLPL_REQUIRE(!uright2 || projxr, SSLPL_ERR_ARG, "stereo frame features need mTrackProjXR");
+    WinArgs A; memset(&A, 0, sizeof(A));
+    if (int rc = grid_geom(A.G, bounds, scaleFactors, nlevels)) return rc;
     for (int j = 0; j < n2; j++) assign2[j] = -1;
     *nmatches = 0;
     if (nmp == 0 || n2 == 0) return SSLPL_OK;
@@ -2801,7 +2788,6 @@ int sslpl_search_by_projection_mps(sslpl_matcher* m,
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
     const int cap = m->cap;
-    WinArgs A; fill_win(A, bounds, scaleFactors, nlevels);
     A.th = th; A.nnratio = nnratio; A.bFactor = th != 1.0f; A.use_right = uright2 ? 1 : 0;
     std::vector<uint8_t> fl(nmp), cl(n2, 0);
     for (int i = 0; i < nmp; i++) fl[i] = (uint8_t)(((inview[i] && !(bad && bad[i])) ? 1 : 0) | ((obs && obs[i]) ? 2 : 0));
@@ -2822,7 +2808,7 @@ int sslpl_search_by_projection_mps(sslpl_matcher* m,
     SSLPL_CUDA(cudaMemcpyAsync(m->flag + cap, cl.data(), n2, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaStreamSynchronize(st));                               // pageable staging vectors go out of scope
     int *goff, *gidx;
-    if (int rc = grid_staging_build(m, k1, k1 + cap, n2, A.minX, A.minY, A.invW, A.invH, goff, gidx)) return rc;
+    if (int rc = grid_staging_build(m, k1, k1 + cap, n2, A.G, goff, gidx)) return rc;
     launch(m, k_proj_match_mps, 1, 32, 0, A, nmp, m->flag, k0, k0 + cap, k0 + 2 * (size_t)cap, reinterpret_cast<const int*>(k0 + 4 * (size_t)cap), k0 + 3 * (size_t)cap, m->desc,
                                        n2, m->desc + (size_t)cap * 32, k1, k1 + cap, reinterpret_cast<const int*>(k1 + 4 * (size_t)cap), k1 + 3 * (size_t)cap,
                                        m->flag + cap, goff, gidx, m->out, m->nmatch);
@@ -2843,13 +2829,14 @@ int sslpl_search_for_initialization(sslpl_matcher* m,
     if (int rc = grid_staging_ok(m)) return rc;
     SSLPL_REQUIRE(n1 == 0 || (d1 && oct1 && angle1 && prev_xy), SSLPL_ERR_ARG, "null first-frame array");
     SSLPL_REQUIRE(n2 == 0 || (d2 && x2 && y2 && oct2 && angle2), SSLPL_ERR_ARG, "null second-frame array");
+    WinArgs A; memset(&A, 0, sizeof(A));
+    if (int rc = grid_geom(A.G, bounds, nullptr, 0)) return rc;
     for (int i = 0; i < n1; i++) matches12[i] = -1;
     *nmatches = 0;
     if (n1 == 0 || n2 == 0) return SSLPL_OK;
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
     const int cap = m->cap;
-    WinArgs A; fill_win(A, bounds, nullptr, 0);
     A.nnratio = nnratio; A.checkOri = checkOri ? 1 : 0; A.window = windowSize;
     std::vector<float> px(n1), py(n1);
     for (int i = 0; i < n1; i++) { px[i] = prev_xy[2 * i]; py[i] = prev_xy[2 * i + 1]; }
@@ -2866,7 +2853,7 @@ int sslpl_search_for_initialization(sslpl_matcher* m,
     SSLPL_CUDA(cudaMemcpyAsync(k1 + 4 * (size_t)cap, oct2, sizeof(int) * n2, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaStreamSynchronize(st));
     int *goff, *gidx;
-    if (int rc = grid_staging_build(m, k1, k1 + cap, n2, A.minX, A.minY, A.invW, A.invH, goff, gidx)) return rc;
+    if (int rc = grid_staging_build(m, k1, k1 + cap, n2, A.G, goff, gidx)) return rc;
     launch(m, k_init_match, 1, 32, 0, A, n1, m->desc, reinterpret_cast<const int*>(k0 + 4 * (size_t)cap), k0 + 3 * (size_t)cap, k0, k0 + cap,
                                    n2, m->desc + (size_t)cap * 32, k1, k1 + cap, reinterpret_cast<const int*>(k1 + 4 * (size_t)cap), k1 + 2 * (size_t)cap,
                                    goff, gidx, m->knn, m->knn + cap, m->out, m->rot, m->nmatch);
@@ -2962,12 +2949,13 @@ int sslpl_fuse_points_search(sslpl_matcher* m, int nmp, const uint8_t* active, c
     if (int rc = grid_staging_ok(m)) return rc;
     SSLPL_REQUIRE(nmp == 0 || (active && u && v && level && dmp && best_idx && best_dist), SSLPL_ERR_ARG, "null MapPoint array");
     SSLPL_REQUIRE(n2 == 0 || (d2 && x2 && y2 && oct2), SSLPL_ERR_ARG, "null KeyFrame array");
+    WinArgs A; memset(&A, 0, sizeof(A));
+    if (int rc = grid_geom(A.G, bounds, scaleFactors, nlevels)) return rc;
     for (int i = 0; i < nmp; i++) { best_idx[i] = -1; best_dist[i] = 256; }
     if (nmp == 0 || n2 == 0) return SSLPL_OK;
     for (int i = 0; i < nmp; i++) SSLPL_REQUIRE(!active[i] || (level[i] >= 0 && level[i] < nlevels), SSLPL_ERR_ARG, "predicted level outside the pyramid");
     SSLPL_CUDA(cudaSetDevice(m->p.device));
     cudaStream_t st = m->stream;
-    WinArgs A; fill_win(A, bounds, scaleFactors, nlevels);
     A.th = th; A.use_right = uright2 ? 1 : 0;
     const size_t need = (size_t)nmp * (1 + 12 + 4 + 32 + 8) + (size_t)n2 * (32 + 16) + 32 * 4 + 16 * 256 + 4096;
     if (int rc = ensure_scratch(m, need)) return rc;
@@ -2983,7 +2971,7 @@ int sslpl_fuse_points_search(sslpl_matcher* m, int nmp, const uint8_t* active, c
     SSLPL_CUDA(e);
     SSLPL_CUDA(cudaStreamSynchronize(st));
     int *goff, *gidx;
-    if (int rc = grid_staging_build(m, d_x2, d_y2, n2, A.minX, A.minY, A.invW, A.invH, goff, gidx)) return rc;
+    if (int rc = grid_staging_build(m, d_x2, d_y2, n2, A.G, goff, gidx)) return rc;
     FuseMap Z; memset(&Z, 0, sizeof(Z));
     launch(m, k_point_fuse_search<false>, (nmp + 3) / 4, 128, 0, A, nmp, d_act, d_u, d_v, d_ur, d_lvl, d_dmp, d_d2, d_x2, d_y2, d_oct, d_ur2, d_is2,
            goff, gidx, d_bi, d_bd, Z);
@@ -3463,14 +3451,12 @@ static int fuse_map_common(FuseMap& M, sslpl_matcher* m, int nkf, int cap, int r
     if (int rc = kf_set_ok(m, nkf, cap, rows)) return rc;
     SSLPL_REQUIRE(nel >= 0 && nentries >= 0, SSLPL_ERR_ARG, "negative count");
     SSLPL_REQUIRE(nlevels >= 1 && nlevels <= SSLPL_MAX_LEVELS, SSLPL_ERR_ARG, "nlevels outside [1, SSLPL_MAX_LEVELS]");
-    SSLPL_REQUIRE(bounds[1] > bounds[0] && bounds[3] > bounds[2], SSLPL_ERR_ARG, "degenerate image bounds");
     memset(&M, 0, sizeof(M));
+    if (int rc = grid_geom(M.G, bounds, scaleFactors, nlevels)) return rc;
     if (int rc = predict_table(M.T, logScaleFactor, nlevels)) return rc;
     M.entry = reinterpret_cast<const int2*>(d_entry); M.skip = d_skip; M.nkf = nkf; M.nel = nel;
     M.pose = d_kfpose; M.el = d_el; M.eldesc = d_eldesc;
     M.fx = cam[0]; M.fy = cam[1]; M.cx = cam[2]; M.cy = cam[3];
-    M.minX = bounds[0]; M.maxX = bounds[1]; M.minY = bounds[2]; M.maxY = bounds[3];
-    for (int k = 0; k < nlevels; k++) M.scale[k] = scaleFactors[k];
     return SSLPL_OK;
 }
 
@@ -3493,9 +3479,9 @@ int sslpl_fuse_points_batch_device(sslpl_matcher* m,
     for (int k = 0; k < nlevels; k++) M.invSigma2[k] = invLevelSigma2[k];
     const float* kf = reinterpret_cast<const float*>(d_kps);              // sslpl_keypoint = 7 x 4 B: x y size angle response octave class_id
     M.kp = kf; M.kp_fs = 7LL * cap; M.desc = d_desc; M.desc_fs = 32LL * cap; M.n = d_n; M.cap = cap;
-    WinArgs A; fill_win(A, bounds, scaleFactors, nlevels);
-    A.th = th;
-    if (int rc = grid_batch_build(m, kf, d_n, nkf, cap, A.minX, A.minY, A.invW, A.invH)) return rc;
+    WinArgs A; memset(&A, 0, sizeof(A));
+    A.G = M.G; A.th = th;
+    if (int rc = grid_batch_build(m, kf, d_n, nkf, cap, A.G)) return rc;
     M.goff = m->pw_off; M.gidx = m->pw_idx; M.goff_fs = nc + 1; M.gidx_fs = fc;
     launch(m, k_point_fuse_search<true>, (nentries + 3) / 4, 128, 0, A, nentries, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
            nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, d_best_idx, d_best_dist, M);
@@ -3587,17 +3573,14 @@ static int reloc_args(RelocArgs& A, const float* cam, const float* bounds, const
                int ORBdist, int checkOri) {
     SSLPL_REQUIRE(cam && bounds && scaleFactors, SSLPL_ERR_ARG, "null argument");
     SSLPL_REQUIRE(nlevels >= 1 && nlevels <= SSLPL_MAX_LEVELS, SSLPL_ERR_ARG, "nlevels outside [1, SSLPL_MAX_LEVELS]");
-    SSLPL_REQUIRE(bounds[1] > bounds[0] && bounds[3] > bounds[2], SSLPL_ERR_ARG, "degenerate image bounds");
+    memset(&A, 0, sizeof(A));
+    if (int rc = grid_geom(A.G, bounds, scaleFactors, nlevels)) return rc;
     SSLPL_REQUIRE(th > 0.f, SSLPL_ERR_ARG, "th must be positive");
     // with no candidate in the window bestDist stays 256 and bestIdx2 -1: ORBdist >= 256 would make the reference write mvpMapPoints[-1]
     SSLPL_REQUIRE(ORBdist < 256, SSLPL_ERR_ARG, "ORBdist must be below 256");
-    memset(&A, 0, sizeof(A));
     if (int rc = predict_table(A.T, logScaleFactor, nlevels)) return rc;
     A.fx = cam[0]; A.fy = cam[1]; A.cx = cam[2]; A.cy = cam[3];
-    A.minX = bounds[0]; A.maxX = bounds[1]; A.minY = bounds[2]; A.maxY = bounds[3];
-    A.invW = (float)GRID_COLS / (bounds[1] - bounds[0]); A.invH = (float)GRID_ROWS / (bounds[3] - bounds[2]);   // Frame.cc:115-116
     A.th = th; A.ORBdist = ORBdist; A.checkOri = checkOri ? 1 : 0;
-    for (int k = 0; k < nlevels; k++) A.scale[k] = scaleFactors[k];
     return SSLPL_OK;
 }
 
@@ -3609,7 +3592,7 @@ static int reloc_run(sslpl_matcher* m, const RelocArgs& A, RelocSet& R) {
     R.claimed = m->rw_claimed; R.sel = m->rw_sel; R.rbin = m->rw_rbin; R.ws_fs = W;
     launch(m, k_reloc_gather_xy, dim3((R.cap + 127) / 128, R.npairs), 128, 0, R);
     launch(m, k_grid_cells, dim3((R.cap + 127) / 128, R.npairs), 128, 0, m->rw_xy, m->rw_xy + 1, 2, 2LL * W, m->rw_n, 0, R.cap,
-           A.minX, A.minY, A.invW, A.invH, m->rw_cell, (long long)W);
+           A.G, m->rw_cell, (long long)W);
     launch(m, k_build_csr, R.npairs, 128, (nc + 1 + R.cap) * sizeof(int), m->rw_cell, (long long)W, m->rw_n, R.cap, nc, m->rw_off,
            (long long)(nc + 1), m->rw_idx, (long long)W);
     launch(m, k_proj_match_kf, R.npairs, 32, 0, A, R);

@@ -92,3 +92,8 @@ def test_row3_edge_cases(mt, oracle, pkg):
     qp["level"] = np.array([0], np.int32)
     bi, bd = mt.fuse_points_search(qp, np.zeros((1, 32), np.uint8), np.zeros((1, 32), np.uint8), [100.], [100.], [0], None, (0, 640, 0, 480), sf, 1 / (sf * sf), 3.0)
     assert list(bi) == [0] and list(bd) == [0]
+    for bad in ((640, 640, 0, 480), (0, 640, 480, 0)):                          # degenerate image bounds: rejected before any launch
+        before = mt.launch_count
+        with pytest.raises(pkg.SslplError):
+            mt.fuse_points_search(qp, np.zeros((1, 32), np.uint8), np.zeros((1, 32), np.uint8), [100.], [100.], [0], None, bad, sf, 1 / (sf * sf), 3.0)
+        assert mt.launch_count == before, bad

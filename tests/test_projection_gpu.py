@@ -34,6 +34,18 @@ def test_projection_edge_cases(pkg, oracle, synth):
         assert n_g == n_o and np.array_equal(a_g, a_o), mod
     with pytest.raises(pkg.SslplError):                                         # needs the 3072-cell grid
         pkg.Matcher(max_features=2048, max_nodes=100).search_by_projection_frame(last, cur, Tcw, Tlw, cam, bounds, sf, 15.0)
+    # degenerate image bounds (zero width, negative height) would give an infinite or negative grid cell: rejected before any launch
+    z32 = np.zeros((1, 32), np.uint8)
+    mp = dict(inview=[1], bad=[0], obs=[0], projx=[100.], projy=[100.], level=[0], viewcos=[1.], desc=z32)
+    one = dict(desc=z32, x=[100.], y=[100.], oct=[0], octave=[0], angle=[0.])
+    for bad in ((640., 640., 0., 480.), (0., 640., 480., 0.)):
+        for call in (lambda: mt.search_by_projection_frame(last, cur, Tcw, Tlw, cam, bad, sf, 15.0),
+                     lambda: mt.search_by_projection_mps(mp, one, bad, sf),
+                     lambda: mt.search_for_initialization(z32, one, z32, one, [[100., 100.]], bad)):
+            before = mt.launch_count
+            with pytest.raises(pkg.SslplError):
+                call()
+            assert mt.launch_count == before, bad
 
 
 @pytest.mark.parametrize("seed,th,ratio", [(1, 1.0, 0.8), (2, 3.0, 0.8), (3, 1.0, 0.6), (4, 5.0, 0.9)])
