@@ -242,6 +242,45 @@ int  sslpl_search_for_initialization(sslpl_matcher* m,
         int n1, const uint8_t* d1, const int32_t* oct1, const float* angle1, float* prev_xy,
         int n2, const uint8_t* d2, const float* x2, const float* y2, const int32_t* oct2, const float* angle2,
         const float* bounds, float nnratio, int checkOrientation, int windowSize, int32_t* matches12, int* nmatches);
+/* ---- Tracking::MonocularInitialization's matchers (Tracking.cc:328-420) over (initial frame, frame) pairs resident in HBM, asynchronous
+   on the handle's stream like the other *_batch_device calls; no caller-visible allocation.  While there is no map, every frame runs
+   ORBmatcher(0.9, true).SearchForInitialization(mInitialFrame, mCurrentFrame, mvbPrevMatched, mvIniMatches, 100) (:366) and
+   LSDmatcher::SerachForInitialize (:368); both frames come from the 2 x nFeatures extractor (:120, :163), so the matcher must be sized
+   for it (max_features >= 2 nFeatures, or cap from that extractor).  Initializer::Initialize and the reset rules (:354-376) stay with
+   the caller.
+   sslpl_search_for_initialization_batch_device: ORBmatcher::SearchForInitialization (ORBmatcher.cc:408-523) for every pair d_pair[p] =
+   (init row, current row) of a row set in the extractors' layout: d_kps[r][cap] = mvKeysUn (sslpl_frame_device_keypoints_un or
+   sslpl_orb_device_results), d_desc[r][cap][32], d_n[r] (clamped to [0, cap]); bounds = {mnMinX, mnMaxX, mnMinY, mnMaxY} (HOST, one
+   for all rows); nnratio, checkOrientation and windowSize as the reference takes them.
+   Chains: a maximal run of consecutive pairs with the same init row runs strictly in order, and vbPrevMatched is carried from one pair to
+   the next exactly as the reference carries it (rewritten at :516-520 and searched around by the next call).  d_prev0[npairs][cap][2]
+   (f32, may be NULL; must not overlap the outputs) holds the vbPrevMatched each chain starts from and is read only at slot c0 of the
+   chain that starts at pair c0; NULL means the init row's own keypoint positions (Tracking.cc:338-340).  Chains are independent, the
+   inputs are never modified, and the first k pairs of a chain give exactly what a call with only those k pairs gives, so a caller cuts
+   a chain where the reference resets (fewer than 100 point plus line matches) or where Initialize succeeds.  A pair with a row outside
+   [0, nrows) or with current row == init row gets the count -1, writes no rows and leaves the chain's state alone.  A current row may
+   appear more than once in a chain: each pair is simply the next call.
+   Results per pair p:
+     d_match12[p][cap]  vnMatches12 (-1 past the init row's count);
+     d_prev[p][cap][2]  vbPrevMatched after this pair (rows past the init row's count are not written); a caller continuing a chain in a
+                        later call passes the slot of its last good pair as that chain's d_prev0;
+     d_nmatch[p]        the return value.
+   Needs nrows in [2, max_batch + 1], npairs in [1, max_batch] and cap <= max_features + 64.  The grids of all rows go in the workspace of
+   sslpl_search_by_projection_frame_batch_device; the first call also allocates [max_batch][max_features + 64] per-chain scratch, freed
+   with the handle.  Bad arguments return SSLPL_ERR_ARG and enqueue nothing. */
+int  sslpl_search_for_initialization_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nrows, int cap, int npairs, const int32_t* d_pair,
+        const float* d_prev0, const float* bounds, float nnratio, int checkOrientation, int windowSize,
+        int32_t* d_match12, float* d_prev, int32_t* d_nmatch);
+/* sslpl_line_search_for_initialize_batch_device: LSDmatcher::SerachForInitialize (LSDmatcher.cpp:257-284), with Frame::lineDescriptorMAD
+   (Frame.cc:189-215) on the device, for every pair d_pair[p] = (init row, current row) of a line row set in the layout of
+   sslpl_line_device_results: d_ldesc[r][capl][32], d_nl[r] (clamped to [0, capl]).  Pairs are independent.  Result: d_lpairs[p][capl][2] =
+   (qdx, tdx) in ascending qdx, (-1, -1) after the count; d_nlmatch[p].  As in sslpl_line_search_for_triangulation_batch_device,
+   d_nlmatch[p] = -1 for a row outside [0, nrows) and when the init row has lines and the current row fewer than 2 (the reference reads
+   lmatches[i][1] out of bounds there; the single call returns SSLPL_ERR_ARG), and 0 when the init row has none.  Needs nrows in [1,
+   max_batch + 1], npairs in [1, max_batch] and capl <= max_lines + 64; bad arguments return SSLPL_ERR_ARG and enqueue nothing. */
+int  sslpl_line_search_for_initialize_batch_device(sslpl_matcher* m, const uint8_t* d_ldesc, const int* d_nl, int nrows, int capl,
+        int npairs, const int32_t* d_pair, int32_t* d_lpairs, int32_t* d_nlmatch);
 
 /* ---- Line projection matchers and Fuse (SURVEY.md 8(f) row 3).  Each reference function is a projection stage (per map element:
    gates and projected quantities, arithmetic in the reference's own cv::Mat / Eigen types - it stays in the adapter, host/matcher_b200.cc,

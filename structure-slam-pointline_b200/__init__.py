@@ -427,6 +427,17 @@ class Matcher(_Handle, kind="matcher", lifecycle=("sync", "set_stream", "stream"
                                                      _p(_f32(k2["angle"])), _p(_f32(bounds)), nnratio, int(check_ori), window, _p(m12), C.byref(nm)))
         return nm.value, m12[:len(k1)], prev
 
+    def search_for_initialization_batch_device(self, d_kps, d_desc, d_n, nrows, cap, npairs, d_pair, d_prev0, bounds, nnratio, check_ori,
+                                               window, d_match12, d_prev, d_nmatch):
+        """ORBmatcher::SearchForInitialization (ORBmatcher.cc:408-523) over the chains of a pair list of a row set in HBM (see
+        sslpl_search_for_initialization_batch_device): d_kps / d_desc / d_n as the extractors give them (2 x nFeatures), d_pair [npairs, 2]
+        i32 (init row, current row), d_prev0 [npairs, cap, 2] f32 or 0 (the init rows' keypoints), host bounds -> d_match12 [npairs, cap]
+        i32, d_prev [npairs, cap, 2] f32 (vbPrevMatched after each pair), d_nmatch [npairs] i32 (-1: bad pair).  Asynchronous on the
+        matcher's stream."""
+        _check(lib().sslpl_search_for_initialization_batch_device(self._h, d_kps, d_desc, d_n, nrows, cap, npairs, d_pair, d_prev0 or None,
+                                                                  _p(_f32(bounds)), nnratio, int(check_ori), window, d_match12, d_prev,
+                                                                  d_nmatch))
+
     def search_by_projection_frame(self, last, cur, Tcw, Tlw, cam, bounds, scale_factors, th, mono=True, check_ori=True, raw=False):
         """ORBmatcher::SearchByProjection(Frame &CurrentFrame, const Frame &LastFrame, th, bMono) (ORBmatcher.cc:1331-1473).
         last = dict(valid, obs, Xw[n,3], dmp[n,32], oct, angle); cur = dict(desc[n,32], x, y, oct, angle, uright|None, claimed|None);
@@ -493,6 +504,13 @@ class Matcher(_Handle, kind="matcher", lifecycle=("sync", "set_stream", "stream"
         KF1 has lines and KF2 fewer than 2).  Asynchronous on the matcher's stream."""
         _check(lib().sslpl_line_search_for_triangulation_batch_device(self._h, d_ldesc, d_nl, nkf, capl, d_has_ml, npairs, d_pair,
                                                                       d_lpairs, d_nlmatch))
+
+    def line_search_for_initialize_batch_device(self, d_ldesc, d_nl, nrows, capl, npairs, d_pair, d_lpairs, d_nlmatch):
+        """LSDmatcher::SerachForInitialize (LSDmatcher.cpp:257-284) for npairs (init row, current row) pairs of a line row set in HBM,
+        with Frame::lineDescriptorMAD on the device.  d_ldesc [nrows, capl, 32], d_nl [nrows], d_pair [npairs, 2] -> d_lpairs [npairs,
+        capl, 2] ((qdx, tdx) ascending qdx, -1 after the count), d_nlmatch [npairs] (-1: a row out of range, or an init row with lines
+        against a row with fewer than 2).  Asynchronous on the matcher's stream."""
+        _check(lib().sslpl_line_search_for_initialize_batch_device(self._h, d_ldesc, d_nl, nrows, capl, npairs, d_pair, d_lpairs, d_nlmatch))
 
     def create_new_map_points_batch_device(self, d_kps, d_desc, d_n, nkf, cap, d_has_mp, vocab, levelsup, npairs, d_pair, d_geom, d_kfpose,
                                            cam, scale_factors, level_sigma2, scale_factor, d_pairs, d_nmatch, d_status, d_x3d, d_nnew):

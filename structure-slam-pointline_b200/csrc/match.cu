@@ -949,10 +949,14 @@ __global__ void __launch_bounds__(128) k_point_fuse_search(const __grid_constant
     }
 }
 
-__global__ void __launch_bounds__(32) k_init_match(const __grid_constant__ WinArgs A, int n1, const uint8_t* d1, const int* oct1, const float* angle1,
-                                                    float* prevx, float* prevy, int n2, const uint8_t* d2, const float* x2, const float* y2, const int* oct2,
-                                                    const float* angle2, const int* goff, const int* gidx, int* matchedDist, int* matches21,
-                                                    int32_t* matches12, uint8_t* rbin, int32_t* nmatch) {
+// ORBmatcher::SearchForInitialization (ORBmatcher.cc:408-523) of one pair, run by one warp (the block's only one): F1's n1 features
+// (descriptors d1, octave / angle at element stride es) are searched around prev[i] = vbPrevMatched[i] (x, y interleaved) among F2's n2
+// features (fields at stride es) on F2's grid CSR goff / gidx.  matchedDist / matches21 [n2] and rbin [n1] are scratch; writes
+// matches12[n1] and prev (:517-520) and returns the count in every lane.
+template <int es>
+__device__ __forceinline__ int init_match(const WinArgs& A, int n1, const uint8_t* d1, const int* oct1, const float* angle1, float* prev,
+                                          int n2, const uint8_t* d2, const float* x2, const float* y2, const int* oct2, const float* angle2,
+                                          const int* goff, const int* gidx, int* matchedDist, int* matches21, int32_t* matches12, uint8_t* rbin) {
     __shared__ int s_hist[HISTO_LENGTH];
     const int lane = threadIdx.x;
     for (int j = lane; j < n2; j += 32) { matchedDist[j] = 0x7fffffff; matches21[j] = -1; }
@@ -962,17 +966,17 @@ __global__ void __launch_bounds__(32) k_init_match(const __grid_constant__ WinAr
     int nmatches = 0;
     const float rad = (float)A.window;
     for (int i1 = 0; i1 < n1; i1++) {
-        const int level1 = oct1[i1];
+        const int level1 = oct1[es * i1];
         if (level1 > 0) continue;                                 // :426
-        const float u = prevx[i1], v = prevy[i1];
+        const float u = prev[2 * i1], v = prev[2 * i1 + 1];
         GridWin w;
         if (!grid_window(A.G, u, v, rad, w)) continue;
         uint4 a0, a1;
         load_desc(d1 + (long long)i1 * 32, a0, a1);
         unsigned long long b1, b2;
         grid_top2(goff, gidx, w, lane, [&](int j, int& d) {
-            { const int o = oct2[j]; if (o < level1 || o > level1) return false; }     // GetFeaturesInArea(..., level1, level1): levels are checked (maxLevel >= 0)
-            if (!(fabsf(__fsub_rn(x2[j], u)) < rad && fabsf(__fsub_rn(y2[j], v)) < rad)) return false;
+            { const int o = oct2[es * j]; if (o < level1 || o > level1) return false; }   // GetFeaturesInArea(..., level1, level1): levels are checked (maxLevel >= 0)
+            if (!(fabsf(__fsub_rn(x2[es * j], u)) < rad && fabsf(__fsub_rn(y2[es * j], v)) < rad)) return false;
             uint4 c0, c1;
             load_desc(d2 + (long long)j * 32, c0, c1);
             d = popc256(a0, a1, c0, c1);
@@ -988,7 +992,7 @@ __global__ void __launch_bounds__(32) k_init_match(const __grid_constant__ WinAr
             if (lane == 0) {
                 if (old >= 0) matches12[old] = -1;
                 matches12[i1] = j; matches21[j] = i1; matchedDist[j] = bestDist;
-                if (A.checkOri) { const int bin = rot_bin(angle1[i1], angle2[j]); rbin[i1] = (uint8_t)bin; s_hist[bin]++; }
+                if (A.checkOri) { const int bin = rot_bin(angle1[es * i1], angle2[es * j]); rbin[i1] = (uint8_t)bin; s_hist[bin]++; }
             }
             nmatches++;
         }
@@ -999,8 +1003,21 @@ __global__ void __launch_bounds__(32) k_init_match(const __grid_constant__ WinAr
         nmatches -= warp_rot_check(s_hist, n1, lane, [&](int i) { return rbin[i] != 255 && matches12[i] >= 0 ? (int)rbin[i] : -1; },
                                    [&](int i) { matches12[i] = -1; });
     __syncwarp();
-    for (int i = lane; i < n1; i += 32) { const int j = matches12[i]; if (j >= 0) { prevx[i] = x2[j]; prevy[i] = y2[j]; } }   // :517-520
-    if (lane == 0) *nmatch = nmatches;
+    for (int i = lane; i < n1; i += 32) {                         // :517-520
+        const int j = matches12[i];
+        if (j >= 0) { prev[2 * i] = x2[es * j]; prev[2 * i + 1] = y2[es * j]; }
+    }
+    __syncwarp();
+    return nmatches;
+}
+
+// The single pair: fields in separate arrays
+__global__ void __launch_bounds__(32) k_init_match(const __grid_constant__ WinArgs A, int n1, const uint8_t* d1, const int* oct1, const float* angle1,
+                                                    float* prev, int n2, const uint8_t* d2, const float* x2, const float* y2, const int* oct2,
+                                                    const float* angle2, const int* goff, const int* gidx, int* matchedDist, int* matches21,
+                                                    int32_t* matches12, uint8_t* rbin, int32_t* nmatch) {
+    const int n = init_match<1>(A, n1, d1, oct1, angle1, prev, n2, d2, x2, y2, oct2, angle2, goff, gidx, matchedDist, matches21, matches12, rbin);
+    if (threadIdx.x == 0) *nmatch = n;
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1156,13 +1173,15 @@ __global__ void k_kfbow_slots(const int2* pmap, int npairs, int nrows, const int
 //   KeyFrame::lineDescriptorMAD's nn12_mad (KeyFrame.cc:820-846; the host form is line_mad() below) over all n1 query rows.  The
 //   distances are integers in [0, 256], so both medians are exact selections over a 257-bin histogram: med12 = element nq / 2 of the
 //   d1 - d0 sorted in DESCENDING order (conpare_descriptor_by_NN12_dist), then element nq / 2 of |d1 - d0 - med12| in ascending order;
-//   then the filter of :398-410 (skip rows whose KF1 or KF2 line has a MapLine, accept d1 - d0 > 0.1 nn12_mad) and an ordered
+//   then the filter of :398-410 (skip rows whose KF1 or KF2 line has a MapLine, accept d1 - d0 > fac nn12_mad, fac = 0.1) and an ordered
 //   compaction: lpairs[p][k] = (qdx, tdx) in ascending qdx, (-1, -1) past the count.
 // nlmatch[p] = -1 when an index is outside [0, nframes) or when KF1 has lines and KF2 fewer than 2 (the reference would read
 // lmatches[i][1] out of bounds, :402); 0 when KF1 has none.
-// nn12_mad * 0.1 (:406) of the n1 >= 1 rows of knn table K, computed by the whole CTA (every thread gets it); s_hist[257] and s_sel are
-// the caller's shared memory
-__device__ __forceinline__ double line_mad_thr(const int4* K, int n1, int tid, int* s_hist, int* s_sel) {
+// With has_ml NULL and fac = 0.5 it is LSDmatcher::SerachForInitialize (LSDmatcher.cpp:257-284; Frame::lineDescriptorMAD, Frame.cc:189-215,
+// computes the same nn12_mad), which tests no MapLines.
+// nn12_mad * fac of the n1 >= 1 rows of knn table K (fac: 0.1 for SearchForTriangulation :406, 0.5 for SerachForInitialize :270), computed
+// by the whole CTA (every thread gets it); s_hist[257] and s_sel are the caller's shared memory
+__device__ __forceinline__ double line_mad_thr(const int4* K, int n1, int tid, int* s_hist, int* s_sel, double fac) {
     const int k = n1 / 2;
     for (int i = tid; i < 257; i += 256) s_hist[i] = 0;
     __syncthreads();
@@ -1185,7 +1204,7 @@ __device__ __forceinline__ double line_mad_thr(const int4* K, int n1, int tid, i
         *s_sel = v;
     }
     __syncthreads();
-    return __dmul_rn(__dmul_rn(1.4826, (double)*s_sel), 0.1);
+    return __dmul_rn(__dmul_rn(1.4826, (double)*s_sel), fac);
 }
 // the KF2 and distance tests of :403-408 for knn row r (the KF1 test is the caller's)
 __device__ __forceinline__ bool line_row_ok(int4 r, const uint8_t* h2, double thr) {
@@ -1193,7 +1212,7 @@ __device__ __forceinline__ bool line_row_ok(int4 r, const uint8_t* h2, double th
 }
 
 __global__ void __launch_bounds__(256) k_line_tri(const int32_t* knn, long long knn_fs, const int* nl, int capl, const int2* pmap, int nframes,
-                                                   const uint8_t* has_ml, int32_t* lpairs, int32_t* nlmatch) {
+                                                   const uint8_t* has_ml, double fac, int32_t* lpairs, int32_t* nlmatch) {
     __shared__ int s_hist[257];
     __shared__ int s_warp[33];
     __shared__ int s_sel;
@@ -1207,15 +1226,16 @@ __global__ void __launch_bounds__(256) k_line_tri(const int32_t* knn, long long 
     const int4* K = reinterpret_cast<const int4*>(knn + p * knn_fs);
     int32_t* O = lpairs + 2LL * capl * p;
     if (ok && n1 > 0) {                                        // CTA-uniform
-        const double thr = line_mad_thr(K, n1, tid, s_hist, &s_sel);
-        const uint8_t* h1 = has_ml + (long long)f1 * capl; const uint8_t* h2 = has_ml + (long long)f2 * capl;
+        const double thr = line_mad_thr(K, n1, tid, s_hist, &s_sel, fac);
+        const uint8_t* h1 = has_ml ? has_ml + (long long)f1 * capl : nullptr; const uint8_t* h2 = has_ml ? has_ml + (long long)f2 * capl : nullptr;
+        const auto keep = [&](int i, int4 r) { return (!has_ml || (!h1[i] && !h2[r.x])) && (double)(r.w - r.y) > thr; };
         const int chunk = (n1 + 255) / 256, pb = min(n1, tid * chunk), pe = min(n1, pb + chunk);
         int c = 0;
-        for (int i = pb; i < pe; i++) { const int4 r = K[i]; c += !h1[i] && !h2[r.x] && (double)(r.w - r.y) > thr; }
+        for (int i = pb; i < pe; i++) c += keep(i, K[i]);
         int o = block_exclusive_scan(c, s_warp, &total);
         for (int i = pb; i < pe; i++) {
             const int4 r = K[i];
-            if (!h1[i] && !h2[r.x] && (double)(r.w - r.y) > thr) { O[2 * o] = i; O[2 * o + 1] = r.x; o++; }
+            if (keep(i, r)) { O[2 * o] = i; O[2 * o + 1] = r.x; o++; }
         }
     }
     for (int i = total + tid; i < capl; i += 256) { O[2 * i] = -1; O[2 * i + 1] = -1; }
@@ -1234,7 +1254,7 @@ __global__ void __launch_bounds__(256) k_line_tri_table(const int32_t* knn, long
     const int n1 = max(0, min(nl[f1], capl));
     if (n1 == 0 || min(nl[f2], capl) < 2) return;              // CTA-uniform
     const int4* K = reinterpret_cast<const int4*>(knn + p * knn_fs);
-    const double thr = line_mad_thr(K, n1, tid, s_hist, &s_sel);
+    const double thr = line_mad_thr(K, n1, tid, s_hist, &s_sel, 0.1);
     const uint8_t* h2 = has_ml + (long long)f2 * capl;
     int32_t* T = tw + (long long)capl * p;
     for (int i = tid; i < n1; i += 256) { const int4 r = K[i]; T[i] = line_row_ok(r, h2, thr) ? r.x : -1; }
@@ -1315,7 +1335,7 @@ __device__ __forceinline__ int create_point(const CreateArgs& C, const float* T1
     return CNMP_CREATED;
 }
 
-// The steps both chain kernels below share.  A chain is a maximal run [c0, c1) of consecutive pairs with the same kf1; false when pair c0
+// The steps the chain kernels below share.  A chain is a maximal run [c0, c1) of consecutive pairs with the same kf1; false when pair c0
 // does not start one.
 __device__ __forceinline__ bool chain_range(const int2* pmap, int npairs, int c0, int& kf1, int& c1) {
     kf1 = pmap[c0].x;
@@ -1324,6 +1344,50 @@ __device__ __forceinline__ bool chain_range(const int2* pmap, int npairs, int c0
     while (c1 < npairs && pmap[c1].x == kf1) c1++;
     return true;
 }
+
+// SearchForInitialization over the chains of a pair list (pmap[p] = (init row, current row) of a row set of sslpl_keypoint rows kp,
+// descriptors desc and counts n, cap rows each): block c0 runs the chain that starts at pair c0 (chain_range; other blocks return at
+// once), pair after pair, because each pair reads the vbPrevMatched the one before it left and the greedy scan inside a pair is itself
+// sequential.  The chain's state starts as prev0[c0] (NULL: the init row's keypoint positions); a good pair p copies it to prev[p],
+// updates it there and makes prev[p] the state of the next pair.  A pair with a row outside [0, nrows) or the init row as its current row
+// gets nmatch -1, writes no rows and leaves the state alone.  Row r2's grid CSR is goff + r2 goff_fs, gidx + r2 gidx_fs; the chain's
+// scratch is ws_* + c0 ws_fs.
+__global__ void __launch_bounds__(32) k_init_chain(const __grid_constant__ WinArgs A, const int2* pmap, int npairs, int nrows, const float* kp,
+                                                    const uint8_t* desc, const int* n_arr, int cap, const float* prev0,
+                                                    const int* goff, const int* gidx, long long goff_fs, long long gidx_fs,
+                                                    int* ws_dist, int* ws_m21, uint8_t* ws_rbin, long long ws_fs,
+                                                    int32_t* match12, float* prev, int32_t* nmatch) {
+    const int c0 = blockIdx.x, lane = threadIdx.x;
+    int r1, c1;
+    if (!chain_range(pmap, npairs, c0, r1, c1)) return;
+    const bool ok1 = (unsigned)r1 < (unsigned)nrows;
+    const int n1 = ok1 ? max(0, min(n_arr[r1], cap)) : 0;
+    const float* K1 = kp + 7LL * cap * (ok1 ? r1 : 0);
+    const float* src = prev0 ? prev0 + 2LL * cap * c0 : nullptr;
+    for (int p = c0; p < c1; p++) {
+        const int r2 = pmap[p].y;
+        if (!ok1 || (unsigned)r2 >= (unsigned)nrows || r2 == r1) {
+            if (lane == 0) nmatch[p] = -1;
+            continue;
+        }
+        float* P = prev + 2LL * cap * p;
+        for (int i = lane; i < n1; i += 32) {                     // Tracking.cc:338-340 without prev0
+            P[2 * i] = src ? src[2 * i] : K1[7 * i];
+            P[2 * i + 1] = src ? src[2 * i + 1] : K1[7 * i + 1];
+        }
+        __syncwarp();
+        const int n2 = max(0, min(n_arr[r2], cap));
+        const float* K2 = kp + 7LL * cap * r2;
+        int32_t* M = match12 + (long long)cap * p;
+        const int n = init_match<7>(A, n1, desc + 32LL * cap * r1, reinterpret_cast<const int*>(K1 + 5), K1 + 3, P, n2, desc + 32LL * cap * r2,
+                                    K2, K2 + 1, reinterpret_cast<const int*>(K2 + 5), K2 + 3, goff + goff_fs * r2, gidx + gidx_fs * r2,
+                                    ws_dist + ws_fs * c0, ws_m21 + ws_fs * c0, M, ws_rbin + ws_fs * c0);
+        for (int i = n1 + lane; i < cap; i += 32) M[i] = -1;
+        if (lane == 0) nmatch[p] = n;
+        src = P;
+    }
+}
+
 // s_bits = row kf1 of the mask as a bitmap of cap bits (all clear when !ok1), visible to the whole CTA on return
 __device__ __forceinline__ void chain_load_bits(unsigned* s_bits, const uint8_t* mask, int kf1, bool ok1, int cap, int tid) {
     const int words = (cap + 31) / 32;
@@ -2188,6 +2252,9 @@ struct sslpl_matcher : sslpl::StreamHandle {
     uint8_t* kb = nullptr;
     int32_t* kb_row = nullptr; int* kb_n = nullptr; int32_t* kb_node = nullptr; int* kb_off = nullptr; int* kb_idx = nullptr;
     int2* kb_pslot = nullptr; int* kb_fn = nullptr;
+    // per-chain scratch of sslpl_search_for_initialization_batch_device ([max_batch][max_features + 64]), allocated by its first call
+    uint8_t* iw = nullptr;
+    int* iw_dist = nullptr; int* iw_m21 = nullptr; uint8_t* iw_rbin = nullptr;
 };
 
 namespace {
@@ -2346,6 +2413,19 @@ int ensure_kfbow_ws(sslpl_matcher* m) {
     return SSLPL_OK;
 }
 
+int ensure_init_ws(sslpl_matcher* m) {
+    const int B = m->p.max_batch, fc = m->p.max_features + 64;
+    Arena A;
+    for (int k = 0; k < 2; k++) {
+        m->iw_dist = A.take<int>((size_t)B * fc); m->iw_m21 = A.take<int>((size_t)B * fc); m->iw_rbin = A.take<uint8_t>((size_t)B * fc);
+        if (k == 0) {
+            if (int rc = first_use(m->iw, A.used)) return rc;
+            A.base = m->iw; A.size = A.used; A.used = 0;
+        }
+    }
+    return SSLPL_OK;
+}
+
 // the sizes of a batched call over a keyframe set: nkf keyframes of cap rows (cap <= rows + 64: max_features or max_lines)
 int kf_set_ok(const sslpl_matcher* m, int nkf, int cap, int rows) {
     SSLPL_REQUIRE(nkf >= 1 && nkf <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nkf outside [1, max_batch + 1]");
@@ -2488,6 +2568,7 @@ void sslpl_matcher_destroy(sslpl_matcher* m) {
     if (m->ltw) cudaFree(m->ltw);
     if (m->rw) cudaFree(m->rw);
     if (m->kb) cudaFree(m->kb);
+    if (m->iw) cudaFree(m->iw);
     delete m;
 }
 
@@ -2838,13 +2919,10 @@ int sslpl_search_for_initialization(sslpl_matcher* m,
     cudaStream_t st = m->stream;
     const int cap = m->cap;
     A.nnratio = nnratio; A.checkOri = checkOri ? 1 : 0; A.window = windowSize;
-    std::vector<float> px(n1), py(n1);
-    for (int i = 0; i < n1; i++) { px[i] = prev_xy[2 * i]; py[i] = prev_xy[2 * i + 1]; }
-    float* k0 = m->kpf; float* k1 = m->kpf + (size_t)cap * 7;
+    float* k0 = m->kpf; float* k1 = m->kpf + (size_t)cap * 7;          // k0: prev [n1][2] in the first 2 cap floats, angle1, oct1
     SSLPL_CUDA(cudaMemcpyAsync(m->desc, d1, (size_t)n1 * 32, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(m->desc + (size_t)cap * 32, d2, (size_t)n2 * 32, cudaMemcpyHostToDevice, st));
-    SSLPL_CUDA(cudaMemcpyAsync(k0, px.data(), sizeof(float) * n1, cudaMemcpyHostToDevice, st));
-    SSLPL_CUDA(cudaMemcpyAsync(k0 + (size_t)cap, py.data(), sizeof(float) * n1, cudaMemcpyHostToDevice, st));
+    SSLPL_CUDA(cudaMemcpyAsync(k0, prev_xy, sizeof(float) * 2 * n1, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(k0 + 3 * (size_t)cap, angle1, sizeof(float) * n1, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(k0 + 4 * (size_t)cap, oct1, sizeof(int) * n1, cudaMemcpyHostToDevice, st));
     SSLPL_CUDA(cudaMemcpyAsync(k1, x2, sizeof(float) * n2, cudaMemcpyHostToDevice, st));
@@ -2854,17 +2932,41 @@ int sslpl_search_for_initialization(sslpl_matcher* m,
     SSLPL_CUDA(cudaStreamSynchronize(st));
     int *goff, *gidx;
     if (int rc = grid_staging_build(m, k1, k1 + cap, n2, A.G, goff, gidx)) return rc;
-    launch(m, k_init_match, 1, 32, 0, A, n1, m->desc, reinterpret_cast<const int*>(k0 + 4 * (size_t)cap), k0 + 3 * (size_t)cap, k0, k0 + cap,
+    launch(m, k_init_match, 1, 32, 0, A, n1, m->desc, reinterpret_cast<const int*>(k0 + 4 * (size_t)cap), k0 + 3 * (size_t)cap, k0,
                                    n2, m->desc + (size_t)cap * 32, k1, k1 + cap, reinterpret_cast<const int*>(k1 + 4 * (size_t)cap), k1 + 2 * (size_t)cap,
                                    goff, gidx, m->knn, m->knn + cap, m->out, m->rot, m->nmatch);
     SSLPL_CUDA(cudaGetLastError());
     SSLPL_CUDA(cudaMemcpyAsync(matches12, m->out, sizeof(int32_t) * n1, cudaMemcpyDeviceToHost, st));
-    SSLPL_CUDA(cudaMemcpyAsync(px.data(), k0, sizeof(float) * n1, cudaMemcpyDeviceToHost, st));
-    SSLPL_CUDA(cudaMemcpyAsync(py.data(), k0 + cap, sizeof(float) * n1, cudaMemcpyDeviceToHost, st));
+    SSLPL_CUDA(cudaMemcpyAsync(prev_xy, k0, sizeof(float) * 2 * n1, cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaMemcpyAsync(m->h_small, m->nmatch, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     SSLPL_CUDA(cudaStreamSynchronize(st));
-    for (int i = 0; i < n1; i++) { prev_xy[2 * i] = px[i]; prev_xy[2 * i + 1] = py[i]; }
     *nmatches = m->h_small[0];
+    return SSLPL_OK;
+}
+
+// The same matcher over the chains of a pair list of a row set in HBM: the grid of every row (one grid_batch_build), then k_init_chain, one
+// warp per chain.
+int sslpl_search_for_initialization_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const uint8_t* d_desc, const int* d_n, int nrows, int cap, int npairs, const int32_t* d_pair,
+        const float* d_prev0, const float* bounds, float nnratio, int checkOri, int windowSize,
+        int32_t* d_match12, float* d_prev, int32_t* d_nmatch) {
+    SSLPL_REQUIRE(m && d_kps && d_desc && d_n && d_pair && bounds && d_match12 && d_prev && d_nmatch, SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nrows >= 2 && nrows <= m->p.max_batch + 1, SSLPL_ERR_ARG, "nrows outside [2, max_batch + 1]");
+    SSLPL_REQUIRE(npairs >= 1 && npairs <= m->p.max_batch, SSLPL_ERR_ARG, "npairs outside [1, max_batch]");
+    SSLPL_REQUIRE(cap >= 1 && cap <= m->p.max_features + 64, SSLPL_ERR_ARG, "cap outside [1, max_features + 64]");
+    WinArgs A; memset(&A, 0, sizeof(A));
+    if (int rc = grid_geom(A.G, bounds, nullptr, 0)) return rc;
+    const int nc = GRID_COLS * GRID_ROWS;
+    if (int rc = csr_fits(nc, cap)) return rc;
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    A.nnratio = nnratio; A.checkOri = checkOri ? 1 : 0; A.window = windowSize;
+    if (int rc = ensure_init_ws(m)) return rc;
+    const float* kf = reinterpret_cast<const float*>(d_kps);
+    if (int rc = grid_batch_build(m, kf, d_n, nrows, cap, A.G)) return rc;
+    const int fc = m->p.max_features + 64;
+    launch(m, k_init_chain, npairs, 32, 0, A, reinterpret_cast<const int2*>(d_pair), npairs, nrows, kf, d_desc, d_n, cap, d_prev0,
+           m->pw_off, m->pw_idx, (long long)(nc + 1), (long long)fc, m->iw_dist, m->iw_m21, m->iw_rbin, (long long)fc, d_match12, d_prev, d_nmatch);
+    SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
 
@@ -3324,7 +3426,23 @@ int sslpl_line_search_for_triangulation_batch_device(sslpl_matcher* m, const uin
     const int2* pmap = reinterpret_cast<const int2*>(d_pair);
     launch(m, k_knn2<true>, dim3((capl + 7) / 8, npairs), 256, 0, d_ldesc, (long long)capl * 32, d_nl, 0, d_ldesc, (long long)capl * 32, d_nl, 0,
            m->b_knn, (long long)lc * 4, capl, pmap, nkf);
-    launch(m, k_line_tri, npairs, 256, 0, m->b_knn, (long long)lc * 4, d_nl, capl, pmap, nkf, d_has_ml, d_lpairs, d_nlmatch);
+    launch(m, k_line_tri, npairs, 256, 0, m->b_knn, (long long)lc * 4, d_nl, capl, pmap, nkf, d_has_ml, 0.1, d_lpairs, d_nlmatch);
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+// LSDmatcher::SerachForInitialize for a list of (initial frame, frame) pairs: k_knn2 over the pair map, then k_line_tri without masks at
+// 0.5 nn12_mad per pair.
+int sslpl_line_search_for_initialize_batch_device(sslpl_matcher* m, const uint8_t* d_ldesc, const int* d_nl, int nrows, int capl,
+        int npairs, const int32_t* d_pair, int32_t* d_lpairs, int32_t* d_nlmatch) {
+    SSLPL_REQUIRE(m && d_ldesc && d_nl && d_pair && d_lpairs && d_nlmatch, SSLPL_ERR_ARG, "null argument");
+    if (int rc = kf_pairs_ok(m, nrows, capl, m->p.max_lines, npairs)) return rc;
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    const int lc = m->p.max_lines + 64;
+    const int2* pmap = reinterpret_cast<const int2*>(d_pair);
+    launch(m, k_knn2<true>, dim3((capl + 7) / 8, npairs), 256, 0, d_ldesc, (long long)capl * 32, d_nl, 0, d_ldesc, (long long)capl * 32, d_nl, 0,
+           m->b_knn, (long long)lc * 4, capl, pmap, nrows);
+    launch(m, k_line_tri, npairs, 256, 0, m->b_knn, (long long)lc * 4, d_nl, capl, pmap, nrows, nullptr, 0.5, d_lpairs, d_nlmatch);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
