@@ -3,7 +3,7 @@
 //
 // Everything stays in HBM between the frame upload and the keypoint/descriptor download:
 //   k_resize      (x L-1)  level l-1 -> l, cv::resize(INTER_LINEAR) fixed-point          ORBextractor.cc:1107-1132
-//   k_fast                 one CTA per 30-px cell: FAST-9-16 score, in-cell NMS, 20/7 rule ORBextractor.cc:789-829
+//   k_fast                 one warp per 30-px cell, 4 cells per CTA: FAST-9-16, NMS, 20/7  ORBextractor.cc:789-829
 //   k_octree               one CTA per (level, frame): DistributeOctTree, array form       ORBextractor.cc:539-763
 //   k_blur                 7x7 sigma-2 fixed-point Gaussian of every level                 ORBextractor.cc:1085-1086
 //   k_orient_desc          one warp per keypoint: IC_Angle + rBRIEF + KeyPoint assembly    ORBextractor.cc:77-147,1043-1105
@@ -25,25 +25,24 @@ constexpr int MAXL = SSLPL_MAX_LEVELS;
 constexpr int EDGE = 19;            // EDGE_THRESHOLD, ORBextractor.cc:74
 constexpr int MINB = EDGE - 3;      // minBorderX/Y, ORBextractor.cc:775
 constexpr int HALF_PATCH = 15;
-constexpr int BLUR_TW = 64, BLUR_TH = 32;
 
 struct LevelGeom {
     int w, h, pitch;                 // level image (level 0: the input view's pitch is used instead)
     long long img_off;               // byte offset inside the per-frame pyramid block (levels >= 1)
     int bpitch; long long blur_off;  // blurred plane inside the per-frame blur block
     int nCols, nRows, wCell, hCell, maxBX, maxBY;
-    int cell_base, ncells, cell_cap;
+    int cell_base, ncells, cell_cap, strip_base;   // strip_base: first k_fast strip of the level
     long long cand_off;              // u32 offset inside the per-frame candidate block
     int key_cap; long long key_off;  // offset inside the per-frame key arrays
     int nfeat, kp_cap, kp_base;
     int pool_cap; long long pool_off;
     int xtab_off, ytab_off;          // resize tables (int2 entries)
-    int tile_base, tiles_x, tiles_y; // blur tiles (64x32 over the whole level)
+    int tile_base, tiles_x, tiles_y; // blur tiles (64x128 over the whole level)
     float scale, patch_size;
 };
 
 struct OrbGeom {
-    int nlevels, total_cells, total_tiles, kp_total_cap, iniTh, minTh, sort_cap;
+    int nlevels, total_cells, total_tiles, kp_total_cap, iniTh, minTh, sort_cap, total_strips;
     long long pyr_stride, blur_stride, cand_stride, key_stride, pool_stride;
     int umax[16];
     LevelGeom lv[MAXL];
@@ -58,12 +57,13 @@ struct OrbWs {
     int2* rtab;
     int* err;
     sslpl_keypoint* kps; uint8_t* desc; int* nkp;
-    CUtensorMap* tmaps;          // MAXL tensor maps in global memory (64-byte aligned)
+    CUtensorMap* tmaps;          // TMaps in global memory (64-byte aligned)
 };
 
 struct View { const uint8_t* base; int pitch; long long frame_stride; };
 
-struct TMaps { CUtensorMap lvl[MAXL]; };     // per pyramid level: 3-D (x, y, frame) u8 tensor map with the 96x38 box of the stencil kernels
+// per pyramid level: 3-D (x, y, frame) u8 tensor maps, one with k_fast's strip box and one with k_blur's tile box
+struct TMaps { CUtensorMap strip[MAXL], blur[MAXL]; };
 
 __constant__ signed char c_pattern[1024] = {
 #include "orb_pattern.inc"
@@ -194,13 +194,13 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* t
                  ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(x), "r"(y), "r"(z), "r"(smem_u32(bar)) : "memory");
 }
 
-constexpr int TL_W = 64, TL_H = 32;            // output tile of the stencil kernels
-constexpr int TL_P = 96, TL_IH = TL_H + 6;     // staged box: 96 x 38 bytes, origin (x0 - 16, y0 - 3).  Constraint: a TMA box of
-                                               // 1-byte elements must START on a 16-byte boundary in x (any other origin is an
-                                               // illegal instruction that kills the context), so every box origin is a multiple of 16
-constexpr int TL_X = 16;                       // smem column of the tile's first output pixel
+// A TMA box of 1-byte elements must START on a 16-byte boundary in x (any other origin is an illegal instruction that kills the
+// context), so every box origin below is a multiple of 16.
+constexpr int BLUR_TW = 64, BLUR_TH = 128;     // output tile of k_blur
+constexpr int BLUR_P = 96, BLUR_IH = BLUR_TH + 6;   // staged box: 96 x 134 bytes, origin (x0 - 16, y0 - 3)
+constexpr int BLUR_X = 16;                     // smem column of the tile's first output pixel
 
-// Stage the 96x38 box of level `l`, frame `f` at (bx, by) into s_img (pitch TL_P).  TMA path: one bulk tensor copy,
+// Stage the 96x134 box of level `l`, frame `f` at (bx, by) into s_img (pitch BLUR_P).  TMA path: one bulk tensor copy,
 // zero fill outside the level.  Fallback: aligned 32-bit loads (clamped to the row) or byte loads.
 template <bool TMA>
 __device__ __forceinline__ void stage_box(uint8_t* s_img, uint64_t* s_bar, const CUtensorMap* tm, const uint8_t* img, int pitch, int w, int h,
@@ -212,7 +212,7 @@ __device__ __forceinline__ void stage_box(uint8_t* s_img, uint64_t* s_bar, const
         if (tid == 0) {
             // the descriptor lives in global memory and level 0 is rewritten by the host between launches
             asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(reinterpret_cast<uint64_t>(tm + l)) : "memory");
-            mbar_expect_tx(s_bar, TL_P * TL_IH);
+            mbar_expect_tx(s_bar, BLUR_P * BLUR_IH);
             tma_load_3d(s_img, tm + l, bx, by, f, s_bar);
         }
         mbar_wait(s_bar, 0);
@@ -220,15 +220,15 @@ __device__ __forceinline__ void stage_box(uint8_t* s_img, uint64_t* s_bar, const
         const bool al = ((reinterpret_cast<uintptr_t>(img) | (unsigned)pitch) & 3) == 0 && (bx & 3) == 0 && bx >= 0;
         if (al) {
             const int wmax = (pitch - bx) / 4 - 1;                       // last whole word of the row
-            for (int i = tid; i < TL_IH * (TL_P / 4); i += blockDim.x) {
-                const int r = i / (TL_P / 4), wi = i - r * (TL_P / 4);
+            for (int i = tid; i < BLUR_IH * (BLUR_P / 4); i += blockDim.x) {
+                const int r = i / (BLUR_P / 4), wi = i - r * (BLUR_P / 4);
                 const int gy = min(max(by + r, 0), h - 1);
                 const uint32_t v = __ldg(reinterpret_cast<const uint32_t*>(img + (long long)gy * pitch + bx) + min(wi, wmax));
-                reinterpret_cast<uint32_t*>(s_img)[r * (TL_P / 4) + wi] = v;
+                reinterpret_cast<uint32_t*>(s_img)[r * (BLUR_P / 4) + wi] = v;
             }
         } else {
-            for (int i = tid; i < TL_IH * TL_P; i += blockDim.x) {
-                const int r = i / TL_P, c = i - r * TL_P;
+            for (int i = tid; i < BLUR_IH * BLUR_P; i += blockDim.x) {
+                const int r = i / BLUR_P, c = i - r * BLUR_P;
                 const int gy = min(max(by + r, 0), h - 1), gx = min(max(bx + c, 0), w - 1);
                 s_img[i] = __ldg(img + (long long)gy * pitch + gx);
             }
@@ -238,12 +238,19 @@ __device__ __forceinline__ void stage_box(uint8_t* s_img, uint64_t* s_bar, const
 }
 
 constexpr int FAST_MAXC = 60;                 // wCell, hCell < 60 (ceil(w / floor(w/30)) < 60)
-constexpr int FAST_TP = FAST_MAXC + 4;        // pitch of the per-cell score tile (1-px zero halo)
-constexpr int FC_ROWS = 36 + TL_IH;           // staged rows: two 96x38 boxes, the second one 36 rows down (36*96 is a multiple of 128)
+constexpr int FAST_STRIP = 4;                 // cells per k_fast CTA, one warp each, horizontally adjacent on one cell row
+// Strip box: FS_P x FS_IH bytes from the 16-byte boundary at or before the first cell's iniX.  A strip of k cells spans at most
+// 15 + k wCell + 6 bytes, and wCell <= 30 + ceil(29 / nCols) (nCols = floor(width / 30)): 4 cells of 38 (nCols = 4) need 173.
+constexpr int FS_P = 176, FS_IH = 38;
+constexpr int FS_ROWS = 32 + FS_IH;           // staged rows: two boxes for cells taller than 32 rows, the second one 32 rows down (32*176 is a multiple of 128)
 
-// One CTA per 30-px cell, the whole FAST stage in shared memory: stage the cell's (aw+6)x(ah+6) image box (TMA, the box
-// starts on the 16-byte boundary at or before iniX), score it in two phases, in-cell NMS, 20/7 rule, ordered compaction.
-//   phase A   the opposite-pair test on 4 pixels per thread with byte-SIMD video instructions; survivors are queued (~25 % of the pixels)
+// Per-warp shared memory of k_fast for cells of the level: three 64-bit masks per row (corners, NMS survivors, survivors >= iniTh), the
+// score tile (pitch 64, written at corners only) and the pixel queue (one entry per pixel of the cell in the worst case).
+__host__ __device__ __forceinline__ int fast_warp_smem(int wCell, int hCell) { return (88 * hCell + 2 * wCell * hCell + 15) & ~15; }
+
+// One warp per 30-px cell, FAST_STRIP horizontally adjacent cells of one level per CTA: stage the strip's image box once (TMA), then each
+// warp scores its own (aw+6)x(ah+6) cell box in two phases, in-cell NMS, 20/7 rule and ordered compaction, with warp primitives only.
+//   phase A   the opposite-pair test on 4 pixels per lane with byte-SIMD video instructions; survivors are queued (~25 % of the pixels)
 //   phase B1  the exact 9-arc corner test on 16-bit ring masks for the queued pixels; corners re-queued (~4 %)
 //   phase B2  the full 16-ring score only for corners, all lanes busy; NMS walks the corner queue, survivors land in per-row bit masks
 // Equivalent to the reference's per-cell cv::FAST(th=20) with fallback cv::FAST(th=7) (ORBextractor.cc:789-829): NMS
@@ -252,75 +259,81 @@ constexpr int FC_ROWS = 36 + TL_IH;           // staged rows: two 96x38 boxes, t
 // ever leaves the SM.
 template <bool TMA>
 __global__ void __launch_bounds__(128) k_fast(const __grid_constant__ OrbGeom g, OrbWs ws, View v, const CUtensorMap* tm) {
-    __shared__ __align__(128) uint8_t s_img[FC_ROWS * TL_P];
-    __shared__ __align__(4) uint8_t s_sc[(FAST_MAXC + 2) * FAST_TP];
-    __shared__ unsigned short s_q[FAST_MAXC * FAST_MAXC];
-    __shared__ unsigned long long s_rowall[FAST_MAXC], s_rowhi[FAST_MAXC];
-    __shared__ int s_warp[33];
-    __shared__ int s_qn, s_qc;
+    __shared__ __align__(128) uint8_t s_img[FS_ROWS * FS_P];
     __shared__ __align__(8) uint64_t s_bar;
-    const int cell = blockIdx.x, f = blockIdx.y, tid = threadIdx.x, lane = tid & 31;
+    extern __shared__ __align__(16) uint8_t s_warps[];
+    const int strip = blockIdx.x, f = blockIdx.y, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     int l = 0;
-    while (l + 1 < g.nlevels && cell >= g.lv[l + 1].cell_base) l++;
+    while (l + 1 < g.nlevels && strip >= g.lv[l + 1].strip_base) l++;
     const LevelGeom& L = g.lv[l];
-    const int ci = cell - L.cell_base, ci_i = ci / L.nCols, ci_j = ci - ci_i * L.nCols;
-    int* cnt_out = ws.cell_cnt + (long long)f * g.total_cells + cell;
-    const int iniX = MINB + ci_j * L.wCell, iniY = MINB + ci_i * L.hCell;
+    const int spr = (L.nCols + FAST_STRIP - 1) / FAST_STRIP;                  // strips per cell row
+    const int si = strip - L.strip_base, ci_i = si / spr, j0 = (si - ci_i * spr) * FAST_STRIP, ci_j = j0 + wid;
+    const int iniX0 = MINB + j0 * L.wCell, iniX = iniX0 + wid * L.wCell, iniY = MINB + ci_i * L.hCell;
     const int maxX = min(iniX + L.wCell + 6, L.maxBX), maxY = min(iniY + L.hCell + 6, L.maxBY);
     const int cw = maxX - iniX, ch = maxY - iniY;
-    if (iniX >= L.maxBX - 6 || iniY >= L.maxBY - 3 || cw < 7 || ch < 7) { if (tid == 0) *cnt_out = 0; return; }
-    const int aw = cw - 6, ah = ch - 6, area = aw * ah;
-    const int bx = iniX & ~15, xo = iniX + 3 - bx;          // smem column of the first detection pixel, 3..18
+    const int ci = ci_i * L.nCols + ci_j;
+    int* cnt_out = ws.cell_cnt + (long long)f * g.total_cells + L.cell_base + ci;
+    const bool live = ci_j < L.nCols && !(iniX >= L.maxBX - 6 || iniY >= L.maxBY - 3 || cw < 7 || ch < 7);
+    if (TMA && tid == 0) mbar_init(&s_bar, 1);
+    if (!__syncthreads_or(live)) { if (lane == 0 && ci_j < L.nCols) *cnt_out = 0; return; }
+    const int bx = iniX0 & ~15;
     int pitch;
     const uint8_t* img = level_ptr(g, ws, v, l, f, &pitch);
-    const bool two = ch > TL_IH;
+    const bool two = ch > FS_IH;
     if (TMA) {
-        if (tid == 0) mbar_init(&s_bar, 1);
-        __syncthreads();
         if (tid == 0) {
+            // the descriptor lives in global memory and level 0 is rewritten by the host between launches
             asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(reinterpret_cast<uint64_t>(tm + l)) : "memory");
-            mbar_expect_tx(&s_bar, (two ? 2 : 1) * TL_P * TL_IH);
+            mbar_expect_tx(&s_bar, (two ? 2 : 1) * FS_P * FS_IH);
             tma_load_3d(s_img, tm + l, bx, iniY, f, &s_bar);
-            if (two) tma_load_3d(s_img + 36 * TL_P, tm + l, bx, iniY + 36, f, &s_bar);   // rows 36, 37 arrive twice with the same bytes
+            if (two) tma_load_3d(s_img + 32 * FS_P, tm + l, bx, iniY + 32, f, &s_bar);   // rows 32..37 arrive twice with the same bytes
         }
     } else {
         const bool al = ((reinterpret_cast<uintptr_t>(img) | (unsigned)pitch) & 3) == 0;
-        const int rows = min(ch, FC_ROWS), wmax = (pitch - bx) / 4 - 1;
+        const int rows = min(ch, FS_ROWS), wmax = (pitch - bx) / 4 - 1;
         if (al) {
-            for (int i = tid; i < rows * (TL_P / 4); i += 128) {
-                const int r = i / (TL_P / 4), wi = i - r * (TL_P / 4);
+            for (int i = tid; i < rows * (FS_P / 4); i += 128) {
+                const int r = i / (FS_P / 4), wi = i - r * (FS_P / 4);
                 reinterpret_cast<uint32_t*>(s_img)[i] =
                     __ldg(reinterpret_cast<const uint32_t*>(img + (long long)min(iniY + r, L.h - 1) * pitch + bx) + min(wi, wmax));
             }
         } else {
-            for (int i = tid; i < rows * TL_P; i += 128) {
-                const int r = i / TL_P, c = i - r * TL_P;
+            for (int i = tid; i < rows * FS_P; i += 128) {
+                const int r = i / FS_P, c = i - r * FS_P;
                 s_img[i] = __ldg(img + (long long)min(iniY + r, L.h - 1) * pitch + min(bx + c, L.w - 1));
             }
         }
+        __syncthreads();
     }
-    if (tid == 0) { s_qn = 0; s_qc = 0; }
-    for (int i = tid; i < (ah + 2) * (FAST_TP / 4); i += 128) reinterpret_cast<uint32_t*>(s_sc)[i] = 0u;
-    if (tid < FAST_MAXC) { s_rowall[tid] = 0ull; s_rowhi[tid] = 0ull; }
+    if (!live) { if (lane == 0 && ci_j < L.nCols) *cnt_out = 0; return; }
+    const int aw = cw - 6, ah = ch - 6;
+    const int xo = iniX + 3 - bx;                                             // smem column of the cell's first detection pixel
+    unsigned long long* s_cm = reinterpret_cast<unsigned long long*>(s_warps + wid * fast_warp_smem(L.wCell, L.hCell));
+    unsigned long long* s_all = s_cm + ah;
+    unsigned long long* s_hi = s_all + ah;
+    uint8_t* s_sc = reinterpret_cast<uint8_t*>(s_hi + ah);                    // score of pixel p = (row << 6) + col, valid where s_cm is set
+    unsigned short* s_q = reinterpret_cast<unsigned short*>(s_sc + ah * 64);
+    for (int i = lane; i < 3 * ah; i += 32) s_cm[i] = 0ull;
     if (TMA) mbar_wait(&s_bar, 0);
-    __syncthreads();
+    __syncwarp();
     const int th = g.minTh;
     const unsigned ltmask = (1u << lane) - 1u;
     // phase A on the aligned word grid of the staged box: groups g0, g0+4, ... cover [xo, xo+aw)
     const unsigned T4 = 0x01010101u * (unsigned)th;
     const int g0 = xo & ~3, ng = (xo + aw - g0 + 3) >> 2, ngroups = ah * ng;
     const float inv_ng = __frcp_rn((float)ng);
-    for (int gb = 0; gb < ngroups; gb += 128) {
-        const int gidx = gb + tid;
+    int nq = 0;
+    for (int gb = 0; gb < ngroups; gb += 32) {
+        const int gidx = gb + lane;
         unsigned pm = 0;
         int r = 0, c4 = 0;
         if (gidx < ngroups) {
             r = __float2int_rz(__fmul_rn((float)gidx + 0.5f, inv_ng));                  // gidx / ng (exact: the quotient is >= 0.5/ng away from an integer)
             c4 = g0 + 4 * (gidx - r * ng);
-            const unsigned* row = reinterpret_cast<const unsigned*>(&s_img[(r + 3) * TL_P + c4]);
+            const unsigned* row = reinterpret_cast<const unsigned*>(&s_img[(r + 3) * FS_P + c4]);
             const unsigned C = row[0];
             const unsigned Rt = __byte_perm(row[0], row[1], 0x6543), Lf = __byte_perm(row[-1], row[0], 0x4321);   // x+3, x-3
-            const unsigned Dn = row[3 * (TL_P / 4)], Up = row[-3 * (TL_P / 4)];                                   // y+3 (k=0), y-3 (k=8)
+            const unsigned Dn = row[3 * (FS_P / 4)], Up = row[-3 * (FS_P / 4)];                                   // y+3 (k=0), y-3 (k=8)
             // A_k: centre brighter than ring_k by more than th; B_k: darker
             const unsigned A0 = __vcmpgtu4(__vsubus4(C, Dn), T4), A8 = __vcmpgtu4(__vsubus4(C, Up), T4);
             const unsigned A4 = __vcmpgtu4(__vsubus4(C, Rt), T4), A12 = __vcmpgtu4(__vsubus4(C, Lf), T4);
@@ -333,32 +346,30 @@ __global__ void __launch_bounds__(128) k_fast(const __grid_constant__ OrbGeom g,
         // warp prefix of the 0..4 survivors per lane from three ballots (the order inside the queue does not matter)
         const int cnt = __popc(pm);
         const unsigned b0 = __ballot_sync(0xffffffffu, cnt & 1), b1 = __ballot_sync(0xffffffffu, cnt & 2), b2 = __ballot_sync(0xffffffffu, cnt & 4);
-        const int tot = __popc(b0) + 2 * __popc(b1) + 4 * __popc(b2);
-        int base = 0;
-        if (lane == 0 && tot) base = atomicAdd(&s_qn, tot);
-        base = __shfl_sync(0xffffffffu, base, 0) + __popc(b0 & ltmask) + 2 * __popc(b1 & ltmask) + 4 * __popc(b2 & ltmask);
+        int base = nq + __popc(b0 & ltmask) + 2 * __popc(b1 & ltmask) + 4 * __popc(b2 & ltmask);
+        nq += __popc(b0) + 2 * __popc(b1) + 4 * __popc(b2);
         const int p0 = (r << 6) + c4 - xo;
 #pragma unroll
         for (int k = 0; k < 4; k++) if (pm & (1u << (8 * k))) s_q[base++] = (unsigned short)(p0 + k);
     }
-    __syncthreads();
+    __syncwarp();
     // phase B1: the exact corner test (9 contiguous ring pixels all brighter or all darker by more than th <=> score >= th) for the queued
-    // pixels, on 16-bit arc masks built with byte-SIMD compares; corners are compacted IN PLACE (entries are read a block of 128 ahead of
-    // where the survivors are written)
-    const int nq = s_qn;
-    for (int qb = 0; qb < nq; qb += 128) {
-        const int qi = qb + tid;
+    // pixels, on 16-bit arc masks built with byte-SIMD compares; corners are compacted IN PLACE (every lane has read its entry of the
+    // block before the ballot, and no survivor is written past the block)
+    int nc = 0;
+    for (int qb = 0; qb < nq; qb += 32) {
+        const int qi = qb + lane;
         bool corner = false;
         int p = 0;
         if (qi < nq) {
             p = s_q[qi];
-            const uint8_t* P = &s_img[((p >> 6) + 3) * TL_P + (p & 63) + xo];
+            const uint8_t* P = &s_img[((p >> 6) + 3) * FS_P + (p & 63) + xo];
             const unsigned v = P[0];
             const unsigned LO4 = 0x01010101u * (unsigned)max((int)v - th, 0), HI4 = 0x01010101u * (unsigned)min((int)v + th, 255);
-            const unsigned W0 = P[3 * TL_P] | (P[3 * TL_P + 1] << 8) | (P[2 * TL_P + 2] << 16) | (P[TL_P + 3] << 24);                    // ring 0..3
-            const unsigned W1 = P[3] | (P[-TL_P + 3] << 8) | (P[-2 * TL_P + 2] << 16) | (P[-3 * TL_P + 1] << 24);                       // 4..7
-            const unsigned W2 = P[-3 * TL_P] | (P[-3 * TL_P - 1] << 8) | (P[-2 * TL_P - 2] << 16) | (P[-TL_P - 3] << 24);               // 8..11
-            const unsigned W3 = P[-3] | (P[TL_P - 3] << 8) | (P[2 * TL_P - 2] << 16) | (P[3 * TL_P - 1] << 24);                         // 12..15
+            const unsigned W0 = P[3 * FS_P] | (P[3 * FS_P + 1] << 8) | (P[2 * FS_P + 2] << 16) | (P[FS_P + 3] << 24);                    // ring 0..3
+            const unsigned W1 = P[3] | (P[-FS_P + 3] << 8) | (P[-2 * FS_P + 2] << 16) | (P[-3 * FS_P + 1] << 24);                       // 4..7
+            const unsigned W2 = P[-3 * FS_P] | (P[-3 * FS_P - 1] << 8) | (P[-2 * FS_P - 2] << 16) | (P[-FS_P - 3] << 24);               // 8..11
+            const unsigned W3 = P[-3] | (P[FS_P - 3] << 8) | (P[2 * FS_P - 2] << 16) | (P[3 * FS_P - 1] << 24);                         // 12..15
             // byte masks -> 4 bits each: (m & 0x08040201) * 0x01010101 >> 24
 #define SSLPL_NIB(m) ((((m) & 0x08040201u) * 0x01010101u) >> 24)
             const unsigned br = SSLPL_NIB(__vcmpltu4(W0, LO4)) | (SSLPL_NIB(__vcmpltu4(W1, LO4)) << 4) | (SSLPL_NIB(__vcmpltu4(W2, LO4)) << 8) | (SSLPL_NIB(__vcmpltu4(W3, LO4)) << 12);
@@ -372,46 +383,58 @@ __global__ void __launch_bounds__(128) k_fast(const __grid_constant__ OrbGeom g,
             corner = ((ab | ad) & 0xffffu) != 0u;
         }
         const unsigned cb = __ballot_sync(0xffffffffu, corner);
-        __syncthreads();                                                                 // every entry of this block has been read
-        int base = 0;
-        if (lane == 0 && cb) base = atomicAdd(&s_qc, __popc(cb));
-        base = __shfl_sync(0xffffffffu, base, 0) + __popc(cb & ltmask);
-        if (corner) s_q[base] = (unsigned short)p;
+        if (corner) s_q[nc + __popc(cb & ltmask)] = (unsigned short)p;
+        nc += __popc(cb);
     }
-    __syncthreads();
-    // phase B2: the score of the corners, all lanes busy
-    const int nc = s_qc;
-    for (int qi = tid; qi < nc; qi += 128) {
+    __syncwarp();
+    // phase B2: the score of the corners, all lanes busy; a corner's score is >= th > 0
+    for (int qi = lane; qi < nc; qi += 32) {
         const int p = s_q[qi], r = p >> 6, c = p & 63;
-        s_sc[(r + 1) * FAST_TP + c + 1] = (uint8_t)fast_score_tile(&s_img[(r + 3) * TL_P + c + xo], TL_P, th);
+        s_sc[p] = (uint8_t)fast_score_tile(&s_img[(r + 3) * FS_P + c + xo], FS_P, th);
+        atomicOr(&s_cm[r], 1ull << c);
     }
-    __syncthreads();
-    // in-cell NMS of the corners; survivors as one bit per pixel in a 64-bit mask per row (all, and those >= iniTh)
-    for (int qi = tid; qi < nc; qi += 128) {
+    __syncwarp();
+    // in-cell NMS of the corners against their 8 neighbours, which score 0 unless they are corners (outside the detection area too);
+    // survivors as one bit per pixel in a 64-bit mask per row (all, and those >= iniTh)
+    for (int qi = lane; qi < nc; qi += 32) {
         const int p = s_q[qi], y = p >> 6, x = p & 63;
-        const uint8_t* c = &s_sc[(y + 1) * FAST_TP + x + 1];
-        const int sc = c[0];
-        if (sc > c[-1] && sc > c[1] && sc > c[-FAST_TP - 1] && sc > c[-FAST_TP] && sc > c[-FAST_TP + 1] &&
-            sc > c[FAST_TP - 1] && sc > c[FAST_TP] && sc > c[FAST_TP + 1]) {
-            atomicOr(&s_rowall[y], 1ull << x);
-            if (sc >= g.iniTh) atomicOr(&s_rowhi[y], 1ull << x);
+        const int sc = s_sc[p];
+        const unsigned up = y > 0 ? (unsigned)((s_cm[y - 1] << 1) >> x) : 0u;            // bit 0, 1, 2: columns x-1, x, x+1
+        const unsigned mid = (unsigned)((s_cm[y] << 1) >> x);
+        const unsigned dn = y + 1 < ah ? (unsigned)((s_cm[y + 1] << 1) >> x) : 0u;
+#define SSLPL_NB(m, k, q) (((m) >> (k) & 1u) ? (int)s_sc[q] : 0)
+        if (sc > SSLPL_NB(mid, 0, p - 1) && sc > SSLPL_NB(mid, 2, p + 1) && sc > SSLPL_NB(up, 0, p - 65) && sc > SSLPL_NB(up, 1, p - 64) &&
+            sc > SSLPL_NB(up, 2, p - 63) && sc > SSLPL_NB(dn, 0, p + 63) && sc > SSLPL_NB(dn, 1, p + 64) && sc > SSLPL_NB(dn, 2, p + 65)) {
+            atomicOr(&s_all[y], 1ull << x);
+            if (sc >= g.iniTh) atomicOr(&s_hi[y], 1ull << x);
         }
+#undef SSLPL_NB
     }
-    __syncthreads();
-    const unsigned long long mh = tid < ah ? s_rowhi[tid] : 0ull;
-    const int any_hi = __syncthreads_or(mh != 0ull);
-    unsigned long long m = tid < ah ? (any_hi ? mh : s_rowall[tid]) : 0ull;             // thread = row: raster order by an exclusive scan over the rows
-    int total;
-    int off = block_exclusive_scan(__popcll(m), s_warp, &total);
+    __syncwarp();
+    // lane = rows 2 lane and 2 lane + 1 (ah < 64): raster order by an exclusive warp scan over the row pairs
+    const int r0 = 2 * lane;
+    const unsigned long long h0 = r0 < ah ? s_hi[r0] : 0ull, h1 = r0 + 1 < ah ? s_hi[r0 + 1] : 0ull;
+    const bool any_hi = __any_sync(0xffffffffu, (h0 | h1) != 0ull);
+    const unsigned long long m0 = any_hi ? h0 : (r0 < ah ? s_all[r0] : 0ull), m1 = any_hi ? h1 : (r0 + 1 < ah ? s_all[r0 + 1] : 0ull);
+    const int n = __popcll(m0) + __popcll(m1);
+    int incl = n;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += t; }
+    const int total = __shfl_sync(0xffffffffu, incl, 31);
+    int off = incl - n;
     uint32_t* out = ws.cand + (long long)f * g.cand_stride + L.cand_off + (long long)ci * L.cell_cap;
     const int ox = iniX + 3 - MINB, oy = iniY + 3 - MINB;   // coordinates relative to (minBorderX, minBorderY)
-    for (; m; m &= m - 1ull) {
-        const int x = __ffsll((long long)m) - 1;
-        const int sc = s_sc[(tid + 1) * FAST_TP + x + 1];
-        if (off < L.cell_cap) out[off] = (uint32_t)(x + ox) | ((uint32_t)(tid + oy) << 12) | ((uint32_t)sc << 24);
-        off++;
+#pragma unroll
+    for (int k = 0; k < 2; k++) {
+        const int y = r0 + k;
+        for (unsigned long long m = k ? m1 : m0; m; m &= m - 1ull) {
+            const int x = __ffsll((long long)m) - 1;
+            const int sc = s_sc[(y << 6) + x];
+            if (off < L.cell_cap) out[off] = (uint32_t)(x + ox) | ((uint32_t)(y + oy) << 12) | ((uint32_t)sc << 24);
+            off++;
+        }
     }
-    if (tid == 0) { *cnt_out = min(total, L.cell_cap); if (total > L.cell_cap) atomicOr(ws.err, DERR_KEY_OVERFLOW); }
+    if (lane == 0) { *cnt_out = min(total, L.cell_cap); if (total > L.cell_cap) atomicOr(ws.err, DERR_KEY_OVERFLOW); }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -639,72 +662,74 @@ __global__ void __launch_bounds__(256) k_octree(const __grid_constant__ OrbGeom 
 // ------------------------------------------------------------------------------------------------
 template <bool TMA>
 __global__ void __launch_bounds__(256) k_blur(const __grid_constant__ OrbGeom g, OrbWs ws, View v, const CUtensorMap* tm) {
-    __shared__ __align__(128) uint8_t s_img[TL_IH * TL_P];
-    __shared__ __align__(16) unsigned s_pair[TL_IH * TL_W];             // [r][x] = row pass of row r | row r+1 << 16
+    __shared__ __align__(128) uint8_t s_img[BLUR_IH * BLUR_P];
+    __shared__ __align__(16) unsigned s_pair[BLUR_IH * BLUR_TW];         // [r][x] = row pass of row r | row r+1 << 16
     __shared__ __align__(8) uint64_t s_bar;
     const int tile = blockIdx.x, f = blockIdx.y, tid = threadIdx.x;
     int l = 0;
     while (l + 1 < g.nlevels && tile >= g.lv[l + 1].tile_base) l++;
     const LevelGeom& L = g.lv[l];
     const int t = tile - L.tile_base, ty = t / L.tiles_x, tx = t - ty * L.tiles_x;
-    const int x0 = tx * TL_W, y0 = ty * TL_H, bx = x0 - TL_X, by = y0 - 3;
+    const int x0 = tx * BLUR_TW, y0 = ty * BLUR_TH, bx = x0 - BLUR_X, by = y0 - 3;
     int pitch;
     const uint8_t* img = level_ptr(g, ws, v, l, f, &pitch);
-    const bool interior = bx >= 0 && by >= 0 && x0 + TL_W + 3 <= L.w && y0 + TL_H + 3 <= L.h;
+    const bool interior = bx >= 0 && by >= 0 && x0 + BLUR_TW + 3 <= L.w && y0 + BLUR_TH + 3 <= L.h;
     if (TMA || interior) {
         stage_box<TMA>(s_img, &s_bar, tm, img, pitch, L.w, L.h, l, f, bx, by);
         if (!interior) {
             // BORDER_REFLECT_101 on top of the zero-filled box: columns first (valid rows), then whole rows
-            for (int i = tid; i < TL_IH * 8; i += 256) {
+            for (int i = tid; i < BLUR_IH * 8; i += 256) {
                 const int r = i >> 3, k = i & 7, gy = by + r;
                 if (gy < 0 || gy >= L.h) continue;
-                const int c = k < 4 ? TL_X - 4 + k : (k - 4) + (L.w - bx);   // left halo cols (gx = x0-4..x0-1), right cols gx = w..w+3
+                const int c = k < 4 ? BLUR_X - 4 + k : (k - 4) + (L.w - bx);   // left halo cols (gx = x0-4..x0-1), right cols gx = w..w+3
                 const int gx = bx + c;
-                if (c >= 0 && c < TL_P && (gx < 0 || gx >= L.w)) { const int sxx = reflect101(gx, L.w) - bx; if (sxx >= 0 && sxx < TL_P) s_img[r * TL_P + c] = s_img[r * TL_P + sxx]; }
+                if (c >= 0 && c < BLUR_P && (gx < 0 || gx >= L.w)) { const int sxx = reflect101(gx, L.w) - bx; if (sxx >= 0 && sxx < BLUR_P) s_img[r * BLUR_P + c] = s_img[r * BLUR_P + sxx]; }
             }
             __syncthreads();
-            for (int i = tid; i < 6 * TL_P; i += 256) {
-                const int k = i / TL_P, c = i - k * TL_P;
+            for (int i = tid; i < 6 * BLUR_P; i += 256) {
+                const int k = i / BLUR_P, c = i - k * BLUR_P;
                 const int r = k < 3 ? k : (k - 3) + (L.h - by);            // top halo rows 0..2, bottom rows h-by..h-by+2
                 const int gy = by + r;
-                if (r >= 0 && r < TL_IH && (gy < 0 || gy >= L.h)) { const int sr = reflect101(gy, L.h) - by; if (sr >= 0 && sr < TL_IH) s_img[r * TL_P + c] = s_img[sr * TL_P + c]; }
+                if (r >= 0 && r < BLUR_IH && (gy < 0 || gy >= L.h)) { const int sr = reflect101(gy, L.h) - by; if (sr >= 0 && sr < BLUR_IH) s_img[r * BLUR_P + c] = s_img[sr * BLUR_P + c]; }
             }
             __syncthreads();
         }
     } else {
-        for (int i = tid; i < TL_IH * (TL_W + 6); i += 256) {
-            const int r = i / (TL_W + 6), c = i - r * (TL_W + 6) + TL_X - 3;
-            s_img[r * TL_P + c] = __ldg(img + (long long)reflect101(by + r, L.h) * pitch + reflect101(bx + c, L.w));
+        for (int i = tid; i < BLUR_IH * (BLUR_TW + 6); i += 256) {
+            const int r = i / (BLUR_TW + 6), c = i - r * (BLUR_TW + 6) + BLUR_X - 3;
+            s_img[r * BLUR_P + c] = __ldg(img + (long long)reflect101(by + r, L.h) * pitch + reflect101(bx + c, L.w));
         }
         __syncthreads();
     }
     // Packed arithmetic (taps 18 34 48 56 48 34 18): horizontal pass = two dp4a per output on byte windows cut out of three
-    // aligned words with funnel shifts (TL_X - 3 = 13 = 12 + 1); the u16 results are stored as vertical PAIRS
+    // aligned words with funnel shifts (BLUR_X - 3 = 13 = 12 + 1); the u16 results are stored as vertical PAIRS
     // (row r | row r+1 << 16) so that the vertical pass is four dp2a per output.  Partial sums stay below 2^16 / 2^32: exact.
-    static_assert(TL_X == 16 && TL_P % 4 == 0, "word-aligned row reads assume TL_X == 16");
+    // Only the rows of the level are computed: output row yy reads staged rows yy..yy+6 (the high half of the last pair has tap 0).
+    static_assert(BLUR_X == 16 && BLUR_P % 4 == 0 && BLUR_TW == 64, "word-aligned row reads assume BLUR_X == 16; 16 words per row");
+    const int orows = min(BLUR_TH, L.h - y0), irows = orows + 6;
     constexpr unsigned T0 = 18u | (34u << 8) | (48u << 16) | (56u << 24), T1 = 48u | (34u << 8) | (18u << 16);
     unsigned short* s_half = reinterpret_cast<unsigned short*>(s_pair);
-    for (int i = tid; i < TL_IH * (TL_W / 4); i += 256) {
+    for (int i = tid; i < irows * (BLUR_TW / 4); i += 256) {
         const int r = i >> 4, x4 = (i & 15) * 4;
-        const unsigned* w = reinterpret_cast<const unsigned*>(&s_img[r * TL_P + x4 + TL_X - 4]);
+        const unsigned* w = reinterpret_cast<const unsigned*>(&s_img[r * BLUR_P + x4 + BLUR_X - 4]);
         const unsigned w0 = w[0], w1 = w[1], w2 = w[2];                   // output k uses bytes 1 + k .. 7 + k of this window
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             const unsigned A = (k < 3) ? __funnelshift_r(w0, w1, 8 * (k + 1)) : w1;
             const unsigned B = (k < 3) ? __funnelshift_r(w1, w2, 8 * (k + 1)) : w2;
             const unsigned q = __dp4a(A, T0, __dp4a(B, T1, 0u));          // <= 65280
-            s_half[(r * TL_W + x4 + k) * 2] = (unsigned short)q;
-            if (r > 0) s_half[((r - 1) * TL_W + x4 + k) * 2 + 1] = (unsigned short)q;
+            s_half[(r * BLUR_TW + x4 + k) * 2] = (unsigned short)q;
+            if (r > 0) s_half[((r - 1) * BLUR_TW + x4 + k) * 2 + 1] = (unsigned short)q;
         }
     }
     __syncthreads();
     uint8_t* out = ws.blur + (long long)f * g.blur_stride + L.blur_off;
     constexpr unsigned C01 = 18u | (34u << 8), C23 = 48u | (56u << 8), C45 = 48u | (34u << 8), C6 = 18u;
-    for (int i = tid; i < TL_H * (TL_W / 4); i += 256) {
+    for (int i = tid; i < orows * (BLUR_TW / 4); i += 256) {
         const int yy = i >> 4, x4 = (i & 15) * 4;
-        if (y0 + yy >= L.h || x0 + x4 >= L.w) continue;
-        const uint4 p0 = *reinterpret_cast<const uint4*>(&s_pair[yy * TL_W + x4]), p2 = *reinterpret_cast<const uint4*>(&s_pair[(yy + 2) * TL_W + x4]);
-        const uint4 p4 = *reinterpret_cast<const uint4*>(&s_pair[(yy + 4) * TL_W + x4]), p6 = *reinterpret_cast<const uint4*>(&s_pair[(yy + 6) * TL_W + x4]);
+        if (x0 + x4 >= L.w) continue;
+        const uint4 p0 = *reinterpret_cast<const uint4*>(&s_pair[yy * BLUR_TW + x4]), p2 = *reinterpret_cast<const uint4*>(&s_pair[(yy + 2) * BLUR_TW + x4]);
+        const uint4 p4 = *reinterpret_cast<const uint4*>(&s_pair[(yy + 4) * BLUR_TW + x4]), p6 = *reinterpret_cast<const uint4*>(&s_pair[(yy + 6) * BLUR_TW + x4]);
         const unsigned a0 = __dp2a_lo(p0.x, C01, __dp2a_lo(p2.x, C23, __dp2a_lo(p4.x, C45, __dp2a_lo(p6.x, C6, 32768u))));
         const unsigned a1 = __dp2a_lo(p0.y, C01, __dp2a_lo(p2.y, C23, __dp2a_lo(p4.y, C45, __dp2a_lo(p6.y, C6, 32768u))));
         const unsigned a2 = __dp2a_lo(p0.z, C01, __dp2a_lo(p2.z, C23, __dp2a_lo(p4.z, C45, __dp2a_lo(p6.z, C6, 32768u))));
@@ -808,9 +833,9 @@ struct sslpl_orb : sslpl::StreamHandle {
     OrbGeom g; OrbWs ws; View view;
     uint8_t* d_input = nullptr;         // staging for host frames
     int cur_w = 0, cur_h = 0, cur_frames = 0;
-    int octree_smem = 0;
+    int octree_smem = 0, fast_smem = 0;
     int kp_max = 0;                     // keypoints per frame: make_geometry's kp_total_cap, the same for every frame size
-    TMaps tm;                           // per-level tensor maps (level 0 re-encoded per call: the input view moves)
+    TMaps tm;                           // per-level tensor maps (level 0's re-encoded per call: the input view moves)
     PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
     bool tma_levels_ok = false, use_tma = true;
     const uint8_t* tm0_base = nullptr; int tm0_pitch = 0, tm0_frames = 0; long long tm0_fs = 0;
@@ -868,7 +893,7 @@ void make_geometry(const sslpl_orb* h, int W, int H, OrbGeom& g, std::vector<int
     g.nlevels = L; g.iniTh = h->p.iniThFAST; g.minTh = h->p.minThFAST;
     for (int i = 0; i < 16; i++) g.umax[i] = h->umax[i];
     long long pyr = 0, blur = 0, cand = 0, key = 0, pool = 0;
-    int cells = 0, tiles = 0, kpc = 0, rt = 0, maxN = 2;
+    int cells = 0, strips = 0, tiles = 0, kpc = 0, rt = 0, maxN = 2;
     for (int l = 0; l < L; l++) {
         LevelGeom& G = g.lv[l];
         G.w = cvRoundF((float)W * h->invscale[l]); G.h = cvRoundF((float)H * h->invscale[l]);     // ORBextractor.cc:1111-1112
@@ -883,6 +908,7 @@ void make_geometry(const sslpl_orb* h, int W, int H, OrbGeom& g, std::vector<int
             G.wCell = (int)ceilf(width / G.nCols); G.hCell = (int)ceilf(height / G.nRows);         // :788-789
         } else { G.nCols = G.nRows = 0; G.wCell = G.hCell = 1; }
         G.cell_base = cells; G.ncells = G.nCols * G.nRows; cells += G.ncells;
+        G.strip_base = strips; strips += G.nRows * ((G.nCols + FAST_STRIP - 1) / FAST_STRIP);
         G.cell_cap = ((G.wCell + 1) / 2) * ((G.hCell + 1) / 2);        // NMS survivors are pairwise non-adjacent
         G.cand_off = cand; cand += (long long)G.ncells * G.cell_cap;
         G.key_cap = G.ncells * G.cell_cap; G.key_off = key; key += align_up(G.key_cap, 64);
@@ -895,7 +921,7 @@ void make_geometry(const sslpl_orb* h, int W, int H, OrbGeom& g, std::vector<int
         G.tile_base = tiles; tiles += G.tiles_x * G.tiles_y;
         G.scale = h->scale[l]; G.patch_size = (float)(int)(31 * h->scale[l]);                      // :836 (int truncation)
     }
-    g.total_cells = cells; g.total_tiles = tiles; g.kp_total_cap = kpc;
+    g.total_cells = cells; g.total_strips = strips; g.total_tiles = tiles; g.kp_total_cap = kpc;
     g.pyr_stride = pyr; g.blur_stride = blur; g.cand_stride = cand; g.key_stride = key; g.pool_stride = pool;
     int sc = 2; while (sc < maxN) sc <<= 1;
     g.sort_cap = sc;
@@ -944,18 +970,19 @@ int carve(sslpl_orb* h, Arena& A, const OrbGeom& g, int B, int W, int H) {
     ws.kps = A.take<sslpl_keypoint>((size_t)B * g.kp_total_cap);
     ws.desc = A.take<uint8_t>((size_t)B * g.kp_total_cap * 32);
     ws.nkp = A.take<int>(B);
-    ws.tmaps = A.take<CUtensorMap>(MAXL);
+    ws.tmaps = A.take<CUtensorMap>(sizeof(TMaps) / sizeof(CUtensorMap));
     return 0;
 }
 
-// 3-D u8 tensor map (x, y, frame) with an 80x38x1 box; returns false when the driver entry point is missing or the
+// 3-D u8 tensor map (x, y, frame) with a box_w x box_h x 1 box; returns false when the driver entry point is missing or the
 // view does not satisfy TMA's 16-byte alignment rules (then the kernels fall back to ordinary loads).
-bool encode_level_map(sslpl_orb* h, CUtensorMap* out, const uint8_t* base, int w, int hgt, int pitch, long long frame_stride, int frames) {
+bool encode_level_map(sslpl_orb* h, CUtensorMap* out, const uint8_t* base, int w, int hgt, int pitch, long long frame_stride, int frames,
+                      int box_w, int box_h) {
     if (!h->encode) return false;
     if ((reinterpret_cast<uintptr_t>(base) & 15) || (pitch & 15) || (frame_stride & 15) || w < 1 || hgt < 1 || frames < 1) return false;
     const cuuint64_t gdim[3] = {(cuuint64_t)w, (cuuint64_t)hgt, (cuuint64_t)frames};
     const cuuint64_t gstr[2] = {(cuuint64_t)pitch, (cuuint64_t)frame_stride};
-    const cuuint32_t box[3] = {(cuuint32_t)TL_P, (cuuint32_t)TL_IH, 1u};
+    const cuuint32_t box[3] = {(cuuint32_t)box_w, (cuuint32_t)box_h, 1u};
     const cuuint32_t estr[3] = {1u, 1u, 1u};
     const CUresult r = h->encode(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<uint8_t*>(base), gdim, gstr, box, estr,
                                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
@@ -979,11 +1006,23 @@ int configure(sslpl_orb* h, int W, int H) {
     SSLPL_CUDA(cudaMemset(h->ws.err, 0, sizeof(int)));
     h->octree_smem = h->g.sort_cap * 8;
     SSLPL_CUDA(cudaFuncSetAttribute(k_octree, cudaFuncAttributeMaxDynamicSharedMemorySize, std::max(h->octree_smem, 1024)));
+    h->fast_smem = 0;
+    for (int l = 0; l < h->g.nlevels; l++) {
+        const LevelGeom& G = h->g.lv[l];
+        if (G.ncells == 0) continue;
+        SSLPL_REQUIRE(G.wCell < FAST_MAXC && G.hCell < FAST_MAXC && 15 + std::min(FAST_STRIP, G.nCols) * G.wCell + 6 <= FS_P,
+                      SSLPL_ERR_UNSUPPORTED, "internal: a FAST strip outgrows its staged box");
+        h->fast_smem = std::max(h->fast_smem, FAST_STRIP * fast_warp_smem(G.wCell, G.hCell));
+    }
+    SSLPL_CUDA(cudaFuncSetAttribute(k_fast<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, std::max(h->fast_smem, 1024)));
+    SSLPL_CUDA(cudaFuncSetAttribute(k_fast<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, std::max(h->fast_smem, 1024)));
     h->tma_levels_ok = h->encode != nullptr;
     memset(&h->tm, 0, sizeof(h->tm));
-    for (int l = 1; l < h->g.nlevels && h->tma_levels_ok; l++)
-        h->tma_levels_ok = encode_level_map(h, &h->tm.lvl[l], h->ws.pyr + h->g.lv[l].img_off, h->g.lv[l].w, h->g.lv[l].h, h->g.lv[l].pitch,
-                                            h->g.pyr_stride, h->p.max_batch);
+    for (int l = 1; l < h->g.nlevels && h->tma_levels_ok; l++) {
+        const LevelGeom& G = h->g.lv[l];
+        h->tma_levels_ok = encode_level_map(h, &h->tm.strip[l], h->ws.pyr + G.img_off, G.w, G.h, G.pitch, h->g.pyr_stride, h->p.max_batch, FS_P, FS_IH) &&
+                           encode_level_map(h, &h->tm.blur[l], h->ws.pyr + G.img_off, G.w, G.h, G.pitch, h->g.pyr_stride, h->p.max_batch, BLUR_P, BLUR_IH);
+    }
     if (h->tma_levels_ok) SSLPL_CUDA(cudaMemcpy(h->ws.tmaps, &h->tm, sizeof(h->tm), cudaMemcpyHostToDevice));
     h->tm0_base = nullptr;
     h->cur_w = W; h->cur_h = H;
@@ -999,20 +1038,25 @@ int run_pipeline(sslpl_orb* h, int B) {
     bool tma = h->use_tma && h->tma_levels_ok;
     if (tma && !(h->tm0_base == h->view.base && h->tm0_pitch == h->view.pitch && h->tm0_fs == h->view.frame_stride && h->tm0_frames >= B)) {
         // level 0 is the caller's buffer: (re-)encode its maps when the view moves
-        tma = encode_level_map(h, &h->tm.lvl[0], h->view.base, g.lv[0].w, g.lv[0].h, h->view.pitch, h->view.frame_stride, B);
+        const View& v = h->view;
+        tma = encode_level_map(h, &h->tm.strip[0], v.base, g.lv[0].w, g.lv[0].h, v.pitch, v.frame_stride, B, FS_P, FS_IH) &&
+              encode_level_map(h, &h->tm.blur[0], v.base, g.lv[0].w, g.lv[0].h, v.pitch, v.frame_stride, B, BLUR_P, BLUR_IH);
         if (tma) {
-            SSLPL_CUDA(cudaMemcpyAsync(h->ws.tmaps, &h->tm.lvl[0], sizeof(CUtensorMap), cudaMemcpyHostToDevice, st));
+            TMaps* d_tm = reinterpret_cast<TMaps*>(h->ws.tmaps);
+            SSLPL_CUDA(cudaMemcpyAsync(&d_tm->strip[0], &h->tm.strip[0], sizeof(CUtensorMap), cudaMemcpyHostToDevice, st));
+            SSLPL_CUDA(cudaMemcpyAsync(&d_tm->blur[0], &h->tm.blur[0], sizeof(CUtensorMap), cudaMemcpyHostToDevice, st));
             h->tm0_base = h->view.base; h->tm0_pitch = h->view.pitch; h->tm0_fs = h->view.frame_stride; h->tm0_frames = B;
         } else h->tm0_base = nullptr;
     }
     for (int l = 1; l < g.nlevels; l++)
         launch(h, k_resize, dim3((g.lv[l].w + 127) / 128, (g.lv[l].h + 7) / 8, B), dim3(32, 8), 0, g, h->ws, h->view, l);
     h->mark("pyramid");
-    if (g.total_cells > 0) launch(h, tma ? k_fast<true> : k_fast<false>, dim3(g.total_cells, B), 128, 0, g, h->ws, h->view, h->ws.tmaps);
+    const TMaps* d_tm = reinterpret_cast<const TMaps*>(h->ws.tmaps);
+    if (g.total_strips > 0) launch(h, tma ? k_fast<true> : k_fast<false>, dim3(g.total_strips, B), 32 * FAST_STRIP, h->fast_smem, g, h->ws, h->view, d_tm->strip);
     h->mark("fast");
     launch(h, k_octree, dim3(g.nlevels, B), 256, h->octree_smem, g, h->ws);
     h->mark("octree");
-    launch(h, tma ? k_blur<true> : k_blur<false>, dim3(g.total_tiles, B), 256, 0, g, h->ws, h->view, h->ws.tmaps);
+    launch(h, tma ? k_blur<true> : k_blur<false>, dim3(g.total_tiles, B), 256, 0, g, h->ws, h->view, d_tm->blur);
     h->mark("blur");
     launch(h, k_orient_desc, dim3((g.kp_total_cap + 7) / 8, B), 256, 0, g, h->ws, h->view);
     h->mark("orient_desc");
