@@ -656,6 +656,32 @@ int  sslpl_fuse_lines_batch_device(sslpl_matcher* m,
         const float* cam, const float* bounds, const float* scaleFactors, int nlevels, float logScaleFactor, float th,
         int32_t* d_best_idx, int32_t* d_best_dist);
 
+/* ---- Optimizer::PoseOptimization(Frame*, isCorner) (Optimizer.cc:666-1022) over frames resident in HBM, monocular, asynchronous on the
+   handle's stream; no caller-visible allocation.  The step after every Tracking matcher (Tracking.cc:1048, :1259, :1328, :2059-2090):
+   four rounds of 10 Levenberg-Marquardt iterations on the frame's 6-DoF pose, each from the input pose, with Huber kernels in rounds
+   0-2 and an inlier / outlier classification after each round.  One CTA per frame; the result of a frame depends on its own rows only.
+   Frame f: d_kps[f][cap] = mvKeysUn (x, y, octave read), d_n[f] (clamped to [0, cap]); d_fmp[f][cap] = mvpMapPoints as element indices
+   into d_mp[nmp][9] (the Fuse element table; Xw = columns 0..2), -1 or any index outside [0, nmp) = NULL.  Lines: d_lineeq[f][capl][3] =
+   mvKeyLineFunctions (sslpl_line_device_results), d_nl[f] (clamped to [0, capl]), d_fml[f][capl] = mvpMapLines as element indices into
+   d_mlpos[nml][6] (f64 mWorldPos, the table of sslpl_update_map_lines_batch_device); d_fml = NULL means no line edges,
+   Optimizer::PoseOptimization(Frame*) (Optimizer.cc:1024, Relocalization), and the other line pointers are not read.  d_Tcw[f][12] = mTcw
+   (3x4 row-major).  cam = {fx, fy, cx, cy} and invLevelSigma2[nlevels] = mvInvLevelSigma2 are HOST arrays, one camera for all frames.
+   Results: d_Tcw_out[f][12] (may alias d_Tcw) = the pose SetPose writes (Converter::toCvMat of the final SE3Quat, narrowed to float);
+   d_outlier[f][cap] / d_line_outlier[f][capl] = mvbOutlier / mvbLineOutlier, written only for features with an edge (other entries are
+   left alone, so a caller passes its current rows); d_ninlier[f] = the return value, nInitialCorrespondences - nBad.  With fewer than
+   3 correspondences the pose is copied, the edges' flags are written 0 and d_ninlier is 0.  A frame in which a feature with an edge has
+   an octave outside [0, nlevels) gets d_ninlier = -1, its pose copied and no flags (the reference indexes mvInvLevelSigma2 out of
+   bounds there).  Stereo edges (mvuRight >= 0) are not supported.  Needs nframes in [1, max_batch], cap <= max_features + 64, capl <=
+   max_lines + 64 (with lines) and nlevels in [1, SSLPL_MAX_LEVELS]; bad arguments return SSLPL_ERR_ARG and enqueue nothing.
+   Results are bitwise reproducible and independent of a frame's position in the batch; against g2o they agree to the tolerance DESIGN.md
+   ("Pose optimisation") states, not bit for bit. */
+int  sslpl_pose_optimization_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const int* d_n, int nframes, int cap,
+        const int32_t* d_fmp, int nmp, const float* d_mp,
+        const double* d_lineeq, const int* d_nl, int capl, const int32_t* d_fml, int nml, const double* d_mlpos,
+        const float* d_Tcw, const float* cam, const float* invLevelSigma2, int nlevels,
+        float* d_Tcw_out, uint8_t* d_outlier, uint8_t* d_line_outlier, int32_t* d_ninlier);
+
 /* =====================================================================================
  * (2) Line segments — replaces LineSegment::ExtractLineSegment (src/ExtractLineSegment.cpp:18-69)
  * ===================================================================================== */

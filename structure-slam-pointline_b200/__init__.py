@@ -660,6 +660,20 @@ class Matcher(_Handle, kind="matcher", lifecycle=("sync", "set_stream", "stream"
         _check(lib().sslpl_match_lines_kf_batch_device(self._h, d_ldesc, d_nl, nrows, capl, d_kfml, nml, npairs, d_pair, d_lmatch,
                                                        d_nlmatch))
 
+    def pose_optimization_batch_device(self, d_kps, d_n, nframes, cap, d_fmp, nmp, d_mp, d_lineeq, d_nl, capl, d_fml, nml, d_mlpos,
+                                       d_Tcw, cam, inv_level_sigma2, d_Tcw_out, d_outlier, d_line_outlier, d_ninlier):
+        """Optimizer::PoseOptimization (Optimizer.cc:666-1022, monocular) for nframes frames in HBM (see
+        sslpl_pose_optimization_batch_device).  Raw device pointers: d_kps [nframes, cap] sslpl_keypoint (mvKeysUn), d_n [nframes] i32,
+        d_fmp [nframes, cap] i32 element indices into d_mp [nmp, 9] f32 (-1 NULL); d_lineeq [nframes, capl, 3] f64, d_nl [nframes],
+        d_fml [nframes, capl] i32 element indices into d_mlpos [nml, 6] f64, or d_fml = 0 for no line edges; d_Tcw [nframes, 12] f32;
+        host cam = fx fy cx cy and inv_level_sigma2 (nlevels = len) -> d_Tcw_out [nframes, 12] f32 (may be d_Tcw), d_outlier
+        [nframes, cap] / d_line_outlier [nframes, capl] u8 (written where a feature has an edge), d_ninlier [nframes] i32 (-1: an octave
+        outside the pyramid).  Asynchronous on the matcher's stream."""
+        isg = _f32(inv_level_sigma2)
+        _check(lib().sslpl_pose_optimization_batch_device(
+            self._h, d_kps, d_n, nframes, cap, d_fmp, nmp, d_mp or None, d_lineeq or None, d_nl or None, capl, d_fml or None, nml,
+            d_mlpos or None, d_Tcw, _p(_f32(cam)[:4].copy()), _p(isg), len(isg), d_Tcw_out, d_outlier, d_line_outlier or None, d_ninlier))
+
     def debug_predict_scale(self, ratio, log_scale_factor, nlevels, clamp=True):
         """MapPoint / MapLine::PredictScale on the device for host ratios (see sslpl_matcher_debug_predict_scale) -> int32 levels."""
         r = _f32(ratio).reshape(-1)

@@ -8,6 +8,7 @@
 #include "common.cuh"
 #include "../../include/sslpl_map.h"
 #include "svd4.cuh"
+#include "pose.cuh"
 #include <algorithm>
 #include <climits>
 #include <cmath>
@@ -3876,6 +3877,38 @@ int sslpl_match_lines_kf_batch_device(sslpl_matcher* m,
     SSLPL_CUDA(cudaMemsetAsync(d_nlmatch, 0, sizeof(int32_t) * npairs, m->stream));
     launch(m, k_line_ratio<true>, dim3((capl + 127) / 128, npairs), 128, 0, m->b_knn, (long long)lc * 4, d_nl, 0, capl, nullptr, 0, d_lmatch,
            capl, d_nlmatch, pmap, nrows, d_kfml, nml);
+    SSLPL_CUDA(cudaGetLastError());
+    return SSLPL_OK;
+}
+
+// Optimizer::PoseOptimization over frames in HBM: k_pose_opt (pose.cuh), one CTA per frame.
+int sslpl_pose_optimization_batch_device(sslpl_matcher* m,
+        const sslpl_keypoint* d_kps, const int* d_n, int nframes, int cap,
+        const int32_t* d_fmp, int nmp, const float* d_mp,
+        const double* d_lineeq, const int* d_nl, int capl, const int32_t* d_fml, int nml, const double* d_mlpos,
+        const float* d_Tcw, const float* cam, const float* invLevelSigma2, int nlevels,
+        float* d_Tcw_out, uint8_t* d_outlier, uint8_t* d_line_outlier, int32_t* d_ninlier) {
+    SSLPL_REQUIRE(m && d_kps && d_n && d_fmp && d_Tcw && cam && invLevelSigma2 && d_Tcw_out && d_outlier && d_ninlier,
+                  SSLPL_ERR_ARG, "null argument");
+    SSLPL_REQUIRE(nframes >= 1 && nframes <= m->p.max_batch, SSLPL_ERR_ARG, "nframes outside [1, max_batch]");
+    SSLPL_REQUIRE(cap >= 1 && cap <= m->p.max_features + 64, SSLPL_ERR_ARG, "cap outside [1, max_features + 64]");
+    SSLPL_REQUIRE(nmp >= 0 && (nmp == 0 || d_mp), SSLPL_ERR_ARG, "nmp must be >= 0, with an element table when > 0");
+    SSLPL_REQUIRE(nlevels >= 1 && nlevels <= SSLPL_MAX_LEVELS, SSLPL_ERR_ARG, "nlevels outside [1, SSLPL_MAX_LEVELS]");
+    if (d_fml) {
+        SSLPL_REQUIRE(d_lineeq && d_nl && d_line_outlier, SSLPL_ERR_ARG, "null line argument");
+        SSLPL_REQUIRE(capl >= 1 && capl <= m->p.max_lines + 64, SSLPL_ERR_ARG, "capl outside [1, max_lines + 64]");
+        SSLPL_REQUIRE(nml >= 0 && (nml == 0 || d_mlpos), SSLPL_ERR_ARG, "nml must be >= 0, with a position table when > 0");
+    }
+    SSLPL_CUDA(cudaSetDevice(m->p.device));
+    PoseArgs A; memset(&A, 0, sizeof(A));
+    A.kps = reinterpret_cast<const float*>(d_kps); A.n = d_n; A.cap = cap;
+    A.fmp = d_fmp; A.nmp = nmp; A.mp = d_mp;
+    if (d_fml) { A.lineeq = d_lineeq; A.nl = d_nl; A.capl = capl; A.fml = d_fml; A.nml = nml; A.mlpos = d_mlpos; A.line_outlier = d_line_outlier; }
+    A.Tcw = d_Tcw; A.Tcw_out = d_Tcw_out; A.outlier = d_outlier; A.ninlier = d_ninlier;
+    A.fx = cam[0]; A.fy = cam[1]; A.cx = cam[2]; A.cy = cam[3];
+    A.nlevels = nlevels;
+    for (int l = 0; l < nlevels; l++) A.invs2[l] = invLevelSigma2[l];
+    launch(m, k_pose_opt, nframes, POSE_THREADS, 0, A);
     SSLPL_CUDA(cudaGetLastError());
     return SSLPL_OK;
 }
